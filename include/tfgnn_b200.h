@@ -78,7 +78,13 @@ enum {
 };
 enum {
   TFGNN_PREPARE_VALIDATE = 1u << 0,
-  TFGNN_PREPARE_TRANSPOSE = 1u << 1 /* key the CSR by SOURCE: the edge list of the backward pass (messages flow tgt->src) */
+  TFGNN_PREPARE_TRANSPOSE = 1u << 1, /* key the CSR by SOURCE: the edge list of the backward pass (messages flow tgt->src) */
+  /* Backward CSR of a target-range shard (tfgnn_b200_prepare_sharded only; takes precedence over TFGNN_PREPARE_TRANSPOSE):
+   * keeps the edges whose TARGET lies in [target_begin, target_begin + target_count), keys them by (type, global source)
+   * over all num_nodes_total sources (row_ptr has L*num_nodes_total+1 entries) and stores the LOCAL target id
+   * tgt - target_begin, ascending within each segment.  With target_begin = 0, target_count = num_nodes_total it is the
+   * TFGNN_PREPARE_TRANSPOSE batch. */
+  TFGNN_PREPARE_TRANSPOSE_OWNED = 1u << 2
 };
 
 TFGNN_API int tfgnn_b200_abi_version(void);
@@ -170,7 +176,13 @@ TFGNN_API int tfgnn_b200_rgcn_fwd_allgather(tfgnn_batch_t* batch, const float* h
  * out = saved forward output, grad_out = dL/dout [V,H]; writes grad_h [V,D] (may be NULL) and grad_W[l] [D,H].
  * Supported: sum/mean/sqrt_n aggregation, activation after aggregation, activations none/relu/tanh/leaky_relu/
  * elu/selu (derivative from the output) and gelu (pre-activation recomputed), source-only or source+target state input (W[l] = [D,H] or [2D,H],
- * TFGNN_FLAG_USE_TARGET_STATE); D and H multiples of 4. */
+ * TFGNN_FLAG_USE_TARGET_STATE); D and H multiples of 4.
+ * On a target-range shard (batch from tfgnn_b200_prepare_sharded over targets [lo, hi)), batch_t must be the same
+ * adjacency and range prepared with TFGNN_PREPARE_TRANSPOSE_OWNED.  h is then the full [num_nodes_total, D] table, out and
+ * grad_out have hi-lo rows, and the call writes THIS SHARD'S CONTRIBUTION: grad_h [num_nodes_total, D] (every row; rows no
+ * owned edge reads are zero; the target-state term lands on rows [lo, hi)) and grad_W[l].  The contributions of all shards
+ * sum to the unsharded gradients (a reduce-scatter of grad_h and an all-reduce of grad_W across the ranks).  Each shard's
+ * result is run-to-run reproducible (no atomics).  An empty shard writes zeros. */
 TFGNN_API int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, const float* h, int32_t D,
                         const float* const* W, int32_t H, uint32_t flags, int32_t aggregation,
                         int32_t activation, const float* out, const float* grad_out, float* grad_h,
@@ -190,7 +202,11 @@ TFGNN_API int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* batch, const float* h, int32_t 
  * tf.GradientTape, models/graph_task_model.py:338-365).  Recomputes the forward intermediates from h; batch_t is
  * the TFGNN_PREPARE_TRANSPOSE batch of the same adjacency lists.  Writes grad_h [V,H], grad_W[l] [H,H],
  * grad_gru_kernel [H,3H], grad_gru_recurrent_kernel [H,3H], grad_gru_bias [2,3H].
- * Supported: 0 hidden layers in the message MLPs, source state only, sum / mean / sqrt_n aggregation, H % 4 == 0. */
+ * Supported: 0 hidden layers in the message MLPs, source state only, sum / mean / sqrt_n aggregation, H % 4 == 0.
+ * On a target-range shard the pair (batch, batch_t) is as for tfgnn_b200_rgcn_bwd: h is the full [num_nodes_total, H]
+ * table, grad_out has hi-lo rows, the GRU reads its state from rows [lo, hi) of h, and the call writes this shard's
+ * contribution to grad_h [num_nodes_total, H] (GRU direct and recurrent terms on rows [lo, hi)), to grad_W and to the GRU
+ * gradients; the contributions of all shards sum to the unsharded gradients.  An empty shard writes zeros. */
 TFGNN_API int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, const float* h, int32_t D,
                         const float* const* W, int32_t H, uint32_t flags, int32_t aggregation,
                         const float* gru_kernel, const float* gru_recurrent_kernel, const float* gru_bias,

@@ -25,6 +25,7 @@ FLAG_NORMALIZE, FLAG_ACT_BEFORE_AGG, FLAG_USE_TARGET = 1, 2, 4
 PATH = {"auto": 0, "atomic": 1, "sorted": 2, "sorted_tc": 3, "fused_tc": 4}
 PREPARE_VALIDATE = 1
 PREPARE_TRANSPOSE = 2
+PREPARE_TRANSPOSE_OWNED = 4
 MAX_EDGE_TYPES = 32
 
 EXPORTED_SYMBOLS = (

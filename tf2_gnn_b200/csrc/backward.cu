@@ -9,6 +9,9 @@
 //   dh[u]   = sum_l sum_{(u,v) in A_l} dA_l[v]                (CSR reduce over the SOURCE-keyed CSR: no atomics)
 // Supported: 0 hidden layers, source or source+target state input, sum / mean / sqrt_n aggregation, activation after the
 // aggregation, every activation of the reference's table (gelu through a recomputed pre-activation).
+// On a target-range shard (DESIGN.md §6) everything but the dh reduce covers the owned rows only; the dh reduce runs over the
+// shard's TFGNN_PREPARE_TRANSPOSE_OWNED CSR (all global sources, local target ids), so each shard writes its contribution
+// to the full grad_h table and the contributions of all shards sum to the unsharded gradient.
 #include "layers.cuh"
 
 namespace tfgnn {
@@ -271,6 +274,21 @@ static int grid_cap(long long n) {
   return g < 1 ? 1 : (g > 132 * 32 ? 132 * 32 : g);
 }
 
+// (b, bt) of a backward call: the unsharded pair (bt = TFGNN_PREPARE_TRANSPOSE of the same graph) or a target-range shard
+// and its TFGNN_PREPARE_TRANSPOSE_OWNED batch over the same range.
+static int check_backward_pair(const tfgnn_batch* b, const tfgnn_batch* bt) {
+  const bool sharded = b->tgt_off != 0 || b->V_src != b->V;
+  TFGNN_REQUIRE(!b->owned_transpose, "the first batch of a backward call must be the forward (target-keyed) batch");
+  if (sharded)
+    TFGNN_REQUIRE(bt->owned_transpose && bt->own_begin == b->tgt_off && bt->own_count == b->V && bt->V == b->V_src &&
+                      bt->L == b->L,
+                  "a target-range shard needs its TFGNN_PREPARE_TRANSPOSE_OWNED batch over the same range");
+  else
+    TFGNN_REQUIRE(bt->V == b->V && bt->L == b->L && bt->V_src == b->V && (!bt->owned_transpose || bt->own_count == b->V),
+                  "forward and transposed batches must describe the same graph");
+  return 0;
+}
+
 }  // namespace tfgnn
 
 using namespace tfgnn;
@@ -282,26 +300,33 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   TFGNN_REQUIRE(b != nullptr && bt != nullptr, "batch / transposed batch is NULL");
   TFGNN_REQUIRE(D > 0 && H > 0, "D and H must be positive");
   TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), "unknown activation / aggregation code");
-  const long long V = b->V;
+  // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
+  const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
-  TFGNN_REQUIRE(bt->V == V && bt->L == L && b->V_src == V && bt->V_src == V,
-                "forward and transposed batches must describe the same (unsharded) graph");
+  {
+    const int rc = check_backward_pair(b, bt);
+    if (rc) return rc;
+  }
   if (flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION)
     return unsupported("rgcn_bwd: activation-before-aggregation is not built yet");
   const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // W_l is then [2D, H]: rows [0,D) source, [D,2D) target
   if (aggregation == TFGNN_AGG_MAX) return unsupported("rgcn_bwd: max aggregation is not built yet");
   if (D % 4 != 0 || H % 4 != 0) return unsupported("rgcn_bwd needs D and H to be multiples of 4");
-  if (V == 0) return 0;
-  TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
   TFGNN_REQUIRE(L == 0 || (W && grad_W), "weight / weight-gradient table is NULL");
   cudaStream_t st = (cudaStream_t)stream;
+  if (V == 0 || L == 0) {   // no owned rows (an empty shard) or no edge types: zero contribution
+    for (int l = 0; l < L && V == 0; ++l) {
+      TFGNN_REQUIRE(grad_W[l], "a weight-gradient pointer is NULL");
+      TFGNN_CUDA(cudaMemsetAsync(grad_W[l], 0, (size_t)(use_target ? 2 * D : D) * H * sizeof(float), st));
+    }
+    if (grad_h && Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
+    return 0;
+  }
+  TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
+  const float* h_tgt = h + (size_t)lo * D;   // rows of the owned targets (target-state input)
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
   const int LD = L * D;
   const int K = use_target ? 2 * LD : LD;
-  if (L == 0) {
-    if (grad_h) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)V * D * sizeof(float), st));
-    return 0;
-  }
   PtrTable wt{}, gwt{};
   for (int l = 0; l < L; ++l) {
     TFGNN_REQUIRE(W[l] && grad_W[l], "a weight pointer is NULL");
@@ -348,7 +373,7 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     rc = launch_edge_reduce(p, /*merged=*/false, st);
     if (rc) return rc;
     if (use_target) {
-      rc = launch_target_term(h, D, b->row_ptr, (int)V, L, D, normalize, (float*)A, K, LD, st);
+      rc = launch_target_term(h_tgt, D, b->row_ptr, (int)V, L, D, normalize, (float*)A, K, LD, st);
       if (rc) return rc;
     }
     dim3 grid((K + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
@@ -377,19 +402,20 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     scale_by_type_kernel<<<grid_cap(V * LD), 256, 0, st>>>((float*)A, K, V, L, D, b->row_ptr);
     TFGNN_LAUNCH_CHECK();
   }
-  // 4. dh[u] = sum over the edges LEAVING u (source-keyed CSR), all types merged
+  // 4. dh[u] = sum over the edges LEAVING u (source-keyed CSR), all types merged.  On a shard: Vs segments per type (every
+  // global source, rows without an owned edge get zeros), values = local target ids = rows of dA
   {
     EdgeReduceParams p;
     p.X = (const float*)A; p.ldx = K; p.x_type_stride = D;
     p.row_ptr = bt->row_ptr; p.src = bt->src_sorted;
     p.out = grad_h; p.ldo = D;
-    p.V = (int)V; p.L = L; p.C = D;
+    p.V = (int)Vs; p.L = L; p.C = D;
     rc = launch_edge_reduce(p, /*merged=*/true, st);
     if (rc) return rc;
   }
-  if (use_target) {   // 5. the target half: grad_h[v] += sum_l coeff(v,l) * dT_l[v]
+  if (use_target) {   // 5. the target half: grad_h[lo + v] += sum_l coeff(v,l) * dT_l[v]
     target_term_bwd_kernel<<<grid_cap(V * D), 256, 0, st>>>((const float*)A + LD, K, b->row_ptr, V, L, D, normalize,
-                                                            grad_h);
+                                                            grad_h + (size_t)lo * D);
     TFGNN_LAUNCH_CHECK();
   }
   return 0;
@@ -408,16 +434,35 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   TFGNN_REQUIRE(b != nullptr && bt != nullptr, "batch / transposed batch is NULL");
   TFGNN_REQUIRE(D == H, "GGNN needs node embedding dimension == hidden_dim (ggnn.py:30)");
   TFGNN_REQUIRE(valid_agg(aggregation), "unknown aggregation code");
-  const long long V = b->V;
+  // V = owned target rows, Vs = rows of h and grad_h; the GRU state of local row v is h[lo + v]
+  const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
+  {
+    const int rc = check_backward_pair(b, bt);
+    if (rc) return rc;
+  }
   if (flags & TFGNN_FLAG_USE_TARGET_STATE) return unsupported("ggnn_bwd: target-state input is not built yet");
   if (aggregation == TFGNN_AGG_MAX) return unsupported("ggnn_bwd: max aggregation is not built yet");
   if (H % 4 != 0) return unsupported("ggnn_bwd needs hidden_dim to be a multiple of 4");
-  if (V == 0) return 0;
-  TFGNN_REQUIRE(h && grad_out && grad_h, "NULL pointer");
-  TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
+  TFGNN_REQUIRE(grad_h, "NULL pointer");
   TFGNN_REQUIRE(grad_gru_kernel && grad_gru_recurrent_kernel && grad_gru_bias, "GRU gradient pointer is NULL");
+  TFGNN_REQUIRE(L == 0 || grad_W, "weight-gradient table is NULL");
   cudaStream_t st = (cudaStream_t)stream;
+  if (V == 0) {   // no owned rows (an empty shard): zero contribution
+    const size_t n3 = (size_t)H * 3 * H;
+    TFGNN_CUDA(cudaMemsetAsync(grad_gru_kernel, 0, n3 * sizeof(float), st));
+    TFGNN_CUDA(cudaMemsetAsync(grad_gru_recurrent_kernel, 0, n3 * sizeof(float), st));
+    TFGNN_CUDA(cudaMemsetAsync(grad_gru_bias, 0, (size_t)2 * 3 * H * sizeof(float), st));
+    for (int l = 0; l < L; ++l) {
+      TFGNN_REQUIRE(grad_W[l], "a weight-gradient pointer is NULL");
+      TFGNN_CUDA(cudaMemsetAsync(grad_W[l], 0, (size_t)D * H * sizeof(float), st));
+    }
+    if (Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
+    return 0;
+  }
+  TFGNN_REQUIRE(h && grad_out, "NULL pointer");
+  TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
+  const float* h_tgt = h + (size_t)lo * D;
   const int N3 = 3 * H;
   const int chunks = (int)((V + kTnChunk - 1) / kTnChunk);
   void *agg = nullptr, *gx = nullptr, *gh = nullptr, *dagg = nullptr, *wT = nullptr, *part = nullptr, *dhd = nullptr,
@@ -451,10 +496,10 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   e1.bias = gru_bias + N3;
   rc = node_gemm((const float*)agg, H, gru_kernel, N3, (float*)gx, N3, V, N3, H, e0, TFGNN_PATH_AUTO, b, 6, st);
   if (rc) return rc;
-  rc = node_gemm(h, D, gru_recurrent_kernel, N3, (float*)gh, N3, V, N3, H, e1, TFGNN_PATH_AUTO, b, 6, st);
+  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, N3, (float*)gh, N3, V, N3, H, e1, TFGNN_PATH_AUTO, b, 6, st);
   if (rc) return rc;
   // 2. gates
-  gru_gate_bwd_kernel<<<grid_cap(V * H), 256, 0, st>>>((float*)gx, (float*)gh, h, D, grad_out, V, H, (float*)dhd);
+  gru_gate_bwd_kernel<<<grid_cap(V * H), 256, 0, st>>>((float*)gx, (float*)gh, h_tgt, D, grad_out, V, H, (float*)dhd);
   TFGNN_LAUNCH_CHECK();
   // 3. bias gradients: rows 0 / 1 of gru_bias belong to gx / gh
   float* cpart = (float*)part + (size_t)chunks * H * N3;
@@ -470,7 +515,7 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     PtrTable gt{};
     gt.p[0] = which ? grad_gru_recurrent_kernel : grad_gru_kernel;
     dim3 grid((H + kTnTile - 1) / kTnTile, (N3 + kTnTile - 1) / kTnTile, chunks);
-    gemm_tn_partial_kernel<<<grid, 256, 0, st>>>(which ? h : (const float*)agg, which ? D : H,
+    gemm_tn_partial_kernel<<<grid, 256, 0, st>>>(which ? h_tgt : (const float*)agg, which ? D : H,
                                                  (const float*)(which ? gh : gx), N3, V, H, N3, (float*)part);
     TFGNN_LAUNCH_CHECK();
     reduce_partials_kernel<<<grid_cap((long long)H * N3), 256, 0, st>>>((const float*)part, chunks, 1, H, N3, gt);
@@ -490,8 +535,8 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   rc = tfgnn_b200_rgcn_bwd(b, bt, h, D, W, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION, aggregation, TFGNN_ACT_NONE,
                            (const float*)dagg, (const float*)dagg, grad_h, grad_W, stream);
   if (rc) return rc;
-  // 7. grad_h += dh_direct + dh_rec
-  add3_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_h, (const float*)dhd, (const float*)tmp, V * H);
+  // 7. grad_h[lo + v] += dh_direct + dh_rec
+  add3_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dhd, (const float*)tmp, V * H);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }

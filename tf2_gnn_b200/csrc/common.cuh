@@ -117,6 +117,10 @@ struct tfgnn_batch {
   long long V = 0;        // number of TARGET nodes owned by this batch (= rows of every layer output)
   long long V_src = 0;    // number of rows of the source node table (== V unless target-range sharded)
   long long tgt_off = 0;  // global id of local target 0 (target-range sharding, SURVEY.md §8e)
+  // TFGNN_PREPARE_TRANSPOSE_OWNED: segments are (type, global source) over V = V_src nodes, values are local target ids of
+  // the owned range [own_begin, own_begin + own_count)
+  bool owned_transpose = false;
+  long long own_begin = 0, own_count = 0;
   int L = 0;
   long long M_in = 0;     // edges handed in
   int device = 0;

@@ -8,8 +8,28 @@
 
 namespace tfgnn {
 
-// ---- 1. histogram of targets per (type, node) -------------------------------------------
-__global__ void count_targets_kernel(PtrTable adj, CountTable E, int V, int V_src, int off, int transpose,
+// How an edge (src, tgt) enters the CSR: segment key and stored value.
+enum CsrKind { kByTarget = 0, kBySource = 1, kBySourceOwned = 2 };
+// kByTarget:      key tgt - off, value src          (kept when tgt - off < V)
+// kBySource:      key src - off, value tgt          (TFGNN_PREPARE_TRANSPOSE: kept when src - off < V)
+// kBySourceOwned: key src,       value tgt - off    (TFGNN_PREPARE_TRANSPOSE_OWNED: kept when tgt - off < V_own; V = V_src)
+// Returns false for an edge this batch does not keep.  Both ids must already lie in [0, V_src).
+__device__ __forceinline__ bool csr_entry(int2 st, int V, int off, int V_own, int kind, int* key, int* value) {
+  if (kind == kBySourceOwned) {
+    const unsigned t = (unsigned)(st.y - off);
+    *key = st.x;
+    *value = (int)t;
+    return t < (unsigned)V_own;
+  }
+  if (kind == kBySource) { const int t0 = st.x; st.x = st.y; st.y = t0; }
+  const unsigned t = (unsigned)(st.y - off);
+  *key = (int)t;
+  *value = st.x;
+  return t < (unsigned)V;   // else: another shard's node
+}
+
+// ---- 1. histogram of edges per (type, key node) ------------------------------------------
+__global__ void count_targets_kernel(PtrTable adj, CountTable E, int V, int V_src, int off, int V_own, int kind,
                                      int* __restrict__ counts, int* __restrict__ invalid) {
   const int l = blockIdx.y;
   const long long n = E.n[l];
@@ -17,11 +37,10 @@ __global__ void count_targets_kernel(PtrTable adj, CountTable E, int V, int V_sr
   int bad = 0;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n;
        e += (long long)gridDim.x * blockDim.x) {
-    int2 st = __ldg(edges + e);
-    if (transpose) { const int t0 = st.x; st.x = st.y; st.y = t0; }     // CSR keyed by source (backward pass)
+    const int2 st = __ldg(edges + e);
     if ((unsigned)st.x < (unsigned)V_src && (unsigned)st.y < (unsigned)V_src) {
-      const unsigned t = (unsigned)(st.y - off);
-      if (t < (unsigned)V) atomicAdd(counts + (long long)l * V + t, 1);   // else: another shard's target
+      int key, value;
+      if (csr_entry(st, V, off, V_own, kind, &key, &value)) atomicAdd(counts + (long long)l * V + key, 1);
     } else {
       ++bad;
     }
@@ -108,20 +127,19 @@ __global__ void scan_apply_kernel(int* __restrict__ data, long long n, const int
 }
 
 // ---- 3. fill: sources into their (type,target) segment -------------------------------------
-__global__ void fill_sources_kernel(PtrTable adj, CountTable E, int V, int V_src, int off, int transpose,
+__global__ void fill_sources_kernel(PtrTable adj, CountTable E, int V, int V_src, int off, int V_own, int kind,
                                     int* __restrict__ cursor, int* __restrict__ src_sorted) {
   const int l = blockIdx.y;
   const long long n = E.n[l];
   const int2* __restrict__ edges = reinterpret_cast<const int2*>(adj.p[l]);
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n;
        e += (long long)gridDim.x * blockDim.x) {
-    int2 st = __ldg(edges + e);
-    if (transpose) { const int t0 = st.x; st.x = st.y; st.y = t0; }
+    const int2 st = __ldg(edges + e);
     if ((unsigned)st.x < (unsigned)V_src && (unsigned)st.y < (unsigned)V_src) {
-      const unsigned t = (unsigned)(st.y - off);
-      if (t < (unsigned)V) {
-        int pos = atomicAdd(cursor + (long long)l * V + t, 1);
-        src_sorted[pos] = st.x;
+      int key, value;
+      if (csr_entry(st, V, off, V_own, kind, &key, &value)) {
+        int pos = atomicAdd(cursor + (long long)l * V + key, 1);
+        src_sorted[pos] = value;
       }
     }
   }
@@ -258,16 +276,23 @@ static int prepare_impl(const int32_t* const* adj, const int64_t* num_edges, int
     M += num_edges[l];
     maxE = num_edges[l] > maxE ? num_edges[l] : maxE;
   }
+  const int kind = (prepare_flags & TFGNN_PREPARE_TRANSPOSE_OWNED) ? kBySourceOwned
+                   : (prepare_flags & TFGNN_PREPARE_TRANSPOSE)    ? kBySource
+                                                                  : kByTarget;
+  const long long V_own = V;                 // edges kept: target (kBySourceOwned) or key node in [tgt_begin, +V)
+  if (kind == kBySourceOwned) V = V_total;   // segments per type: every global source
   const long long S = (long long)L * V;  // number of segments
   TFGNN_REQUIRE(M < (1ll << 31) - 1 && S < (1ll << 31) - 1,
                 "batch too large for int32 CSR (shard it across GPUs)");
   cudaStream_t st = (cudaStream_t)stream;
-  const int transpose = (prepare_flags & TFGNN_PREPARE_TRANSPOSE) ? 1 : 0;
 
   tfgnn_batch* b = new tfgnn_batch();
   b->V = V;
   b->V_src = V_total;
-  b->tgt_off = tgt_begin;
+  b->tgt_off = kind == kBySourceOwned ? 0 : tgt_begin;
+  b->owned_transpose = kind == kBySourceOwned;
+  b->own_begin = tgt_begin;
+  b->own_count = V_own;
   b->L = L;
   b->M_in = M;
   int rc = 0;
@@ -303,8 +328,8 @@ static int prepare_impl(const int32_t* const* adj, const int64_t* num_edges, int
     if (bx > 132 * 16) bx = 132 * 16;
     if (bx < 1) bx = 1;
     dim3 grid(bx, L);
-    count_targets_kernel<<<grid, 256, 0, st>>>(pt, ct, (int)V, (int)V_total, (int)tgt_begin, transpose, b->row_ptr,
-                                               b->invalid_count);
+    count_targets_kernel<<<grid, 256, 0, st>>>(pt, ct, (int)V, (int)V_total, (int)tgt_begin, (int)V_own, kind,
+                                               b->row_ptr, b->invalid_count);
     g_launch_count.fetch_add(1);
     TRY_CUDA(cudaGetLastError());
   }
@@ -322,8 +347,8 @@ static int prepare_impl(const int32_t* const* adj, const int64_t* num_edges, int
     int bx = ceil_div(maxE, 256);
     if (bx > 132 * 16) bx = 132 * 16;
     dim3 grid(bx, L);
-    fill_sources_kernel<<<grid, 256, 0, st>>>(pt, ct, (int)V, (int)V_total, (int)tgt_begin, transpose, (int*)cursor,
-                                              b->src_sorted);
+    fill_sources_kernel<<<grid, 256, 0, st>>>(pt, ct, (int)V, (int)V_total, (int)tgt_begin, (int)V_own, kind,
+                                              (int*)cursor, b->src_sorted);
     g_launch_count.fetch_add(1);
     TRY_CUDA(cudaGetLastError());
     long long warps_needed = S;

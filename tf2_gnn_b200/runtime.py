@@ -68,10 +68,13 @@ class PreparedBatch:
     and shared by all layers (the adjacency is layer-invariant, gnn.py:278,301)."""
 
     def __init__(self, adjacency_lists: Sequence[torch.Tensor], num_nodes: int, validate: bool = False,
-                 target_range: Optional[Tuple[int, int]] = None, transpose: bool = False):
+                 target_range: Optional[Tuple[int, int]] = None, transpose: bool = False,
+                 transpose_owned: bool = False):
         """target_range=(lo, hi): this batch is one rank's target-range shard of a graph with `num_nodes`
         nodes (sharding.py case 2); layer outputs then have hi-lo rows and `node_embeddings` passed to the
-        layers must be the full [num_nodes, D] table."""
+        layers must be the full [num_nodes, D] table.
+        transpose / transpose_owned: the backward CSR (TFGNN_PREPARE_TRANSPOSE / TFGNN_PREPARE_TRANSPOSE_OWNED); use
+        transposed() rather than building one directly."""
         self.adjacency_lists = tuple(adjacency_lists)  # keep caller memory alive (atomic path reads it)
         self.num_source_nodes = int(num_nodes)
         self.target_range = (0, int(num_nodes)) if target_range is None else (int(target_range[0]), int(target_range[1]))
@@ -85,7 +88,8 @@ class PreparedBatch:
         counts = (c_int64 * max(self.num_edge_types, 1))(*self.num_edges)
         _ffi.check(_ffi.lib().tfgnn_b200_prepare_sharded(
             ptrs, counts, self.num_edge_types, self.num_source_nodes, self.target_range[0], self.num_nodes,
-            (_ffi.PREPARE_VALIDATE if validate else 0) | (_ffi.PREPARE_TRANSPOSE if transpose else 0),
+            (_ffi.PREPARE_VALIDATE if validate else 0) | (_ffi.PREPARE_TRANSPOSE if transpose else 0)
+            | (_ffi.PREPARE_TRANSPOSE_OWNED if transpose_owned else 0),
             byref(self._handle), stream_ptr()))
         self._transposed: Optional["PreparedBatch"] = None
         self._finalizer = weakref.finalize(self, PreparedBatch._free, self._handle.value)
@@ -103,11 +107,15 @@ class PreparedBatch:
         return self._handle
 
     def transposed(self) -> "PreparedBatch":
-        """The same edges keyed by SOURCE (built lazily, once): the CSR of the backward pass."""
+        """The same edges keyed by SOURCE (built lazily, once): the CSR of the backward pass.  On a target-range shard it
+        holds the edges into the owned targets, keyed by global source, with local target ids
+        (TFGNN_PREPARE_TRANSPOSE_OWNED); its csr() then has L * num_source_nodes segments."""
         if self._transposed is None:
             if self.target_range != (0, self.num_source_nodes):
-                raise NotImplementedError("backward through a target-range shard is not built yet")
-            self._transposed = PreparedBatch(self.adjacency_lists, self.num_source_nodes, transpose=True)
+                self._transposed = PreparedBatch(self.adjacency_lists, self.num_source_nodes,
+                                                 target_range=self.target_range, transpose_owned=True)
+            else:
+                self._transposed = PreparedBatch(self.adjacency_lists, self.num_source_nodes, transpose=True)
         return self._transposed
 
     def in_degree(self) -> torch.Tensor:

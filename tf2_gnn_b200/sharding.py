@@ -11,12 +11,17 @@ Two cases, both with host-side index bookkeeping only (numpy; bit-exact, tested 
    [lo_g, hi_g) and every edge whose target falls there (ids stay global); it needs h[src] for
    arbitrary sources, i.e. one all-gather of the node-state shards per layer
    (tfgnn_b200_prepare_sharded + torch.distributed.all_gather_into_tensor over NCCL/NVLink).
+   Training (DESIGN.md §6): gather_node_states is the differentiable all-gather, its backward the
+   reduce-scatter reduce_scatter_node_grads; regather_saved_tables() keeps only a rank's own rows of
+   every gathered table until backward.  Weight gradients come out partial per rank: sum them with
+   torch.distributed.all_reduce before the optimiser step.
 """
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
+import torch
 
 
 # ------------------------------------------------------------------------------------------------
@@ -139,6 +144,91 @@ def all_gather_node_states(h_local, bounds: Sequence[Tuple[int, int]], group=Non
     if all((hi - lo) == rows for lo, hi in bounds):
         return recv
     return torch.cat([recv[r * rows: r * rows + (hi - lo)] for r, (lo, hi) in enumerate(bounds)], dim=0)
+
+
+# ------------------------------------------------------------------------------------------------
+# 2a. training on target-range shards: reduce-scatter backward, re-gather instead of saving the table
+# ------------------------------------------------------------------------------------------------
+def reduce_scatter_node_grads(partial_full, bounds: Sequence[Tuple[int, int]], group=None):
+    """The adjoint of all_gather_node_states.  Every rank passes its partial gradient w.r.t. the full [V, D] table
+    (e.g. the grad_h a layer's backward writes on a shard); rank r gets the sum over ranks of rows [lo_r, hi_r),
+    [hi_r - lo_r, D].  Uneven and empty ranges are padded to padded_shard_rows like the all-gather."""
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    rank = dist.get_rank(group)
+    rows = padded_shard_rows(bounds)
+    D = int(partial_full.shape[1])
+    if all((hi - lo) == rows for lo, hi in bounds):
+        send = partial_full.contiguous()
+    else:
+        send = torch.zeros((world * rows, D), dtype=partial_full.dtype, device=partial_full.device)
+        for r, (lo, hi) in enumerate(bounds):
+            send[r * rows: r * rows + (hi - lo)] = partial_full[lo:hi]
+    recv = torch.empty((rows, D), dtype=partial_full.dtype, device=partial_full.device)
+    dist.reduce_scatter_tensor(recv, send, op=dist.ReduceOp.SUM, group=group)
+    lo, hi = bounds[rank]
+    return recv[: hi - lo]
+
+
+class _GatherNodeStates(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, h_local, bounds, group):
+        ctx.bounds, ctx.group = bounds, group
+        return all_gather_node_states(h_local.detach(), bounds, group)
+
+    @staticmethod
+    def backward(ctx, grad_full):
+        return reduce_scatter_node_grads(grad_full, ctx.bounds, ctx.group), None, None
+
+
+def gather_node_states(h_local, bounds: Sequence[Tuple[int, int]], group=None):
+    """Differentiable all_gather_node_states: the full [V, D] table from every rank's rows; its backward is
+    reduce_scatter_node_grads, so the gradient of h_local is the sum of every rank's gradient w.r.t. its rows.
+    Backward is collective: every rank must run it through the same chain of gathers.  The result remembers h_local,
+    so that regather_saved_tables() can save h_local in its place."""
+    bounds = tuple((int(lo), int(hi)) for lo, hi in bounds)
+    full = _GatherNodeStates.apply(h_local, bounds, group)
+    full._tfgnn_gathered_from = (h_local.detach(), bounds, group)
+    return full
+
+
+class _Regather:
+    """What regather_saved_tables() saves for a gathered table: the rank's own rows."""
+
+    def __init__(self, h_local, bounds, group):
+        self.h_local, self.bounds, self.group = h_local, bounds, group
+        self.version = h_local._version
+
+    def gather(self):
+        if self.h_local._version != self.version:
+            raise RuntimeError("a node-state shard saved for backward was modified in place before the re-gather")
+        return all_gather_node_states(self.h_local, self.bounds, self.group)
+
+
+class regather_saved_tables(torch.autograd.graph.saved_tensors_hooks):
+    """Context manager: while it is active, autograd saves a table made by gather_node_states as the rank's own rows
+    (h_local) and all-gathers it again when backward unpacks it.
+
+        with sharding.regather_saved_tables():
+            for layer in layers:
+                h_local = layer(MessagePassingInput(sharding.gather_node_states(h_local, bounds), adj), prepared=shard)
+        loss.backward()
+
+    A layer hook (e.g. the fused RGCN / GGNN backward) saves its input table; without this context every rank keeps
+    the full [V, D] table of every layer until backward, with it O(hi - lo) rows per layer, and a full table exists only
+    while its layer runs forward or backward.  Only the forward has to run inside the context.  The re-gather in
+    backward is a collective: it works because every rank runs the same chain of layers, so every rank unpacks the
+    saved tables in the same order.  Other saved tensors are kept as they are."""
+
+    def __init__(self):
+        super().__init__(self._pack, self._unpack)
+
+    def _pack(self, t):
+        src = getattr(t, "_tfgnn_gathered_from", None)
+        return t if src is None else _Regather(*src)
+
+    def _unpack(self, saved):
+        return saved.gather() if isinstance(saved, _Regather) else saved
 
 
 # ------------------------------------------------------------------------------------------------

@@ -7,6 +7,12 @@ Every rank builds the same seeded graph, owns one target range (tfgnn_b200_prepa
 lists), and runs `layers` RGCN layers with ONE all-gather of the node-state shards per layer
 (torch.distributed.all_gather_into_tensor, NCCL over NVLink).  Rank 0 also runs the unsharded layers and
 checks the gathered result against it, then prints one JSON line with per-layer times (max over ranks).
+
+With --train every step runs the layers forward AND backward (DESIGN.md §6): sharding.gather_node_states (all-gather
+forward, reduce-scatter backward) under sharding.regather_saved_tables() (a rank keeps only its own rows of each layer's
+input until backward), weight gradients summed with all_reduce.  Rank 0 checks the input and weight gradients against
+unsharded autograd on its own GPU; the JSON line reports ms per step (max over ranks) and each rank's peak
+torch.cuda.max_memory_allocated.
 """
 import argparse
 import json
@@ -31,6 +37,7 @@ def main():
     ap.add_argument("--hidden", type=int, default=256)
     ap.add_argument("--layers", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--train", action="store_true", help="forward + backward per step (gradient check on rank 0)")
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
@@ -56,6 +63,8 @@ def main():
         layers.append(layer)
     shard = PreparedBatch(adj_dev, V, target_range=(lo, hi))
     h_local0 = torch.from_numpy(h0[lo:hi]).cuda()
+    if args.train:
+        return train(args, rank, world, bounds, layers, adj_dev, shard, h0, h_local0)
 
     def forward_sharded():
         h_local = h_local0
@@ -90,6 +99,73 @@ def main():
                           "ms_per_forward_max_over_ranks": float(t.item()),
                           "edges_per_s": M * args.layers / (float(t.item()) * 1e-3),
                           "allgather_bytes_per_layer_per_rank": int(V * H * 4)}), flush=True)
+    dist.barrier()
+    dist.destroy_process_group()
+    if not ok:
+        raise SystemExit(1)
+
+
+def train(args, rank, world, bounds, layers, adj_dev, shard, h0, h_local0):
+    V, L, H = args.nodes, args.types, args.hidden
+    lo, hi = bounds[rank]
+    params = [v for layer in layers for v in layer.variables]
+    for v in params:
+        v.requires_grad_()
+    g_full = torch.from_numpy(np.random.default_rng(8).random((V, H), dtype=np.float32) * 2 - 1).cuda()
+    g_local = g_full[lo:hi].contiguous()
+
+    def step():
+        for v in params:
+            v.value.grad = None
+        x = h_local0.clone().requires_grad_()
+        with sharding.regather_saved_tables():
+            h_local = x
+            for layer in layers:
+                h_local = layer(MessagePassingInput(sharding.gather_node_states(h_local, bounds), adj_dev), prepared=shard)
+        h_local.backward(g_local)
+        for v in params:
+            dist.all_reduce(v.value.grad)     # weight gradients are partial per rank
+        return x.grad
+
+    step()
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    dist.barrier()
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    for _ in range(args.steps):
+        grad_local = step()
+    ev1.record()
+    torch.cuda.synchronize()
+    peak = torch.tensor([float(torch.cuda.max_memory_allocated())], device="cuda")
+    peaks = [torch.zeros_like(peak) for _ in range(world)]
+    dist.all_gather(peaks, peak)
+    t = torch.tensor([ev0.elapsed_time(ev1) / args.steps], device="cuda")
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    grad_h = sharding.all_gather_node_states(grad_local, bounds)
+    ok = True
+    if rank == 0:
+        sharded_w = [v.value.grad.clone() for v in params]
+        for v in params:
+            v.value.grad = None
+        full = PreparedBatch(adj_dev, V)
+        x = torch.from_numpy(h0).cuda().requires_grad_()
+        h = x
+        for layer in layers:
+            h = layer(MessagePassingInput(h, adj_dev), prepared=full)
+        h.backward(g_full)
+
+        def rel(a, b):
+            return float((a - b).abs().max() / b.abs().max().clamp(min=1e-30))
+
+        err_h = rel(grad_h, x.grad)
+        err_w = max(rel(a, v.value.grad) for a, v in zip(sharded_w, params))
+        ok = err_h <= 2e-5 and err_w <= 2e-5
+        print(json.dumps({"check": "target-range sharded RGCN training == unsharded autograd", "world_size": world,
+                          "nodes": V, "edges": L * args.edges_per_type, "hidden": H, "layers": args.layers,
+                          "max_rel_err_grad_h": err_h, "max_rel_err_grad_w": err_w, "ok": ok,
+                          "ms_per_step_max_over_ranks": float(t.item()),
+                          "max_memory_allocated_per_rank": [int(p.item()) for p in peaks]}), flush=True)
     dist.barrier()
     dist.destroy_process_group()
     if not ok:
