@@ -733,6 +733,133 @@ def test_rgcn_backward_with_target_state_input(V, D, H, L, E, agg, act, normaliz
         assert_states_close(var.grad.cpu().numpy(), w64.grad.numpy(), tol=2e-5)
 
 
+def _forward_backward_twice(layer, h, adjs, g, weights):
+    """Two independent forward + backward runs through the autograd hook; they must agree bit for bit.
+    Returns [out, grad_h, *grad_weights] as numpy arrays."""
+    from tf2_gnn_b200.layers import MessagePassingInput
+    adj_dev = tuple(torch.from_numpy(a).cuda() for a in adjs)
+    runs = []
+    for _ in range(2):
+        ht = torch.from_numpy(h).cuda().requires_grad_()
+        out = layer(MessagePassingInput(ht, adj_dev), training=True)
+        grads = torch.autograd.grad(out, [ht] + weights, torch.from_numpy(g).cuda())
+        runs.append([out.detach().cpu().numpy()] + [x.cpu().numpy() for x in grads])
+    for a, b in zip(*runs):
+        assert np.array_equal(a, b)
+    return runs[0]
+
+
+@pytest.mark.parametrize("V,D,H,L,E,agg,act,normalize,opts", [
+    (3000, 384, 64, 3, 15000, "sum", "tanh", True, {}),             # NV = 3 (D in 257..384), split-tile mode
+    (3000, 384, 320, 3, 15000, "mean", "elu", False, {}),
+    (9000, 448, 64, 3, 30000, "sqrt_n", "tanh", False, {}),         # NV = 4, 71 tiles: one CTA per tile
+    (9000, 448, 320, 3, 30000, "sum", "gelu", True, {}),
+    (20000, 512, 64, 3, 60000, "mean", "tanh", False, {}),          # D = 512: 2 stages, 7 gather slots per warp
+    (20000, 512, 320, 3, 60000, "sum", "elu", False, {}),
+    (3000, 64, 128, 7, 8000, "sum", "tanh", True, {}),              # several N passes: the ring at its 8-slot limit
+    (3000, 64, 512, 7, 8000, "mean", "gelu", False, {}),
+    (9000, 64, 512, 7, 20000, "sum", "tanh", False, {}),
+    (2000, 32, 64, 14, 3000, "sum", "tanh", True, {}),              # one N pass, 14 types on the tensor cores
+    (2000, 64, 16, 3, 8000, "sum", "tanh", False, {}),              # BN = 16, one pass
+    (2000, 64, 80, 3, 8000, "mean", "tanh", True, {}),              # BN = 16, 5 passes
+    (9000, 64, 112, 3, 30000, "sqrt_n", "elu", False, {}),          # BN = 16, 7 passes
+    (8191, 64, 64, 2, 24000, "sum", "tanh", False, {}),             # around the 8192-row chunks of the dW reduction
+    (8192, 64, 64, 2, 24000, "mean", "tanh", True, {}),
+    (8193, 64, 64, 2, 24000, "mean", "tanh", False, dict(hub=True)),
+    (16385, 64, 64, 2, 50000, "sum", "elu", False, {}),
+    (3000, 128, 128, 4, 12000, "sum", "tanh", True, dict(empty_type=2)),
+])
+def test_rgcn_backward_shape_limits(V, D, H, L, E, agg, act, normalize, opts):
+    """Fused-kernel instantiations and backward tilings at their limits: forward forced to fused_tc, backward through the
+    autograd hook, both against the float64 reference; two runs give the same bits.  Only activations with a continuous
+    derivative: with relu / leaky_relu / selu, a pre-activation within rounding of 0 takes the other derivative in fp32
+    and moves a whole gradient row by |grad_out| |W| (0.06 of a 6.5 scale measured at D = 512, H = 320), so the kinked
+    activations are checked by the exact-arithmetic tests of test_gpu_backward_scale.py instead."""
+    _need_gpu()
+    import reference64 as r64
+    from tf2_gnn_b200.layers import RGCN
+    rng = np.random.default_rng(V + D + H + L)
+    adjs = random_graph(rng, V, L, E, **opts)
+    p = RGCN.get_default_hyperparameters()
+    p.update(hidden_dim=H, aggregation_function=agg, message_activation_function=act, normalize_by_num_incoming=normalize,
+             b200_path="fused_tc")
+    h = rng.uniform(-1, 1, (V, D)).astype(np.float32)
+    Ws = [mo.glorot_uniform(rng, (D, H)) for _ in range(L)]
+    g = rng.uniform(-1, 1, (V, H)).astype(np.float32)
+    layer = make_layer("rgcn", p, D, L, {"edge_mlps": [[w] for w in Ws]})
+    weights = [v.value.requires_grad_() for v in layer.variables]
+    out, grad_h, *grad_W = _forward_backward_twice(layer, h, adjs, g, weights)
+    ref = r64.rgcn_layer(h, adjs, Ws, g, agg=agg, act=act, normalize=normalize)
+    assert_states_close(out, ref["out"].numpy())
+    assert_states_close(grad_h, ref["grad_h"].numpy(), tol=2e-5)
+    for l in range(L):
+        if opts.get("empty_type") == l:
+            assert np.all(grad_W[l] == 0.0)
+        else:
+            assert_states_close(grad_W[l], ref["grad_W"][l].numpy(), tol=2e-5)
+
+
+def test_rgcn_fused_refuses_eight_types_with_several_passes():
+    """L = 8 with H > 64 needs 9 ring slots: fused_tc raises instead of computing something else, and auto (which then
+    takes another path) still matches the float64 reference, gradients included."""
+    _need_gpu()
+    import reference64 as r64
+    from tf2_gnn_b200.layers import MessagePassingInput, RGCN
+    V, D, H, L = 3000, 64, 128, 8
+    rng = np.random.default_rng(88)
+    adjs = random_graph(rng, V, L, 6000)
+    h = rng.uniform(-1, 1, (V, D)).astype(np.float32)
+    Ws = [mo.glorot_uniform(rng, (D, H)) for _ in range(L)]
+    g = rng.uniform(-1, 1, (V, H)).astype(np.float32)
+    p = RGCN.get_default_hyperparameters()
+    p.update(hidden_dim=H, aggregation_function="sum", message_activation_function="tanh", normalize_by_num_incoming=False,
+             b200_path="fused_tc")
+    layer = make_layer("rgcn", p, D, L, {"edge_mlps": [[w] for w in Ws]})
+    with pytest.raises(NotImplementedError):
+        layer(MessagePassingInput(torch.from_numpy(h).cuda(), tuple(torch.from_numpy(a).cuda() for a in adjs)))
+    layer = make_layer("rgcn", dict(p, b200_path="auto"), D, L, {"edge_mlps": [[w] for w in Ws]})
+    weights = [v.value.requires_grad_() for v in layer.variables]
+    out, grad_h, *grad_W = _forward_backward_twice(layer, h, adjs, g, weights)
+    ref = r64.rgcn_layer(h, adjs, Ws, g, act="tanh")
+    assert_states_close(out, ref["out"].numpy())
+    assert_states_close(grad_h, ref["grad_h"].numpy(), tol=2e-5)
+    for l in range(L):
+        assert_states_close(grad_W[l], ref["grad_W"][l].numpy(), tol=2e-5)
+
+
+@pytest.mark.parametrize("H", [160, 320])
+def test_ggnn_backward_wide_gru_epilogue(H, monkeypatch):
+    """GGNN with more than 4 GRU N tiles (fused-GRU forward) against the float64 reference; two runs give the same bits."""
+    _need_gpu()
+    import reference64 as r64
+    from tf2_gnn_b200.layers import GGNN
+    monkeypatch.setenv("TFGNN_B200_GGNN_FUSED_GRU", "1")
+    V, L = 3000, 3
+    rng = np.random.default_rng(H)
+    adjs = random_graph(rng, V, L, 3 * V, hub=True, dups=True)
+    p = GGNN.get_default_hyperparameters()
+    p.update(hidden_dim=H, b200_path="fused_tc")
+    h = rng.uniform(-1, 1, (V, H)).astype(np.float32)
+    Ws = [mo.glorot_uniform(rng, (H, H)) for _ in range(L)]
+    K, U = mo.glorot_uniform(rng, (H, 3 * H)), mo.glorot_uniform(rng, (H, 3 * H))
+    b = rng.uniform(-0.2, 0.2, (2, 3 * H)).astype(np.float32)
+    g = rng.uniform(-1, 1, (V, H)).astype(np.float32)
+    layer = make_layer("ggnn", p, H, L, {"edge_mlps": [[w] for w in Ws], "gru_kernel": K, "gru_recurrent_kernel": U,
+                                         "gru_bias": b})
+    by_name = {v.name: v.value for v in layer.variables}
+    gru = [[t for n, t in by_name.items() if n.endswith(s)][0]
+           for s in ("gru_cell/kernel:0", "gru_cell/recurrent_kernel:0", "gru_cell/bias:0")]
+    weights = [t.requires_grad_() for t in [m.layers[0].value for m in layer._edge_type_mlps] + gru]
+    out, grad_h, *grads = _forward_backward_twice(layer, h, adjs, g, weights)
+    ref = r64.ggnn_layer(h, adjs, Ws, K, U, b, g, agg=p["aggregation_function"], normalize=p["normalize_by_num_incoming"])
+    assert_states_close(out, ref["out"].numpy())
+    assert_states_close(grad_h, ref["grad_h"].numpy(), tol=2e-5)
+    for l in range(L):
+        assert_states_close(grads[l], ref["grad_W"][l].numpy(), tol=2e-5)
+    for got, key in zip(grads[L:], ("grad_K", "grad_U", "grad_b")):
+        assert_states_close(got, ref[key].numpy(), tol=2e-5)
+
+
 # ------------------------------------------------------------------------------------------
 # Node-level dense and error behaviour
 # ------------------------------------------------------------------------------------------
@@ -769,6 +896,50 @@ def test_dense_fwd_tensor_core_3xtf32(V, K, N):
     ref = np.maximum(x.astype(np.float64) @ w.astype(np.float64), 0.0)
     # measured: 4e-7 (K=32) .. 3.2e-6 (K=1024): accumulate-truncation bias of the tensor core, see gemm_tc.cu
     assert_states_close(out.cpu().numpy(), ref, tol=5e-6)
+
+
+@pytest.mark.parametrize("N", [16, 32, 48, 64, 80, 96, 112, 128, 176, 384])
+def test_dense_fwd_tensor_core_3xtf32_tiles_and_tails(N):
+    """Every BN instantiation of the wgmma GEMM (N = 176: BN = 16, 11 column tiles), M tails around the 64-row consumer
+    halves and 128-row tiles, M = 33921 (every CTA runs several tiles, so the stage ring wraps inside a tile), and K from
+    one partial K block to 32 (K = 160: 5 K blocks over a 3- or 4-stage ring).  Integer inputs in [-8, 8] must come out
+    exact; random inputs within 1e-5 of (|x||w| + |b|) element by element."""
+    _need_gpu()
+    from tf2_gnn_b200 import _ffi
+    from tf2_gnn_b200.runtime import stream_ptr
+    lib = _ffi.lib()
+    rng = np.random.default_rng(N)
+    for M in (1, 63, 64, 65, 128, 129, 33921):
+        for K in (4, 36, 160, 1024):
+            for integer in (True, False):
+                if integer:
+                    x, w, bias = (rng.integers(-8, 9, s).astype(np.float32) for s in ((M, K), (K, N), (N,)))
+                else:
+                    x = rng.uniform(-1, 1, (M, K)).astype(np.float32)
+                    w = rng.uniform(-0.3, 0.3, (K, N)).astype(np.float32)
+                    bias = rng.uniform(-0.5, 0.5, N).astype(np.float32)
+                x64, w64 = x.astype(np.float64), w.astype(np.float64)
+                ref = x64 @ w64
+                bound = np.abs(x64) @ np.abs(w64)
+                xt, wt, bt = (torch.from_numpy(a).cuda() for a in (x, w, bias))
+                for with_bias in (False, True):
+                    out = torch.full((M, N), float("nan"), dtype=torch.float32, device="cuda")
+                    if with_bias:
+                        _ffi.check(lib.tfgnn_b200_dense_bias_fwd(xt.data_ptr(), wt.data_ptr(), bt.data_ptr(), out.data_ptr(),
+                                                                 M, K, N, 0, _ffi.PATH["sorted_tc"], stream_ptr()))
+                    else:
+                        _ffi.check(lib.tfgnn_b200_dense_fwd(xt.data_ptr(), wt.data_ptr(), out.data_ptr(), M, K, N, 0,
+                                                            _ffi.PATH["sorted_tc"], stream_ptr()))
+                    got = out.cpu().numpy().astype(np.float64)
+                    want = ref + bias.astype(np.float64) if with_bias else ref
+                    what = f"M={M} K={K} N={N} {'integer' if integer else 'random'} bias={with_bias}"
+                    if integer:
+                        assert np.array_equal(got, want), what
+                    else:
+                        bnd = bound + np.abs(bias.astype(np.float64)) if with_bias else bound
+                        excess = np.abs(got - want) - 1e-5 * bnd
+                        assert np.isfinite(got).all() and excess.max() <= 0.0, \
+                            f"{what}: worst |err| / (|x||w|) = {(np.abs(got - want) / bnd).max():.3e}"
 
 
 def test_unknown_names_raise_like_the_reference():
