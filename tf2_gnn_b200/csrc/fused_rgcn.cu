@@ -12,7 +12,8 @@
 // registers.  The gather of the next slots overlaps the MMAs of slot i, and the [V, L*D] intermediate never touches HBM.
 // The accumulators of a 64 x BN half tile take BN registers per thread, and with 17 warps a thread has 96 (five warps share
 // an SM quarter's register file), so a tile is at most 64 columns wide: wider layers take several N passes over the same
-// gathered ring slots (the ring then holds all L types of the tile).
+// gathered ring slots (the ring then holds all L types of the tile).  Layers with 64 < H <= 256 (H % 32 == 0) outside
+// split-tile mode take fused_rgcn_rows_kernel instead: 64-row tiles of all H columns in one pass (see there).
 //
 // Warp roles (544 threads):
 //   0-7: two consumer warpgroups (split, MMA, epilogue) | 8: TMA | 9-16: gather.
@@ -104,8 +105,10 @@ struct GatherIssue {
   int lane, gw, Q, ncalls;
   long long unit0, unit_step;
   int ctas, rank;
+  int tile_rows;         // rows per tile (128, or 64 in the row tiling)
   int rpw, row_off;      // rows of the tile owned by this warp, first row of this CTA's share of the tile
-  uint32_t buf_s;        // shared-window address of this warp's slot 0, + 16 * lane
+  int w_row0;            // first row of this warp inside that share
+  uint32_t buf_s;       // shared-window address of this warp's slot 0, + 16 * lane
   uint32_t row_bytes;
   int ic;                // call being issued
   int i_pos, i_end, in_blk, i_blk;
@@ -118,7 +121,7 @@ struct GatherIssue {
     const int u = n / L;
     l = n - u * L;
     const long long tile = (unit0 + (long long)u * unit_step) * ctas + rank;
-    v0 = (int)(tile * kFuBM) + row_off + gw * rpw;
+    v0 = (int)(tile * tile_rows) + row_off + w_row0;
     nr = V - v0;
     nr = nr < 0 ? 0 : (nr > rpw ? rpw : nr);
   }
@@ -197,17 +200,17 @@ __device__ __forceinline__ void cp_async_wait_oldest(int Q) {   // at most Q-1 g
   }
 }
 
+// Tile (rank + ctas * unit) has tile_rows rows, and a ring slot as many; this warp gathers rows
+// [row_off + w_row0, row_off + w_row0 + rpw) of it.
 // split != 0 (split-tile mode): this CTA gathers only rows [split_rank*64, split_rank*64 + 64) of every tile; the slot
 // is shared with the peer CTA of the cluster, whose slot_ready barrier gets a (cluster-scope release) arrival as well.
 template <int NV, int QT = 0, bool FULL = false>
 __device__ __forceinline__ void gather_warp_main(const FusedParams& p, int lane, int gw, int Q_in, uint8_t* bufs,
                                                  long long unit0, long long unit_step, long long total_units,
-                                                 int ctas, int rank, int ring_row0, uint64_t* slot_ready,
-                                                 uint64_t* slot_free, int split, int split_rank,
-                                                 uint32_t peer_slot_ready0) {
+                                                 int ctas, int rank, int tile_rows, int row_off, int w_row0, int rpw,
+                                                 int ring_row0, uint64_t* slot_ready, uint64_t* slot_free, int split,
+                                                 int split_rank, uint32_t peer_slot_ready0) {
   const int Q = QT > 0 ? QT : Q_in;
-  const int kRowsPerWarp = split ? kFuBM / 2 / kFuGatherWarps : kFuBM / kFuGatherWarps;
-  const int row_off = split ? split_rank * (kFuBM / 2) : 0;
   const int D = p.D, C4 = p.D >> 2, normalize = p.normalize;
   const bool no_store = p.debug_skip & 16;   // timing experiment: gathered rows are not written to the ring
   const int kFuSlots = p.num_slots;
@@ -219,7 +222,7 @@ __device__ __forceinline__ void gather_warp_main(const FusedParams& p, int lane,
   g.skip = p.debug_skip & 1; g.C4 = C4;
   g.lane = lane; g.gw = gw; g.Q = Q; g.ncalls = (int)(my_units * p.L);
   g.unit0 = unit0; g.unit_step = unit_step; g.ctas = ctas; g.rank = rank;
-  g.rpw = kRowsPerWarp; g.row_off = row_off;
+  g.tile_rows = tile_rows; g.rpw = rpw; g.row_off = row_off; g.w_row0 = w_row0;
   g.buf_s = ptx::smem_u32(bufs) + (uint32_t)lane * 16u;
   g.row_bytes = (uint32_t)p.D * 4;
   g.ic = 0; g.islot = 0; g.in_blk = 0; g.ibuf = g.buf_s;
@@ -249,7 +252,7 @@ __device__ __forceinline__ void gather_warp_main(const FusedParams& p, int lane,
     const int slot = cc % kFuSlots;
     if (split) ptx::mbar_wait_cluster(&slot_free[slot], ((cc / kFuSlots) & 1) ^ 1);   // the peer's reads are done too
     else ptx::mbar_wait_backoff(&slot_free[slot], ((cc / kFuSlots) & 1) ^ 1, p.sleep_long);
-    float* dst = ring + ((size_t)ring_row0 + (size_t)slot * kFuBM + (size_t)row_off + (size_t)gw * kRowsPerWarp) * D + 4 * lane;
+    float* dst = ring + ((size_t)ring_row0 + (size_t)slot * tile_rows + (size_t)row_off + (size_t)w_row0) * D + 4 * lane;
     int row = 0;
     int seg_begin = __shfl_sync(0xffffffffu, rp, 0);
     int seg_end = __shfl_sync(0xffffffffu, rp, 1);
@@ -306,7 +309,8 @@ __device__ __forceinline__ void gather_warp_main(const FusedParams& p, int lane,
 // Epilogue of one 64 x BN half tile (rows m0 + 64 cw + ..., columns n0 + ...) from the accumulator registers: row norm / bias /
 // activation, the fused LayerNorm (single N pass: the tile holds whole rows), stores.  Thread (warp w, lane) holds rows
 // 16 w + lane / 4 + {0, 8} and, of each 8-column group, columns 2 (lane % 4) + {0, 1}: a lane quad writes 32 contiguous bytes.
-template <int BN>
+// FOLDED: the caller has already added the correction accumulator into the main one (the same single addition).
+template <int BN, bool FOLDED = false>
 __device__ __forceinline__ void fused_epilogue(const FusedParams& p, const HalfTileAcc<BN>& c, long long m0, int n0, int cw,
                                                int t) {
   const int w = t >> 5, lane = t & 31, cq = 2 * (lane & 3);
@@ -317,7 +321,15 @@ __device__ __forceinline__ void fused_epilogue(const FusedParams& p, const HalfT
     const long long row = m0 + 64 * cw + 16 * w + (lane >> 2) + 8 * h;
     const bool row_ok = row < p.V;
     float v[BN / 4];
-    acc_row<BN>(c, h, v);
+    if (FOLDED) {
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        v[2 * i] = c.main[4 * i + 2 * h];
+        v[2 * i + 1] = c.main[4 * i + 2 * h + 1];
+      }
+    } else {
+      acc_row<BN>(c, h, v);
+    }
     if (p.epi.row_norm && row_ok) {
       const float inv_rn = 1.0f / fu_row_norm(p.epi, row);
 #pragma unroll
@@ -508,9 +520,12 @@ fused_rgcn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     // common case (ring depth 8, D a multiple of 128): depth and column predicate resolved at compile time - the gather
     // loop runs once per EDGE
     uint8_t* my_bufs = gbuf + (size_t)gw * p.gather_q * ((size_t)p.D * 4);
-#define TFGNN_FU_GATHER(QT, FULL)                                                                                      \
-    gather_warp_main<NV, QT, FULL>(p, lane, gw, p.gather_q, my_bufs, unit0, unit_step, total_units, 1, 0, ring_row0,     \
-                                   slot_ready, slot_free, split ? 1 : 0, (int)srank, peer_slot_ready0)
+    const int rpw = split ? kFuBM / 2 / kFuGatherWarps : kFuBM / kFuGatherWarps;
+    const int row_off = split ? (int)srank * (kFuBM / 2) : 0;
+#define TFGNN_FU_GATHER(QT, FULL)                                                                                     \
+    gather_warp_main<NV, QT, FULL>(p, lane, gw, p.gather_q, my_bufs, unit0, unit_step, total_units, 1, 0, kFuBM,       \
+                                   row_off, gw * rpw, rpw, ring_row0, slot_ready, slot_free, split ? 1 : 0, (int)srank, \
+                                   peer_slot_ready0)
     if (p.gather_q == kFuMaxQ && p.D == 128 * NV) TFGNN_FU_GATHER(kFuMaxQ, true);
     else TFGNN_FU_GATHER(0, false);
 #undef TFGNN_FU_GATHER
@@ -520,6 +535,168 @@ fused_rgcn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     __syncwarp();
     ptx::cluster_sync_all();   // remote arrivals target the peer's shared memory: leave together
   }
+}
+
+// ---- row tiling (64 < H <= 256, H % 32 == 0): a tile is 64 target rows x all H columns, contracted in ONE pass -----------
+// Both consumer warpgroups read the same 64 rows of A and own H / 2 = BN columns each (main + correction: BN registers per
+// thread, 128 at H = 256).  The registers come from setmaxnreg: the kernel launches at 128 per thread (512 threads) and the
+// TMA / gather warpgroups hand theirs to the consumers.  A ring slot (64 rows, one edge type) is released as soon as its
+// K blocks are consumed, so the gather runs up to a whole tile ahead of the MMAs.  The two CTAs of a cluster take
+// neighbouring tiles and walk the same (type, K block) sequence in lockstep: each producer loads half of every weight
+// stage (the tf32-hi rows from CTA 0, the correction rows from CTA 1) and multicasts it into both CTAs, so a weight tile
+// crosses L2 -> SM once per 128 target rows.  Gather and ring stay per CTA; with an odd tile count the last cluster's
+// second CTA runs every stage on an empty tile and stores nothing.  The K order of every output element (type, K block,
+// k8 step; main and correction added in the epilogue) is that of fused_rgcn_kernel, so both give the same bits.
+//
+// Warp roles (512 threads, warpgroup-aligned):
+//   0-7: two consumer warpgroups | 8: TMA | 9-15: gather (64 / 7 rows each: 9 or 10).
+constexpr int kRtBM = 64;
+constexpr int kRtATileBytes = kRtBM * kFuBK * 4;
+constexpr int kRtGatherWarps = 7;
+constexpr int kRtFirstGatherWarp = 9;
+constexpr int kRtThreads = 512;
+constexpr int kRtMaxH = 256;
+constexpr uint32_t kRtConsumerRegs = 184;   // + kRtOtherRegs = 256: the register file at 512 threads
+constexpr uint32_t kRtOtherRegs = 72;
+
+template <int NV, int BN>
+__global__ void __launch_bounds__(kRtThreads, 1)
+fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                       const FusedParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr int H = 2 * BN;
+  constexpr int w_tile_bytes = H * kFuBK * 4;     // one of the two weight halves (hi or correction), all H columns
+  constexpr int stage_bytes = 2 * kRtATileBytes + 2 * w_tile_bytes;
+  const int S = p.num_stages;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);
+  uint64_t* full = bars;                          // this CTA's A and both weight halves landed
+  uint64_t* empty = bars + S;                     // the MMAs of all four consumer warpgroups of the cluster retired
+  uint64_t* slot_ready = bars + 2 * S;
+  uint64_t* slot_free = bars + 2 * S + kFuMaxSlots;
+  uint8_t* gbuf = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(bars + 2 * S + 2 * kFuMaxSlots) + 127) & ~uintptr_t(127));   // [7 * Q] rows
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const uint32_t srank = ptx::cluster_ctarank();
+  // one unit = the cluster's pair of 64-row tiles; this CTA's tile is 2 unit + srank
+  const long long total_units = (p.m_tiles + 1) / 2;
+  const long long unit0 = blockIdx.x / 2, unit_step = gridDim.x / 2;
+  const int kSlots = p.num_slots;
+
+  if (threadIdx.x == 0) {
+    ptx::prefetch_tensormap(&map_a);
+    ptx::prefetch_tensormap(&map_b);
+    for (int s = 0; s < S; ++s) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 4);
+    }
+    for (int r = 0; r < kFuMaxSlots; ++r) {
+      ptx::mbar_init(&slot_ready[r], kRtGatherWarps);
+      ptx::mbar_init(&slot_free[r], 2);
+    }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+  ptx::cluster_sync_all();   // both CTAs' barriers exist before any multicast or remote arrive can land on them
+  const int ring_row0 = blockIdx.x * kSlots * kRtBM;
+
+  if (wg >= 2) {
+    ptx::setmaxnreg_dec<kRtOtherRegs>();
+    if (warp == 8) {
+      // ================= TMA producer =================
+      if (lane == 0) {
+        uint32_t it = 0, slot_it = 0;
+        const uint64_t pol_keep = ptx::policy_evict_last();   // ring slots and the weights stay in L2
+        for (long long unit = unit0; unit < total_units; unit += unit_step, slot_it += p.L) {
+          for (int l = 0; l < p.L; ++l) {
+            const uint32_t sq = slot_it + l;
+            const int slot = sq % kSlots;
+            ptx::mbar_wait_backoff(&slot_ready[slot], (sq / kSlots) & 1, p.sleep_long);
+            for (int kb = 0; kb < p.kb_per_type; ++kb, ++it) {
+              const int s = it % S;
+              const uint32_t ph = (it / S) & 1;
+              // both CTAs' copies of the stage are free (the multicast below writes into the peer's as well)
+              ptx::mbar_wait_cluster(&empty[s], ph ^ 1);
+              uint8_t* st = smem + (size_t)s * stage_bytes;
+              ptx::mbar_arrive_expect_tx(&full[s], kRtATileBytes + 2 * w_tile_bytes);
+              ptx::tma_load_2d_hint(st, &map_a, &full[s], kb * kFuBK, ring_row0 + slot * kRtBM, pol_keep);
+              const int kcol = (l * p.kb_per_type + kb) * kFuBK;
+              ptx::tma_load_2d_multicast_hint(st + 2 * kRtATileBytes + (int)srank * w_tile_bytes, &map_b, &full[s], kcol,
+                                              (int)srank * H, (uint16_t)0x3, pol_keep);
+            }
+          }
+        }
+      }
+    } else {
+      // ================= gather warps =================
+      const int gw = warp - kRtFirstGatherWarp;
+      const int w_row0 = kRtBM * gw / kRtGatherWarps, rpw = kRtBM * (gw + 1) / kRtGatherWarps - w_row0;
+      uint8_t* my_bufs = gbuf + (size_t)gw * p.gather_q * ((size_t)p.D * 4);
+#define TFGNN_RT_GATHER(QT, FULL)                                                                                      \
+      gather_warp_main<NV, QT, FULL>(p, lane, gw, p.gather_q, my_bufs, unit0, unit_step, total_units, 2, (int)srank,   \
+                                     kRtBM, 0, w_row0, rpw, ring_row0, slot_ready, slot_free, 0, 0, 0u)
+      if (p.gather_q == kFuMaxQ && p.D == 128 * NV) TFGNN_RT_GATHER(kFuMaxQ, true);
+      else TFGNN_RT_GATHER(0, false);
+#undef TFGNN_RT_GATHER
+    }
+  } else {
+    // ================= consumers: warpgroup cw -> columns [cw BN, cw BN + BN) of the tile's 64 rows =================
+    ptx::setmaxnreg_inc<kRtConsumerRegs>();
+    const int cw = wg, t = threadIdx.x & 127;
+    const uint32_t empty0_cta0 = ptx::mapa_shared(ptx::smem_u32(&empty[0]), 0u);
+    const uint32_t empty0_cta1 = ptx::mapa_shared(ptx::smem_u32(&empty[0]), 1u);
+    auto release_stage = [&](int s) {   // one arrival per consumer warpgroup on the stage's barrier in BOTH CTAs
+      if (t == 0) {
+        ptx::mbar_arrive_cluster_release(empty0_cta0 + (uint32_t)s * 8u);
+        ptx::mbar_arrive_cluster_release(empty0_cta1 + (uint32_t)s * 8u);
+      }
+    };
+    HalfTileAcc<BN> c;
+    uint32_t it = 0, slot_base_it = 0;
+    for (long long unit = unit0; unit < total_units; unit += unit_step, slot_base_it += p.L) {
+      bool first = true;
+      for (int l = 0; l < p.L; ++l) {
+        const int slot = (slot_base_it + l) % kSlots;
+        for (int kb = 0; kb < p.kb_per_type; ++kb, ++it) {
+          const int s = it % S;
+          const uint32_t ph = (it / S) & 1;
+          ptx::mbar_wait_backoff(&full[s], ph, p.sleep_crit);
+          // the last K block of the slot has landed: its lines are dead.  This warpgroup discards half of the rows from L2
+          // (never written back to HBM), and the slot goes back to the gather warps.
+          const bool slot_done = kb == p.kb_per_type - 1;
+          if (slot_done && p.discard_ring) {
+            const char* sb = reinterpret_cast<const char*>(
+                p.ring + ((size_t)ring_row0 + (size_t)slot * kRtBM + (size_t)cw * (kRtBM / 2)) * p.D);
+            const int lines = kRtBM / 2 * p.D * 4 / 128;
+            for (int i = t; i < lines; i += 128) ptx::discard_l2_128(sb + (size_t)i * 128);
+          }
+          const uint32_t st = ptx::smem_u32(smem + (size_t)s * stage_bytes);
+          split_a_half<128, kRtBM>(st, cw, t, p.corr_bf16);   // each warpgroup splits 32 of the 64 shared rows
+          ptx::fence_proxy_async_smem();
+          ptx::warpgroup_pair_sync(1);                        // ... and both halves are split before either MMA reads them
+          if (slot_done && t == 0) ptx::mbar_arrive(&slot_free[slot]);
+          const uint32_t w = st + 2 * kRtATileBytes + (uint32_t)(cw * BN * 128);
+          ptx::wgmma_fence();
+          mma_kblock_at<BN, 128>(c, st, st + kRtATileBytes, w, w + w_tile_bytes, p.corr_bf16, first);
+          ptx::wgmma_commit();
+          // The stage goes back to both producers as soon as its MMAs retire, before the next stage is waited for: with
+          // two 80 KB stages, holding it one more block (wait_group 1) would leave a single stage load in flight.
+          ptx::wgmma_wait<0>();
+          release_stage(s);
+          first = false;
+        }
+      }
+      fence_acc<BN>(c);
+      // main + correction first: the correction registers are free for the epilogue
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) c.main[j] += c.corr[j];
+      // rows past V (the idle CTA of the last cluster: all of them) are not stored
+      fused_epilogue<BN, true>(p, c, (2 * unit + srank) * kRtBM, cw * BN, 0, t);
+    }
+  }
+  __syncwarp();
+  ptx::cluster_sync_all();   // multicasts and remote arrivals target the peer's shared memory: leave together
 }
 
 // ---- host side -------------------------------------------------------------------------------
@@ -629,13 +806,15 @@ void restore_l2_persist_carveout() {
 }
 
 constexpr int kFuMaxGrid = 160;
-static int fused_num_slots(int L, bool multi_pass) {
+// Row tiling: 3 slots of 64 rows by default (26 MB of ring at D = 256 on 132 SMs).  On cfg2 (H100 SXM, 400 W) 3 slots ran
+// the layer in 12.05 ms and 4 slots in 12.96 ms: the smaller ring leaves more of L2 to the weights and the source rows.
+static int fused_num_slots(int L, bool multi_pass, bool rows = false) {
   static const int env_slots = [] { const char* e = getenv("TFGNN_B200_RING_SLOTS"); return e ? atoi(e) : 0; }();
   if (multi_pass) return L + 1;
-  return (env_slots >= 2 && env_slots <= kFuMaxSlots) ? env_slots : 4;
+  return (env_slots >= 2 && env_slots <= kFuMaxSlots) ? env_slots : rows ? 3 : 4;
 }
 size_t fused_rgcn_ring_bytes(int D, int L, int H) {
-  (void)H;   // covers every tiling (single or several N passes, split-tile mode)
+  (void)H;   // covers every tiling (single or several N passes, split-tile mode; the row tiling's 64-row slots need half)
   int slots = fused_num_slots(L, false);
   if (L + 1 <= kFuMaxSlots && L + 1 > slots) slots = L + 1;
   return (size_t)kFuMaxGrid * slots * kFuBM * D * sizeof(float);
@@ -661,6 +840,54 @@ static cudaError_t launch_fused_nv(cudaLaunchConfig_t& cfg, const CUtensorMap& m
     case 32: return launch_fused_nv_bn<NV, 32>(cfg, map_a, map_b, p);
     case 48: return launch_fused_nv_bn<NV, 48>(cfg, map_a, map_b, p);
     default: return launch_fused_nv_bn<NV, 64>(cfg, map_a, map_b, p);
+  }
+}
+
+// Row tiling: clusters of 2 CTAs, each a whole SM; the grid is sized to the clusters that can be resident at once (the
+// kernel is persistent: a cluster that has to wait for a free SM pair would run its tiles after everybody else's).
+template <int NV, int BN>
+static cudaError_t launch_fused_rows_nv_bn(cudaLaunchConfig_t& cfg, const CUtensorMap& map_a, const CUtensorMap& map_b,
+                                           const FusedParams& p, long long units, int max_clusters) {
+  static std::mutex mu;
+  static cudaError_t attr_err = cudaSuccess;
+  static bool attr_set = false;
+  static size_t occ_smem = 0;
+  static int occ_clusters = 0;
+  int clusters = 0;
+  {
+    std::lock_guard<std::mutex> lock(mu);
+    if (!attr_set) {
+      attr_err = cudaFuncSetAttribute(fused_rgcn_rows_kernel<NV, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kFuSmemLimit);
+      attr_set = true;
+    }
+    if (attr_err != cudaSuccess) return attr_err;
+    if (occ_smem != cfg.dynamicSmemBytes) {
+      cfg.gridDim = dim3(2u * (unsigned)max_clusters);
+      int n = 0;
+      cudaError_t e = cudaOccupancyMaxActiveClusters(&n, fused_rgcn_rows_kernel<NV, BN>, &cfg);
+      if (e != cudaSuccess) return e;
+      if (n < 1) return cudaErrorInvalidConfiguration;
+      occ_smem = cfg.dynamicSmemBytes;
+      occ_clusters = n;
+    }
+    clusters = std::min(occ_clusters, max_clusters);
+  }
+  if (units < clusters) clusters = (int)units;
+  cfg.gridDim = dim3(2u * (unsigned)clusters);
+  return cudaLaunchKernelEx(&cfg, fused_rgcn_rows_kernel<NV, BN>, map_a, map_b, p);
+}
+
+template <int NV>
+static cudaError_t launch_fused_rows_nv(cudaLaunchConfig_t& cfg, const CUtensorMap& map_a, const CUtensorMap& map_b,
+                                        const FusedParams& p, long long units, int max_clusters) {
+  switch (p.block_n) {
+    case 48: return launch_fused_rows_nv_bn<NV, 48>(cfg, map_a, map_b, p, units, max_clusters);
+    case 64: return launch_fused_rows_nv_bn<NV, 64>(cfg, map_a, map_b, p, units, max_clusters);
+    case 80: return launch_fused_rows_nv_bn<NV, 80>(cfg, map_a, map_b, p, units, max_clusters);
+    case 96: return launch_fused_rows_nv_bn<NV, 96>(cfg, map_a, map_b, p, units, max_clusters);
+    case 112: return launch_fused_rows_nv_bn<NV, 112>(cfg, map_a, map_b, p, units, max_clusters);
+    default: return launch_fused_rows_nv_bn<NV, 128>(cfg, map_a, map_b, p, units, max_clusters);
   }
 }
 
@@ -698,11 +925,16 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
   const int split_env = split_str ? atoi(split_str) : 1;
   const bool split = !want_ln && split_env != 0 && 2 * p.m_tiles <= sms && H % 32 == 0 &&
                      (fused_block_n(H / 2) == H / 2 || L + 1 <= kFuMaxSlots);
+  // Row tiling (fused_rgcn_rows_kernel): 64 x H tiles in one N pass, for the full-size launch of the layers wider than one
+  // 64-column tile up to H = 256.  Split-tile mode, the fused LayerNorm (H <= 64) and H > 256 keep fused_rgcn_kernel.
+  const bool rows = !split && !want_ln && H > kFuMaxBN && H <= kRtMaxH && H % 32 == 0;
   p.split = split ? 1 : 0;
   p.cta_n = split ? H / 2 : H;
-  p.block_n = fused_block_n(p.cta_n);
-  p.n_tiles = p.cta_n / p.block_n;                      // N passes (per CTA)
-  p.num_slots = fused_num_slots(L, p.n_tiles > 1);
+  p.block_n = rows ? H / 2 : fused_block_n(p.cta_n);   // row tiling: the columns of one consumer warpgroup
+  p.n_tiles = rows ? 1 : p.cta_n / p.block_n;          // N passes (per CTA)
+  p.num_slots = fused_num_slots(L, p.n_tiles > 1, rows);
+  const int tile_rows = rows ? kRtBM : kFuBM;
+  if (rows) p.m_tiles = ((long long)V + kRtBM - 1) / kRtBM;
   p.C = out; p.ldc = ldo; p.epi = epi;
   {
     const char* sc = getenv("TFGNN_B200_SLEEP_CRIT");
@@ -710,17 +942,21 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
     p.sleep_crit = sc ? (uint32_t)atoi(sc) : 0u;
     p.sleep_long = sl ? (uint32_t)atoi(sl) : 0u;
   }
-  const int grid = split ? (int)(2 * p.m_tiles < (sms & ~1) ? 2 * p.m_tiles : (sms & ~1)) : (int)(p.m_tiles < sms ? p.m_tiles : sms);
-  // shared memory: S pipeline stages + Q row slots for each of the 8 gather warps.  The gather gets its Q rows in flight
-  // first (8 per warp: as many bytes in flight as 16 warps x 4); the pipeline gets what is left (2..4 stages).
+  // row tiling: the largest grid (the launch may shrink it to the co-resident clusters); it sizes the ring's tensor map
+  const int grid = rows ? (sms & ~1)
+                 : split ? (int)(2 * p.m_tiles < (sms & ~1) ? 2 * p.m_tiles : (sms & ~1)) : (int)(p.m_tiles < sms ? p.m_tiles : sms);
+  // shared memory: S pipeline stages + Q row slots for each gather warp.  The gather gets its Q rows in flight first (8 per
+  // warp: as many bytes in flight as 16 warps x 4); the pipeline gets what is left (2..4 stages).
   static const int stage_env = [] { const char* e = getenv("TFGNN_B200_FUSED_STAGES"); return e ? atoi(e) : 0; }();
   const char* q_str = getenv("TFGNN_B200_GATHER_Q");   // read per call: the tests sweep it
   const int q_env = q_str ? atoi(q_str) : 0;
   const int fixed_bytes = 2048 + 128 + 1024;   // barriers, alignment slack
   const int row_bytes = D * 4;
   const int want_q = q_env >= 1 && q_env <= kFuMaxQ ? q_env : kFuMaxQ;
-  const int stage_bytes = 2 * kFuATileBytes + 2 * p.block_n * kFuBK * 4;
-  auto q_for = [&](int s_) { return (kFuSmemLimit - fixed_bytes - s_ * stage_bytes) / (kFuGatherWarps * row_bytes); };
+  const int gather_warps = rows ? kRtGatherWarps : kFuGatherWarps;
+  // row tiling: A and its correction operand (64 rows each) + the hi and correction rows of all H weight columns
+  const int stage_bytes = rows ? 2 * kRtATileBytes + 2 * H * kFuBK * 4 : 2 * kFuATileBytes + 2 * p.block_n * kFuBK * 4;
+  auto q_for = [&](int s_) { return (kFuSmemLimit - fixed_bytes - s_ * stage_bytes) / (gather_warps * row_bytes); };
   int stages = stage_env >= 2 ? stage_env : 4;
   while (stages > 2 && q_for(stages) < want_q) --stages;
   int q = q_for(stages);
@@ -734,9 +970,9 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
   const int Kp = L * D;
   CUtensorMap map_a, map_b;
   {
-    cuuint64_t dims[2] = {(cuuint64_t)D, (cuuint64_t)grid * p.num_slots * kFuBM};
+    cuuint64_t dims[2] = {(cuuint64_t)D, (cuuint64_t)grid * p.num_slots * tile_rows};
     cuuint64_t strides[1] = {(cuuint64_t)D * sizeof(float)};
-    cuuint32_t box[2] = {(cuuint32_t)kFuBK, (cuuint32_t)kFuBM};
+    cuuint32_t box[2] = {(cuuint32_t)kFuBK, (cuuint32_t)tile_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = encode(&map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ring, dims, strides, box, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -749,7 +985,8 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
   {
     cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)(2 * H)};
     cuuint64_t strides[1] = {(cuuint64_t)Kp * sizeof(float)};
-    cuuint32_t box[2] = {(cuuint32_t)kFuBK, (cuuint32_t)p.block_n};
+    // row tiling: one box is the hi (or the correction) half of the stage, all H rows
+    cuuint32_t box[2] = {(cuuint32_t)kFuBK, (cuuint32_t)(rows ? H : p.block_n)};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = encode(&map_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(packedB), dims, strides, box,
                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -760,28 +997,39 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
     }
   }
   const size_t smem_bytes = (size_t)stages * stage_bytes + (2 * stages + 2 * kFuMaxSlots) * sizeof(uint64_t) + 128 +
-                            (size_t)kFuGatherWarps * q * row_bytes + 1024;
+                            (size_t)gather_warps * q * row_bytes + 1024;
   TFGNN_REQUIRE(smem_bytes <= (size_t)kFuSmemLimit, "fused RGCN: shared memory budget exceeded");
   const int nv = (D + 127) / 128;
   // L2 set-aside for the evict_last (persisting) lines: the ring + the packed weights.  Without a carve-out
   // the evict_last hint is advisory only and the ring gets written back to HBM.
   {
-    const int rc_l2 = ensure_l2_persist_carveout((size_t)grid * p.num_slots * kFuBM * D * sizeof(float) +
+    const int rc_l2 = ensure_l2_persist_carveout((size_t)grid * p.num_slots * tile_rows * D * sizeof(float) +
                                                  (size_t)2 * H * L * D * sizeof(float));
     if (rc_l2) return rc_l2;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(kFuThreads);
+  cfg.blockDim = dim3(rows ? kRtThreads : kFuThreads);
   cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = split ? 2u : 1u;
+  attr[0].val.clusterDim.x = split || rows ? 2u : 1u;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  if (rows) {
+    const long long units = (p.m_tiles + 1) / 2;
+    switch (nv) {
+      case 1: TFGNN_CUDA(launch_fused_rows_nv<1>(cfg, map_a, map_b, p, units, grid / 2)); break;
+      case 2: TFGNN_CUDA(launch_fused_rows_nv<2>(cfg, map_a, map_b, p, units, grid / 2)); break;
+      case 3: TFGNN_CUDA(launch_fused_rows_nv<3>(cfg, map_a, map_b, p, units, grid / 2)); break;
+      default: TFGNN_CUDA(launch_fused_rows_nv<4>(cfg, map_a, map_b, p, units, grid / 2)); break;
+    }
+    TFGNN_LAUNCH_CHECK();
+    return 0;
+  }
   switch (nv) {
     case 1: TFGNN_CUDA(launch_fused_nv<1>(cfg, map_a, map_b, p)); break;
     case 2: TFGNN_CUDA(launch_fused_nv<2>(cfg, map_a, map_b, p)); break;

@@ -96,6 +96,24 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorM
       : "memory");
 }
 
+// The same tile written to the same shared-memory offset in every CTA of the cluster named in cta_mask; each destination
+// CTA's mbarrier at the offset of `bar` receives the complete_tx of its copy.
+__device__ __forceinline__ void tma_load_2d_multicast_hint(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0,
+                                                           int c1, uint16_t cta_mask, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+        "h"(cta_mask), "l"(policy)
+      : "memory");
+}
+
+// ---- register reallocation between warpgroups (every warp of the warpgroup executes it) ----
+template <uint32_t REGS>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <uint32_t REGS>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
+
 // ---- L2 eviction policies (keep the producer/consumer ring, stream everything else) ----
 __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t p;
@@ -142,6 +160,8 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 __device__ __forceinline__ void reg_fence(float& x) { asm volatile("" : "+f"(x)::"memory"); }
 // Barrier over the 128 threads of one warpgroup (id 1..15; 0 is __syncthreads).
 __device__ __forceinline__ void warpgroup_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// Barrier over the 256 threads of two warpgroups.
+__device__ __forceinline__ void warpgroup_pair_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
 
 // Shared-memory matrix descriptor of a K-major tile with 128-byte (ROW_BYTES = 128: 32 tf32 per row, 8-row groups 1024 B
 // apart) or 64-byte swizzle (ROW_BYTES = 64, groups 512 B apart): start[0,14) LBO[16,30) SBO[32,46) layout[62,64)
