@@ -229,6 +229,27 @@ TFGNN_API int tfgnn_b200_film_fwd(tfgnn_batch_t* batch, const float* h, int32_t 
                         int32_t aggregation, int32_t activation, int32_t path, float* out,
                         void* stream);
 
+/* Backward of tfgnn_b200_film_fwd (the reference differentiates with tf.GradientTape,
+ * models/graph_task_model.py:338-365) in the aggregate-then-transform form: no tensor has a per-edge dimension.
+ * batch_t is the SAME adjacency prepared with TFGNN_PREPARE_TRANSPOSE.  out = saved forward output, grad_out = dL/dout
+ * [V,H]; writes grad_h [V,D] (may be NULL), grad_W[l] [D,H] or [2D,H] (the edge-MLP kernels, mlp_weights) and grad_film[l]
+ * [D,2H] (the FiLM kernels, film_weights).
+ * Supported: 0 hidden layers in the edge MLPs and in the FiLM MLPs, sum/mean/sqrt_n aggregation, activation after
+ * aggregation, activations none/relu/tanh/leaky_relu/elu/selu (derivative from the output) and gelu (pre-activation
+ * recomputed), source-only or source+target state input (TFGNN_FLAG_USE_TARGET_STATE); D and H multiples of 4.  Anything
+ * else returns TFGNN_ERR_UNSUPPORTED.
+ * On a target-range shard (batch from tfgnn_b200_prepare_sharded over targets [lo, hi)), batch_t must be the same
+ * adjacency and range prepared with TFGNN_PREPARE_TRANSPOSE_OWNED.  h is then the full [num_nodes_total, D] table, out and
+ * grad_out have hi-lo rows, and the call writes THIS SHARD'S CONTRIBUTION: grad_h [num_nodes_total, D] (every row; the
+ * FiLM and target-state terms land on rows [lo, hi)), grad_W[l] and grad_film[l].  The contributions of all shards sum to
+ * the unsharded gradients.  Each shard's result is run-to-run reproducible (no atomics).  An empty shard, or a batch
+ * without edge types, writes zeros. */
+TFGNN_API int tfgnn_b200_film_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, const float* h, int32_t D,
+                        const float* const* mlp_weights, const float* const* film_weights, int32_t H,
+                        uint32_t flags, int32_t aggregation, int32_t activation, const float* out,
+                        const float* grad_out, float* grad_h, float* const* grad_W, float* const* grad_film,
+                        void* stream);
+
 /* RGAT (rgat.py:91-163): per-type projection W_l [D,H], attention a_l [K, 2H/K]; softmax over all
  * incoming edges of all types jointly, per head; activation after. */
 TFGNN_API int tfgnn_b200_rgat_fwd(tfgnn_batch_t* batch, const float* h, int32_t D, const float* const* W,

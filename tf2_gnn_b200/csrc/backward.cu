@@ -542,6 +542,214 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
 }
 
 // =====================================================================================================================
+// GNN-FiLM backward in the aggregate-then-transform form of tfgnn_b200_film_fwd (variants.cu, DESIGN.md §3).  Per target v
+// and type l, with c = c_{v,l}, s = 1/(c+eps) or 1, A_l = s sum_e h_u, T_l = c s h_v, [gamma_l | beta_l] = h_v F_l:
+//   Q_l = A_l W^s_l (+ T_l W^t_l),   Z = sum_l gamma_l * Q_l + c beta_l,   out = act(rn(v) Z)
+// and with dZ = dOut * act' * rn(v):
+//   dQ_l = dZ * gamma_l        (GEMM h_v Fgamma_l, epilogue mul = dZ)
+//   dgamma_l = dZ * Q_l        (GEMM [A_l | T_l] W_l, epilogue mul = dZ),   dbeta_l = c dZ
+//   dW_l = [A_l | T_l]^T dQ_l,   dF_l = h_v^T [dgamma_l | dbeta_l]          (TN, fixed 8192-row chunks)
+//   dA_l = s dQ_l W^s_l^T       -> grad_h[u] through the source-keyed CSR (all types merged, no atomics)
+//   grad_h[v] += [dgamma_l | dbeta_l] F_l^T (+ c s dQ_l W^t_l^T)            (owned rows)
+// Every per-type temporary is [V, D], [V, H] or [V, 2H]; only dA holds all types ([V, L*D], the forward's slot-2 table).
+// =====================================================================================================================
+namespace tfgnn {
+
+// dGB[v, H + c] = c_{v,l} * dZ[v, c]: the beta half of [dgamma_l | dbeta_l] (row_ptr_l = the CSR offsets of type l), next to
+// the gamma half so that one TN pass gives dF_l
+__global__ void film_beta_grad_kernel(const float* __restrict__ dz, const int* __restrict__ row_ptr_l, long long V, int H,
+                                      float* __restrict__ dgb) {
+  const long long total = V * H;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long v = i / H;
+    const int c = (int)(i - v * H);
+    dgb[v * 2 * H + H + c] = (float)(row_ptr_l[v + 1] - row_ptr_l[v]) * dz[i];
+  }
+}
+
+// acc += a
+__global__ void add_kernel(float* __restrict__ acc, const float* __restrict__ a, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    acc[i] += a[i];
+}
+
+}  // namespace tfgnn
+
+extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int32_t D,
+                                   const float* const* mlp_weights, const float* const* film_weights, int32_t H,
+                                   uint32_t flags, int32_t aggregation, int32_t activation, const float* out,
+                                   const float* grad_out, float* grad_h, float* const* grad_W, float* const* grad_film,
+                                   void* stream) {
+  // the configuration is judged from the scalar arguments alone, before any batch is read
+  TFGNN_REQUIRE(D > 0 && H > 0, "D and H must be positive");
+  TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), "unknown activation / aggregation code");
+  if (flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION)
+    return unsupported("film_bwd: activation-before-aggregation is not built yet");
+  if (aggregation == TFGNN_AGG_MAX) return unsupported("film_bwd: max aggregation is not built yet");
+  if (D % 4 != 0 || H % 4 != 0) return unsupported("film_bwd needs D and H to be multiples of 4");
+  TFGNN_REQUIRE(b != nullptr && bt != nullptr, "batch / transposed batch is NULL");
+  // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
+  const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
+  const int L = b->L;
+  {
+    const int rc = check_backward_pair(b, bt);
+    if (rc) return rc;
+  }
+  TFGNN_REQUIRE(L == 0 || (mlp_weights && film_weights && grad_W && grad_film), "weight / weight-gradient table is NULL");
+  const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // W_l is then [2D, H]: rows [0,D) source, [D,2D) target
+  const int KT = use_target ? 2 * D : D;                          // columns of [A_l | T_l], rows of W_l
+  for (int l = 0; l < L; ++l)
+    TFGNN_REQUIRE(mlp_weights[l] && film_weights[l] && grad_W[l] && grad_film[l], "a weight pointer is NULL");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (V == 0 || L == 0) {   // no owned rows (an empty shard) or no edge types: zero contribution
+    for (int l = 0; l < L; ++l) {
+      TFGNN_CUDA(cudaMemsetAsync(grad_W[l], 0, (size_t)KT * H * sizeof(float), st));
+      TFGNN_CUDA(cudaMemsetAsync(grad_film[l], 0, (size_t)D * 2 * H * sizeof(float), st));
+    }
+    if (grad_h && Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
+    return 0;
+  }
+  TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
+  const float* h_tgt = h + (size_t)lo * D;   // rows of the owned targets (FiLM parameters, target-state input)
+  const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
+  const int LD = L * D;
+  int rc = batch_enter(b, st);
+  if (rc) return rc;
+  rc = batch_enter(bt, st);
+  if (rc) return rc;
+  // 1a. gelu: act'(pre-activation).  The pre-activation is recomputed by the forward entry without activation BEFORE any
+  // other scratch pointer of this function is taken: the nested forward may re-grow (= free and re-allocate) slots 2, 3,
+  // 4, 6, 11 and 12, which would leave pointers taken earlier dangling.  Slot 10 is not among them.
+  if (activation == TFGNN_ACT_GELU) {
+    void* z = nullptr;
+    rc = batch_scratch(b, 10, (size_t)V * H * sizeof(float), &z);
+    if (rc) return rc;
+    rc = tfgnn_b200_film_fwd(b, h, D, mlp_weights, 0, film_weights, H, flags, aggregation, TFGNN_ACT_NONE,
+                             TFGNN_PATH_AUTO, (float*)z, stream);
+    if (rc) return rc;
+    out = (const float*)z;
+  }
+  void *dz = nullptr, *AT = nullptr, *dQ = nullptr, *dGB = nullptr, *part = nullptr;
+  void *dA = nullptr, *dHt = nullptr, *WT = nullptr, *FT = nullptr;
+  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &dz);
+  if (rc) return rc;
+  rc = batch_scratch(b, 4, (size_t)V * KT * sizeof(float), &AT);   // [A_l | T_l], later dT_l
+  if (rc) return rc;
+  rc = batch_scratch(b, 5, (size_t)V * H * sizeof(float), &dQ);
+  if (rc) return rc;
+  rc = batch_scratch(b, 11, (size_t)V * 2 * H * sizeof(float), &dGB);   // [dgamma_l | dbeta_l]
+  if (rc) return rc;
+  const int chunks = (int)((V + kTnChunk - 1) / kTnChunk);
+  rc = batch_scratch(b, 9, (size_t)chunks * D * 2 * H * sizeof(float), &part);   // KT * H <= D * 2H
+  if (rc) return rc;
+  if (grad_h) {
+    rc = batch_scratch(b, 2, (size_t)V * LD * sizeof(float), &dA);
+    if (rc) return rc;
+    rc = batch_scratch(b, 13, (size_t)V * D * sizeof(float), &dHt);   // target-side terms of grad_h, summed over types
+    if (rc) return rc;
+    rc = batch_scratch(b, 7, (size_t)H * KT * sizeof(float), &WT);
+    if (rc) return rc;
+    rc = batch_scratch(b, 3, (size_t)2 * H * D * sizeof(float), &FT);
+    if (rc) return rc;
+  }
+
+  // 1b. dZ = dOut * act'(out) * rn(v)
+  act_grad_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_out, out, V, H, activation, b->row_ptr, L,
+                                                   agg_row_norm(aggregation), (float*)dz);
+  TFGNN_LAUNCH_CHECK();
+  GemmEpilogue none, by_dz;
+  by_dz.mul = (const float*)dz;
+  by_dz.ldm = H;
+  for (int l = 0; l < L; ++l) {
+    const int* rp = b->row_ptr + (size_t)l * V;   // the V segments of type l
+    const float* Wl = mlp_weights[l];
+    const float* Fl = film_weights[l];
+    // 2. [A_l | T_l] (recomputed)
+    {
+      EdgeReduceParams p;
+      p.X = h; p.ldx = D; p.x_type_stride = 0;
+      p.row_ptr = rp; p.src = b->src_sorted;
+      p.out = (float*)AT; p.ldo = KT; p.out_type_stride = 0;
+      p.V = (int)V; p.L = 1; p.C = D; p.normalize = normalize;
+      rc = launch_edge_reduce(p, /*merged=*/false, st);
+      if (rc) return rc;
+      if (use_target) {
+        rc = launch_target_term(h_tgt, D, rp, (int)V, 1, D, normalize, (float*)AT, KT, D, st);
+        if (rc) return rc;
+      }
+    }
+    // 3. dQ_l = dZ * (h_v Fgamma_l);  dgamma_l = dZ * ([A_l | T_l] W_l);  dbeta_l = c dZ
+    rc = node_gemm(h_tgt, D, Fl, 2 * H, (float*)dQ, H, V, H, D, by_dz, TFGNN_PATH_AUTO, b, 6, st);
+    if (rc) return rc;
+    rc = node_gemm((const float*)AT, KT, Wl, H, (float*)dGB, 2 * H, V, H, KT, by_dz, TFGNN_PATH_AUTO, b, 6, st);
+    if (rc) return rc;
+    film_beta_grad_kernel<<<grid_cap(V * H), 256, 0, st>>>((const float*)dz, rp, V, H, (float*)dGB);
+    TFGNN_LAUNCH_CHECK();
+    // 4. dW_l = [A_l | T_l]^T dQ_l,  dF_l = h_v^T [dgamma_l | dbeta_l]
+    {
+      PtrTable gw{}, gf{};
+      gw.p[0] = grad_W[l];
+      gf.p[0] = grad_film[l];
+      dim3 gridw((KT + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
+      gemm_tn_partial_kernel<<<gridw, 256, 0, st>>>((const float*)AT, KT, (const float*)dQ, H, V, KT, H, (float*)part);
+      TFGNN_LAUNCH_CHECK();
+      reduce_partials_kernel<<<grid_cap((long long)KT * H), 256, 0, st>>>((const float*)part, chunks, 1, KT, H, gw);
+      TFGNN_LAUNCH_CHECK();
+      dim3 gridf((D + kTnTile - 1) / kTnTile, (2 * H + kTnTile - 1) / kTnTile, chunks);
+      gemm_tn_partial_kernel<<<gridf, 256, 0, st>>>(h_tgt, D, (const float*)dGB, 2 * H, V, D, 2 * H, (float*)part);
+      TFGNN_LAUNCH_CHECK();
+      reduce_partials_kernel<<<grid_cap((long long)D * 2 * H), 256, 0, st>>>((const float*)part, chunks, 1, D, 2 * H, gf);
+      TFGNN_LAUNCH_CHECK();
+    }
+    if (!grad_h) continue;
+    // 5. dA_l = dQ_l W^s_l^T into columns [l*D, (l+1)*D) of dA (scaled by s after the loop)
+    PtrTable wt{}, ft{};
+    wt.p[0] = Wl;
+    ft.p[0] = Fl;
+    pack_transposed_kernel<<<grid_cap((long long)KT * H), 256, 0, st>>>(wt, 1, KT, H, (float*)WT);   // [H, KT]
+    TFGNN_LAUNCH_CHECK();
+    rc = node_gemm((const float*)dQ, H, (const float*)WT, KT, (float*)dA + (size_t)l * D, LD, V, D, H, none,
+                   TFGNN_PATH_AUTO, b, 6, st);
+    if (rc) return rc;
+    // 6. target side: dHt (+)= [dgamma_l | dbeta_l] F_l^T (+ coeff(v,l) dQ_l W^t_l^T)
+    pack_transposed_kernel<<<grid_cap((long long)D * 2 * H), 256, 0, st>>>(ft, 1, D, 2 * H, (float*)FT);   // [2H, D]
+    TFGNN_LAUNCH_CHECK();
+    GemmEpilogue sum_types;
+    sum_types.accumulate = l > 0;
+    rc = node_gemm((const float*)dGB, 2 * H, (const float*)FT, D, (float*)dHt, D, V, D, 2 * H, sum_types, TFGNN_PATH_AUTO,
+                   b, 6, st);
+    if (rc) return rc;
+    if (use_target) {   // dT_l overwrites [A_l | T_l] (read for the last time by the dW_l pass above)
+      rc = node_gemm((const float*)dQ, H, (const float*)WT + D, KT, (float*)AT, KT, V, D, H, none, TFGNN_PATH_AUTO, b, 6,
+                     st);
+      if (rc) return rc;
+      target_term_bwd_kernel<<<grid_cap(V * D), 256, 0, st>>>((const float*)AT, KT, rp, V, 1, D, normalize, (float*)dHt);
+      TFGNN_LAUNCH_CHECK();
+    }
+  }
+  if (!grad_h) return 0;
+  if (normalize) {
+    scale_by_type_kernel<<<grid_cap(V * LD), 256, 0, st>>>((float*)dA, LD, V, L, D, b->row_ptr);
+    TFGNN_LAUNCH_CHECK();
+  }
+  // 7. grad_h[u] = sum over the edges LEAVING u (source-keyed CSR; on a shard its owned transpose over all Vs sources)
+  {
+    EdgeReduceParams p;
+    p.X = (const float*)dA; p.ldx = LD; p.x_type_stride = D;
+    p.row_ptr = bt->row_ptr; p.src = bt->src_sorted;
+    p.out = grad_h; p.ldo = D;
+    p.V = (int)Vs; p.L = L; p.C = D;
+    rc = launch_edge_reduce(p, /*merged=*/true, st);
+    if (rc) return rc;
+  }
+  // 8. grad_h[lo + v] += target-side terms
+  add_kernel<<<grid_cap(V * D), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dHt, V * D);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+// =====================================================================================================================
 // Node-level glue of GNN._internal_call under training (gnn.py:279-327): backward of the bias-free / biased Dense layers,
 // LayerNormalization, and the Philox dropout shared by forward and backward.  The reference gets all of these from
 // tf.GradientTape (models/graph_task_model.py:338-365).

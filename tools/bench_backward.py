@@ -1,6 +1,10 @@
 """Measurement of the backward pass (SURVEY.md §8f-1) at bench.py's workloads: forward and backward device time of one
-RGCN (or GGNN) layer through the autograd hook, CUDA events, inputs resident in HBM.
-  python tools/bench_backward.py [--workload cfg2] [--steps 10] [--warmup 3] [--shards N]
+RGCN, GGNN or GNN-FiLM layer through the autograd hook, CUDA events, inputs resident in HBM.
+  python tools/bench_backward.py [--workload cfg2] [--steps 10] [--warmup 3] [--shards N] [--film-literal]
+For GNN-FiLM the line also carries the device memory in use after the steps (the library's pool and torch's allocator keep
+their high-water marks, so this is the peak of the run, inputs included).
+With --film-literal: a reduced FiLM graph on which the literal per-edge path (layers/differentiable.py) fits, 250k nodes /
+6 x 666,667 edges / D = H = 320, with the fused and the literal training step alternated in one process.
 With --shards N: the per-rank compute of training on N target-range shards (DESIGN.md §6), on ONE GPU and without
 communication: for each shard, the build of its owned-transpose batch (TFGNN_PREPARE_TRANSPOSE_OWNED) and the backward of
 the layer on the shard from the full [V, D] table; one JSON line per workload.
@@ -17,6 +21,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
+from tf2_gnn_b200 import _ffi  # noqa: E402
 from tf2_gnn_b200.layers import MessagePassingInput, get_message_passing_class  # noqa: E402
 from tf2_gnn_b200.runtime import PreparedBatch  # noqa: E402
 
@@ -27,7 +32,11 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--shards", type=int, default=0, help="time the backward of each of N target-range shards")
+    ap.add_argument("--film-literal", action="store_true",
+                    help="fused vs literal GNN-FiLM training step on a reduced graph the literal path fits")
     args = ap.parse_args()
+    if args.film_literal:
+        return bench_film_literal(args)
     wl = bench.WORKLOADS[args.workload]
     V, H, L = wl["V"], wl["H"], len(wl["E"])
     h_np, adjs_np, w_np = bench.make_inputs(wl, seed=0)
@@ -67,12 +76,102 @@ def main():
             bwd_ms.append(e1.elapsed_time(e2))
     M = sum(wl["E"])
     alg_fwd = bench.algorithmic_bytes(kind, V, wl["E"], H, H, params)
-    print(json.dumps({
+    rec = {
         "workload": wl["desc"], "kind": kind, "forward_ms": float(np.median(fwd_ms)), "backward_ms": float(np.median(bwd_ms)),
         "edges_per_s_fwd_bwd": M / ((np.median(fwd_ms) + np.median(bwd_ms)) * 1e-3),
-        "forward_algorithmic_bytes": alg_fwd,
-        "note": "backward = recompute A (CSR reduce) + TN GEMM dW (fp32 FFMA) + tensor-core GEMM dA + source-keyed CSR "
-                "reduce dh; autograd hook overhead included; not tuned (two-kernel form, SIMT dW)"}), flush=True)
+        "forward_algorithmic_bytes": alg_fwd, "card": card(), "note": NOTES.get(kind, NOTES["rgcn"])}
+    if kind == "gnn_film":
+        rec["device_memory_used_GB"] = device_used_gb()
+    print(json.dumps(rec), flush=True)
+
+
+NOTES = {
+    "rgcn": "backward = recompute A (CSR reduce) + TN GEMM dW (fp32 FFMA) + tensor-core GEMM dA + source-keyed CSR reduce dh; "
+            "autograd hook overhead included; not tuned (two-kernel form, SIMT dW)",
+    "ggnn": "backward = recomputed GRU inputs + gate backward + TN GEMMs for the GRU kernels + the RGCN-style message backward; "
+            "autograd hook overhead included",
+    "gnn_film": "backward = per type: recompute [A_l | T_l] (CSR reduce), dQ_l and dgamma_l (tensor-core GEMMs with the dZ "
+                "multiply in the epilogue), dW_l and dF_l (TN GEMMs, fp32 FFMA), dA_l and the target-side terms "
+                "(tensor-core GEMMs); then one source-keyed CSR reduce for dh; autograd hook overhead included",
+}
+
+
+def card():
+    """Name of device 0 and its power limit (read-only query)."""
+    import subprocess
+    rec = {"name": torch.cuda.get_device_name(0)}
+    try:
+        q = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        rec["power_limit_W"] = float(q.stdout.strip().splitlines()[0])
+    except Exception as e:   # the number is then reported without its power limit
+        rec["power_limit_W"] = f"unavailable: {type(e).__name__}"
+    return rec
+
+
+def device_used_gb():
+    torch.cuda.synchronize()
+    free, total = torch.cuda.mem_get_info()
+    return (total - free) / 1e9
+
+
+def release_memory():
+    import gc
+    gc.collect()
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+    _ffi.lib().tfgnn_b200_release_device_state()
+
+
+def bench_film_literal(args):
+    """Fused (tfgnn_b200_film_bwd) vs literal (layers/differentiable.py) GNN-FiLM training step, alternated step by step."""
+    from tf2_gnn_b200.layers.differentiable import edge_mlp_family_forward
+    wl = dict(V=250_000, E=[666_667] * 6, H=320, kind="gnn_film", graph="er",
+              desc="GNN-FiLM reduced graph: 250k nodes / 4M edges / 6 edge types, D = H = 320 (class defaults)")
+    V, H, L = wl["V"], wl["H"], len(wl["E"])
+    h_np, adjs_np, _ = bench.make_inputs(wl, seed=0)
+    layer = get_message_passing_class("gnn_film")(dict(get_message_passing_class("gnn_film").get_default_hyperparameters(),
+                                                       hidden_dim=H))
+    torch.manual_seed(1)
+    layer.build(MessagePassingInput((None, H), tuple((None, 2) for _ in range(L))))
+    for v in layer.variables:
+        v.requires_grad_()
+    dev = torch.device("cuda", 0)
+    h = torch.from_numpy(h_np).to(dev).requires_grad_()
+    adj = tuple(torch.from_numpy(a).to(dev) for a in adjs_np)
+    g = torch.rand((V, H), device=dev) * 2 - 1
+    prepared = PreparedBatch(adj, V)
+    prepared.transposed()
+    film = [[v.value for v in m.layers] for m in layer._edge_type_film_layer_computations]
+    paths = {"fused": lambda: layer(MessagePassingInput(h, adj), prepared=prepared),
+             "literal": lambda: edge_mlp_family_forward(layer, h, prepared, film_kernels=film)}
+    ms = {k: ([], []) for k in paths}
+    mem = {k: 0.0 for k in paths}
+    for i in range(args.warmup + args.steps):
+        for name, fwd in paths.items():
+            release_memory()
+            e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            h.grad = None
+            for v in layer.variables:
+                v.value.grad = None
+            e0.record()
+            out = fwd()
+            e1.record()
+            out.backward(g)
+            e2.record()
+            torch.cuda.synchronize()
+            mem[name] = max(mem[name], device_used_gb())
+            del out
+            if i >= args.warmup:
+                ms[name][0].append(e0.elapsed_time(e1))
+                ms[name][1].append(e1.elapsed_time(e2))
+    print(json.dumps({
+        "workload": wl["desc"], "kind": "gnn_film", "steps": args.steps, "card": card(),
+        "paths": {k: {"forward_ms": float(np.median(f)), "backward_ms": float(np.median(b)),
+                      "device_memory_used_GB": mem[k]} for k, (f, b) in ms.items()},
+        "note": "alternated step by step in one process; memory = device memory in use after the step with the library's "
+                "pool and torch's allocator cache emptied before it (their high-water mark for that path, inputs included)"}),
+        flush=True)
 
 
 def _median_ms(fn, steps, warmup):
@@ -127,7 +226,7 @@ def bench_shards(args, wl, layer, h, adj, g):
     print(json.dumps({
         "workload": wl["desc"], "kind": wl["kind"], "shards": args.shards, "bounds": bounds,
         "owned_transpose_prepare_ms": prep_ms, "backward_ms": bwd_ms, "backward_ms_max": max(bwd_ms),
-        "backward_ms_sum": sum(bwd_ms), "prepare_ms_max": max(prep_ms),
+        "backward_ms_sum": sum(bwd_ms), "prepare_ms_max": max(prep_ms), "card": card(),
         "note": "one GPU, per-rank compute only: no all-gather / reduce-scatter / all-reduce; grad_h is the full [V, D] "
                 "table per shard"}), flush=True)
 
