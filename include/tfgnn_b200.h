@@ -138,6 +138,26 @@ TFGNN_API int tfgnn_b200_edge_mlp_fwd(tfgnn_batch_t* batch, const float* h, int3
                             uint32_t flags, int32_t aggregation, int32_t activation, int32_t path,
                             float* out, void* stream);
 
+/* Backward of tfgnn_b200_edge_mlp_fwd with ONE hidden layer (the class defaults of GNN_Edge_MLP and RGIN; the reference
+ * differentiates with tf.GradientTape, models/graph_task_model.py:338-365) in the hoisted form of the forward: no tensor has
+ * a per-edge dimension.  batch_t is the SAME adjacency prepared with TFGNN_PREPARE_TRANSPOSE.  mlp_weights = the L*2 tables
+ * of the forward (U_l [D_in, H], W2_l [H, H], type-major); out = saved forward output, grad_out = dL/dout [V,H]; writes
+ * grad_h [V,D] (may be NULL) and grad_weights, the L*2 gradients in the same order.  The hidden ReLU's derivative is
+ * [pre-activation > 0] (0 at 0, as TF's ReluGrad).
+ * Supported: num_hidden_layers 1, sum/mean/sqrt_n aggregation, activation after aggregation, every activation (gelu
+ * through a recomputed pre-activation), source-only or source+target state input (TFGNN_FLAG_USE_TARGET_STATE), D and H
+ * multiples of 4, H <= 512.  Anything else returns TFGNN_ERR_UNSUPPORTED (0 hidden layers: tfgnn_b200_rgcn_bwd).
+ * On a target-range shard (batch from tfgnn_b200_prepare_sharded over targets [lo, hi)), batch_t must be the same
+ * adjacency and range prepared with TFGNN_PREPARE_TRANSPOSE_OWNED.  h is then the full [num_nodes_total, D] table, out and
+ * grad_out have hi-lo rows, and the call writes THIS SHARD'S CONTRIBUTION: grad_h [num_nodes_total, D] (every row; the
+ * target-state terms land on rows [lo, hi)) and every weight gradient.  The contributions of all shards sum to the
+ * unsharded gradients.  Each shard's result is run-to-run reproducible (no atomics).  An empty shard, or a batch without
+ * edge types, writes zeros. */
+TFGNN_API int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, const float* h, int32_t D,
+                            const float* const* mlp_weights, int32_t num_hidden_layers, int32_t H, uint32_t flags,
+                            int32_t aggregation, int32_t activation, const float* out, const float* grad_out,
+                            float* grad_h, float* const* grad_weights, void* stream);
+
 /* RGCN convenience entry (rgcn.py:12-62): edge_mlp_fwd with 0 hidden layers, source state only. */
 TFGNN_API int tfgnn_b200_rgcn_fwd(tfgnn_batch_t* batch, const float* h, int32_t D, const float* const* W,
                         int32_t H, uint32_t flags, int32_t aggregation, int32_t activation,

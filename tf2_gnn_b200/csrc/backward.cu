@@ -750,6 +750,373 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
 }
 
 // =====================================================================================================================
+// Edge MLP with one hidden layer (GNN_Edge_MLP defaults, RGIN defaults) in the hoisted form of tfgnn_b200_edge_mlp_fwd
+// (api.cu, DESIGN.md §3).  Per edge e = (u -> v) of type l, with Xs = h [U^s_0 | ..], Xt = h_v [U^t_0 | ..] (target-state
+// input only, else 0), P_e = Xs_l[u] + Xt_l[v], m_e = [P_e > 0] (TF ReluGrad: the derivative at 0 is 0):
+//   A_l[v] = s_{v,l} sum_e relu(P_e),   out = act(rn(v) [A_0 | ..] [W2_0; ..])
+// and with dZ = dOut * act' * rn(v):
+//   dW2_l = A_l^T dZ                                   (A recomputed; TN, fixed 8192-row chunks)
+//   dA = dZ [W2_0; ..]^T, dA_l[v] *= s_{v,l}           (one [V, L*H] GEMM)
+//   dXs_l[u] = sum_{e leaving u, type l} dA_l[v] m_e   (source-keyed CSR, one warp per (type, source), no atomics)
+//   dXt_l[v] = dA_l[v] * cnt_l[v],  cnt_l[v, c] = sum_{e into v} m_e[c]   (counted in the recompute pass)
+//   dU^s_l = h^T dXs_l,  dU^t_l = h_v^T dXt_l          (TN)
+//   grad_h = dXs [U^s_0^T; ..] (+ dXt [U^t_0^T; ..] on the owned rows)
+// Every temporary is [V or Vs, L*H] at most; nothing has a per-edge dimension.
+// =====================================================================================================================
+namespace tfgnn {
+
+// A_l[v] and cnt_l[v] for target-state input: one warp per (type, target) segment.  The edge order per lane, the sum and
+// the end-of-segment scale are those of the forward's hidden_relu edge reduce, so A has the forward's bits.  All tables
+// have L*H columns.
+template <int NV>
+__global__ void __launch_bounds__(256) hidden_relu_count_kernel(const float* __restrict__ Xs, const float* __restrict__ Xt,
+                                                                const int* __restrict__ row_ptr, const int* __restrict__ src,
+                                                                int V, int L, int H, int normalize, float* __restrict__ A,
+                                                                float* __restrict__ cnt) {
+  const int lane = threadIdx.x & 31;
+  const long long ld = (long long)L * H;
+  const int C4 = H >> 2;
+  const long long items = (long long)L * V;
+  for (long long item = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; item < items;
+       item += ((long long)gridDim.x * blockDim.x) >> 5) {
+    const int l = (int)(item / V), v = (int)(item - (long long)l * V);
+    const int beg = __ldg(row_ptr + item), end = __ldg(row_ptr + item + 1);
+    const long long col = (long long)l * H;
+    float4 t[NV], acc[NV], n[NV];
+#pragma unroll
+    for (int j = 0; j < NV; ++j) {
+      const int c4 = lane + 32 * j;
+      t[j] = (c4 < C4 && end > beg) ? ldg_f4(Xt + v * ld + col + 4 * c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+      acc[j] = n[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    for (int base = beg; base < end; base += 32) {
+      const int m = min(32, end - base);
+      const int my_src = lane < m ? __ldg(src + base + lane) : 0;
+#pragma unroll 1   // unrolled, the three float4 accumulator sets spill at NV = 3, 4
+      for (int e = 0; e < m; ++e) {
+        const float* row = Xs + (long long)__shfl_sync(0xffffffffu, my_src, e) * ld + col;
+#pragma unroll
+        for (int j = 0; j < NV; ++j) {
+          const int c4 = lane + 32 * j;
+          if (c4 >= C4) continue;
+          const float4 r = ldg_f4(row + 4 * c4);
+          const float4 x = make_float4(r.x + t[j].x, r.y + t[j].y, r.z + t[j].z, r.w + t[j].w);
+          acc[j] = make_float4(acc[j].x + fmaxf(x.x, 0.f), acc[j].y + fmaxf(x.y, 0.f), acc[j].z + fmaxf(x.z, 0.f),
+                               acc[j].w + fmaxf(x.w, 0.f));
+          n[j] = make_float4(n[j].x + (x.x > 0.f ? 1.f : 0.f), n[j].y + (x.y > 0.f ? 1.f : 0.f),
+                             n[j].z + (x.z > 0.f ? 1.f : 0.f), n[j].w + (x.w > 0.f ? 1.f : 0.f));
+        }
+      }
+    }
+    const float s = normalize ? 1.0f / ((float)(end - beg) + kSmallNumber) : 1.0f;
+#pragma unroll
+    for (int j = 0; j < NV; ++j) {
+      const int c4 = lane + 32 * j;
+      if (c4 >= C4) continue;
+      float4 a = acc[j];
+      if (normalize) a = make_float4(a.x * s, a.y * s, a.z * s, a.w * s);
+      *reinterpret_cast<float4*>(A + v * ld + col + 4 * c4) = make_float4(0.f + a.x, 0.f + a.y, 0.f + a.z, 0.f + a.w);
+      *reinterpret_cast<float4*>(cnt + v * ld + col + 4 * c4) = n[j];
+    }
+  }
+}
+
+// dXs_l[u] = sum over the edges (u -> v) of type l of dA_l[v] * m_e, over the source-keyed CSR (row_ptr_t: segment
+// (l, u) = l*Vs + u; tgt: local target ids), in canonical order, one warp per segment.  Xs_l[u] stays in registers.
+// Without target-state input (TGT = false) m_e = [Xs_l[u] > 0] is the same for every edge of the segment: applied once.
+template <int NV, bool TGT>
+__global__ void __launch_bounds__(256) hidden_relu_src_bwd_kernel(const float* __restrict__ Xs, const float* __restrict__ Xt,
+                                                                  const float* __restrict__ dA,
+                                                                  const int* __restrict__ row_ptr_t,
+                                                                  const int* __restrict__ tgt, int Vs, int L, int H,
+                                                                  float* __restrict__ dXs) {
+  const int lane = threadIdx.x & 31;
+  const long long ld = (long long)L * H;
+  const int C4 = H >> 2;
+  const long long items = (long long)L * Vs;
+  for (long long item = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; item < items;
+       item += ((long long)gridDim.x * blockDim.x) >> 5) {
+    const int l = (int)(item / Vs), u = (int)(item - (long long)l * Vs);
+    const int beg = __ldg(row_ptr_t + item), end = __ldg(row_ptr_t + item + 1);
+    const long long col = (long long)l * H;
+    float4 xs[NV], acc[NV];
+#pragma unroll
+    for (int j = 0; j < NV; ++j) {
+      const int c4 = lane + 32 * j;
+      xs[j] = (c4 < C4 && end > beg) ? ldg_f4(Xs + u * ld + col + 4 * c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+      acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    for (int base = beg; base < end; base += 32) {
+      const int m = min(32, end - base);
+      const int my_tgt = lane < m ? __ldg(tgt + base + lane) : 0;
+#pragma unroll 4
+      for (int e = 0; e < m; ++e) {
+        const long long off = (long long)__shfl_sync(0xffffffffu, my_tgt, e) * ld + col;
+#pragma unroll
+        for (int j = 0; j < NV; ++j) {
+          const int c4 = lane + 32 * j;
+          if (c4 >= C4) continue;
+          const float4 g = ldg_f4(dA + off + 4 * c4);
+          if (TGT) {
+            const float4 t = ldg_f4(Xt + off + 4 * c4);
+            acc[j].x += (xs[j].x + t.x > 0.f) ? g.x : 0.f;
+            acc[j].y += (xs[j].y + t.y > 0.f) ? g.y : 0.f;
+            acc[j].z += (xs[j].z + t.z > 0.f) ? g.z : 0.f;
+            acc[j].w += (xs[j].w + t.w > 0.f) ? g.w : 0.f;
+          } else {
+            acc[j] = make_float4(acc[j].x + g.x, acc[j].y + g.y, acc[j].z + g.z, acc[j].w + g.w);
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < NV; ++j) {
+      const int c4 = lane + 32 * j;
+      if (c4 >= C4) continue;
+      float4 a = acc[j];
+      if (!TGT)
+        a = make_float4(xs[j].x > 0.f ? a.x : 0.f, xs[j].y > 0.f ? a.y : 0.f, xs[j].z > 0.f ? a.z : 0.f,
+                        xs[j].w > 0.f ? a.w : 0.f);
+      *reinterpret_cast<float4*>(dXs + u * ld + col + 4 * c4) = a;
+    }
+  }
+}
+
+// x *= y
+__global__ void mul_inplace_kernel(float* __restrict__ x, const float* __restrict__ y, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    x[i] *= y[i];
+}
+
+static int warp_grid(long long items) {
+  const long long g = (items * 32 + 255) / 256;
+  return g < 1 ? 1 : (g > 132 * 64 ? 132 * 64 : (int)g);
+}
+
+static int launch_hidden_relu_count(const float* Xs, const float* Xt, const int* row_ptr, const int* src, int V, int L,
+                                    int H, int normalize, float* A, float* cnt, cudaStream_t st) {
+  const int g = warp_grid((long long)L * V);
+  switch ((H + 127) / 128) {
+    case 1: hidden_relu_count_kernel<1><<<g, 256, 0, st>>>(Xs, Xt, row_ptr, src, V, L, H, normalize, A, cnt); break;
+    case 2: hidden_relu_count_kernel<2><<<g, 256, 0, st>>>(Xs, Xt, row_ptr, src, V, L, H, normalize, A, cnt); break;
+    case 3: hidden_relu_count_kernel<3><<<g, 256, 0, st>>>(Xs, Xt, row_ptr, src, V, L, H, normalize, A, cnt); break;
+    case 4: hidden_relu_count_kernel<4><<<g, 256, 0, st>>>(Xs, Xt, row_ptr, src, V, L, H, normalize, A, cnt); break;
+    default: return unsupported("edge_mlp_bwd: hidden width above 512 is not built");
+  }
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+static int launch_hidden_relu_src_bwd(const float* Xs, const float* Xt, const float* dA, const int* row_ptr_t,
+                                      const int* tgt, int Vs, int L, int H, float* dXs, cudaStream_t st) {
+  const int g = warp_grid((long long)L * Vs);
+#define TFGNN_SRC_BWD(NV)                                                                                            \
+  do {                                                                                                               \
+    if (Xt) hidden_relu_src_bwd_kernel<NV, true><<<g, 256, 0, st>>>(Xs, Xt, dA, row_ptr_t, tgt, Vs, L, H, dXs);    \
+    else hidden_relu_src_bwd_kernel<NV, false><<<g, 256, 0, st>>>(Xs, Xt, dA, row_ptr_t, tgt, Vs, L, H, dXs);      \
+  } while (0)
+  switch ((H + 127) / 128) {
+    case 1: TFGNN_SRC_BWD(1); break;
+    case 2: TFGNN_SRC_BWD(2); break;
+    case 3: TFGNN_SRC_BWD(3); break;
+    case 4: TFGNN_SRC_BWD(4); break;
+    default: return unsupported("edge_mlp_bwd: hidden width above 512 is not built");
+  }
+#undef TFGNN_SRC_BWD
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace tfgnn
+
+extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int32_t D,
+                                       const float* const* mlp_weights, int32_t num_hidden_layers, int32_t H,
+                                       uint32_t flags, int32_t aggregation, int32_t activation, const float* out,
+                                       const float* grad_out, float* grad_h, float* const* grad_weights, void* stream) {
+  // the configuration is judged from the scalar arguments alone, before any batch is read
+  TFGNN_REQUIRE(D > 0 && H > 0, "D and H must be positive");
+  TFGNN_REQUIRE(num_hidden_layers >= 0, "num_hidden_layers must be >= 0");
+  TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), "unknown activation / aggregation code");
+  if (num_hidden_layers != 1)
+    return unsupported("edge_mlp_bwd differentiates one hidden layer (0: tfgnn_b200_rgcn_bwd; 2 or more are not built)");
+  if (flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION)
+    return unsupported("edge_mlp_bwd: activation-before-aggregation is not built yet");
+  if (aggregation == TFGNN_AGG_MAX) return unsupported("edge_mlp_bwd: max aggregation is not built yet");
+  if (D % 4 != 0 || H % 4 != 0) return unsupported("edge_mlp_bwd needs D and H to be multiples of 4");
+  if (H > 512) return unsupported("edge_mlp_bwd: hidden width above 512 is not built");
+  TFGNN_REQUIRE(b != nullptr && bt != nullptr, "batch / transposed batch is NULL");
+  // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
+  const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
+  const int L = b->L;
+  {
+    const int rc = check_backward_pair(b, bt);
+    if (rc) return rc;
+  }
+  TFGNN_REQUIRE(L == 0 || (mlp_weights && grad_weights), "weight / weight-gradient table is NULL");
+  const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // U_l is then [2D, H]: rows [0,D) source, [D,2D) target
+  const int KU = use_target ? 2 * D : D;                          // rows of U_l
+  PtrTable us{}, w2{}, gw2{};
+  for (int l = 0; l < L; ++l) {
+    TFGNN_REQUIRE(mlp_weights[2 * l] && mlp_weights[2 * l + 1] && grad_weights[2 * l] && grad_weights[2 * l + 1],
+                  "a weight pointer is NULL");
+    us.p[l] = mlp_weights[2 * l];
+    w2.p[l] = mlp_weights[2 * l + 1];
+    gw2.p[l] = grad_weights[2 * l + 1];
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (V == 0 || L == 0) {   // no owned rows (an empty shard) or no edge types: zero contribution
+    for (int l = 0; l < L; ++l) {
+      TFGNN_CUDA(cudaMemsetAsync(grad_weights[2 * l], 0, (size_t)KU * H * sizeof(float), st));
+      TFGNN_CUDA(cudaMemsetAsync(grad_weights[2 * l + 1], 0, (size_t)H * H * sizeof(float), st));
+    }
+    if (grad_h && Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
+    return 0;
+  }
+  TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
+  const float* h_tgt = h + (size_t)lo * D;   // rows of the owned targets (target-state input)
+  const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
+  const int LH = L * H;
+  int rc = batch_enter(b, st);
+  if (rc) return rc;
+  rc = batch_enter(bt, st);
+  if (rc) return rc;
+  // 1a. gelu: act'(pre-activation).  The pre-activation is recomputed by the forward entry without activation BEFORE any
+  // other scratch pointer of this function is taken: the nested forward may re-grow (= free and re-allocate) slots 2, 3,
+  // 4, 5, 6 and 7, which would leave pointers taken earlier dangling.  Slot 12 is not among them.
+  if (activation == TFGNN_ACT_GELU) {
+    void* z = nullptr;
+    rc = batch_scratch(b, 12, (size_t)V * H * sizeof(float), &z);
+    if (rc) return rc;
+    rc = edge_mlp_core(b, h, D, mlp_weights, 1, H, flags, aggregation, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, (float*)z, H, st);
+    if (rc) return rc;
+    out = (const float*)z;
+  }
+  void *dz = nullptr, *Xs = nullptr, *Xt = nullptr, *A = nullptr, *cnt = nullptr, *dXs = nullptr, *Wp = nullptr,
+       *W2T = nullptr, *part = nullptr;
+  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &dz);
+  if (rc) return rc;
+  rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &Xs);   // the forward's slots for Xs, Xt, A, Wcat, W2
+  if (rc) return rc;
+  rc = batch_scratch(b, 5, (size_t)V * LH * sizeof(float), &A);      // A, then dA
+  if (rc) return rc;
+  rc = batch_scratch(b, 3, (size_t)(D > H ? D : H) * LH * sizeof(float), &Wp);   // [D, LH] packs, then [LH, D]
+  if (rc) return rc;
+  rc = batch_scratch(b, 7, (size_t)LH * H * sizeof(float), &W2T);
+  if (rc) return rc;
+  rc = batch_scratch(b, 13, (size_t)Vs * LH * sizeof(float), &dXs);
+  if (rc) return rc;
+  if (use_target) {
+    rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Xt);
+    if (rc) return rc;
+    rc = batch_scratch(b, 11, (size_t)V * LH * sizeof(float), &cnt);   // cnt, then dXt
+    if (rc) return rc;
+  }
+  const int chunks = (int)((V + kTnChunk - 1) / kTnChunk), chunks_s = (int)((Vs + kTnChunk - 1) / kTnChunk);
+  {
+    const size_t a = (size_t)chunks * LH * H, c = (size_t)chunks_s * D * H;
+    rc = batch_scratch(b, 9, (a > c ? a : c) * sizeof(float), &part);
+    if (rc) return rc;
+  }
+
+  // 1b. dZ = dOut * act'(out) * rn(v)
+  act_grad_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_out, out, V, H, activation, b->row_ptr, L,
+                                                   agg_row_norm(aggregation), (float*)dz);
+  TFGNN_LAUNCH_CHECK();
+  // 2. Xs, Xt and A_l (+ cnt_l) recomputed with the forward's GEMMs and summation order
+  GemmEpilogue none;
+  rc = launch_pack_horizontal(us, L, 0, D, H, H, (float*)Wp, LH, st);
+  if (rc) return rc;
+  rc = node_gemm(h, D, (const float*)Wp, LH, (float*)Xs, LH, Vs, LH, D, none, TFGNN_PATH_AUTO, b, 6, st);
+  if (rc) return rc;
+  if (use_target) {
+    rc = launch_pack_horizontal(us, L, D, D, H, H, (float*)Wp, LH, st);
+    if (rc) return rc;
+    rc = node_gemm(h_tgt, D, (const float*)Wp, LH, (float*)Xt, LH, V, LH, D, none, TFGNN_PATH_AUTO, b, 6, st);
+    if (rc) return rc;
+    rc = launch_hidden_relu_count((const float*)Xs, (const float*)Xt, b->row_ptr, b->src_sorted, (int)V, L, H, normalize,
+                                  (float*)A, (float*)cnt, st);
+    if (rc) return rc;
+  } else {
+    EdgeReduceParams p;
+    p.X = (const float*)Xs; p.ldx = LH; p.x_type_stride = H;
+    p.row_ptr = b->row_ptr; p.src = b->src_sorted;
+    p.out = (float*)A; p.ldo = LH; p.out_type_stride = H;
+    p.V = (int)V; p.L = L; p.C = H; p.normalize = normalize; p.hidden_relu = 1;
+    rc = launch_edge_reduce(p, /*merged=*/false, st);
+    if (rc) return rc;
+  }
+  // 3. dW2_l = A_l^T dZ
+  {
+    dim3 grid((LH + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
+    gemm_tn_partial_kernel<<<grid, 256, 0, st>>>((const float*)A, LH, (const float*)dz, H, V, LH, H, (float*)part);
+    TFGNN_LAUNCH_CHECK();
+    reduce_partials_kernel<<<grid_cap((long long)LH * H), 256, 0, st>>>((const float*)part, chunks, L, H, H, gw2);
+    TFGNN_LAUNCH_CHECK();
+  }
+  // 4. dA = dZ [W2_0; ..]^T (overwrites A), dA_l[v] *= s_{v,l}
+  pack_transposed_kernel<<<grid_cap((long long)LH * H), 256, 0, st>>>(w2, L, H, H, (float*)W2T);   // [H, LH]
+  TFGNN_LAUNCH_CHECK();
+  rc = node_gemm((const float*)dz, H, (const float*)W2T, LH, (float*)A, LH, V, LH, H, none, TFGNN_PATH_AUTO, b, 6, st);
+  if (rc) return rc;
+  if (normalize) {
+    scale_by_type_kernel<<<grid_cap(V * LH), 256, 0, st>>>((float*)A, LH, V, L, H, b->row_ptr);
+    TFGNN_LAUNCH_CHECK();
+  }
+  // 5. dXs over the source-keyed CSR (on a shard: its owned transpose, every global source, local target ids);
+  //    dXt = dA * cnt in place of cnt
+  rc = launch_hidden_relu_src_bwd((const float*)Xs, (const float*)Xt, (const float*)A, bt->row_ptr, bt->src_sorted,
+                                  (int)Vs, L, H, (float*)dXs, st);
+  if (rc) return rc;
+  if (use_target) {
+    mul_inplace_kernel<<<grid_cap(V * LH), 256, 0, st>>>((float*)cnt, (const float*)A, V * LH);
+    TFGNN_LAUNCH_CHECK();
+  }
+  // 6. dU^s_l = h^T dXs_l over all Vs rows, dU^t_l = h_v^T dXt_l over the owned rows (rows [D, 2D) of U_l)
+  for (int l = 0; l < L; ++l) {
+    PtrTable gu{};
+    gu.p[0] = grad_weights[2 * l];
+    dim3 grid_s((D + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks_s);
+    gemm_tn_partial_kernel<<<grid_s, 256, 0, st>>>(h, D, (const float*)dXs + (size_t)l * H, LH, Vs, D, H, (float*)part);
+    TFGNN_LAUNCH_CHECK();
+    reduce_partials_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>((const float*)part, chunks_s, 1, D, H, gu);
+    TFGNN_LAUNCH_CHECK();
+    if (use_target) {
+      dim3 grid_t((D + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
+      gemm_tn_partial_kernel<<<grid_t, 256, 0, st>>>(h_tgt, D, (const float*)cnt + (size_t)l * H, LH, V, D, H,
+                                                     (float*)part);
+      TFGNN_LAUNCH_CHECK();
+      reduce_partials_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>((const float*)part, chunks, 1, D, H, gu, 0, 0, D);
+      TFGNN_LAUNCH_CHECK();
+    }
+  }
+  if (!grad_h) return 0;
+  // 7. grad_h = dXs [U^s_0^T; ..] (K = L*H), then the owned rows += dXt [U^t_0^T; ..]
+  for (int l = 0; l < L; ++l) {
+    PtrTable ul{};
+    ul.p[0] = mlp_weights[2 * l];
+    pack_transposed_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>(ul, 1, D, H, (float*)Wp + (size_t)l * H * D, D);
+    TFGNN_LAUNCH_CHECK();
+  }
+  rc = node_gemm((const float*)dXs, LH, (const float*)Wp, D, grad_h, D, Vs, D, LH, none, TFGNN_PATH_AUTO, b, 6, st);
+  if (rc) return rc;
+  if (use_target) {
+    for (int l = 0; l < L; ++l) {
+      PtrTable ul{};
+      ul.p[0] = mlp_weights[2 * l];
+      pack_transposed_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>(ul, 1, D, H, (float*)Wp + (size_t)l * H * D, D,
+                                                                         0, D);
+      TFGNN_LAUNCH_CHECK();
+    }
+    GemmEpilogue acc;
+    acc.accumulate = 1;
+    rc = node_gemm((const float*)cnt, LH, (const float*)Wp, D, grad_h + (size_t)lo * D, D, V, D, LH, acc,
+                   TFGNN_PATH_AUTO, b, 6, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+// =====================================================================================================================
 // Node-level glue of GNN._internal_call under training (gnn.py:279-327): backward of the bias-free / biased Dense layers,
 // LayerNormalization, and the Philox dropout shared by forward and backward.  The reference gets all of these from
 // tf.GradientTape (models/graph_task_model.py:338-365).

@@ -13,8 +13,8 @@ from .message_passing import (MessagePassing, MessagePassingInput, Variable, _la
 
 class _EdgeMLPLayerFunction(torch.autograd.Function):
     """Autograd hook of the fused layer (SURVEY.md §8f-1): forward = tfgnn_b200_edge_mlp_fwd, backward =
-    tfgnn_b200_rgcn_bwd.  The reference gets these gradients from tf.GradientTape
-    (models/graph_task_model.py:338-365)."""
+    tfgnn_b200_rgcn_bwd (no hidden layer) or tfgnn_b200_edge_mlp_bwd (one hidden layer).  The reference gets these
+    gradients from tf.GradientTape (models/graph_task_model.py:338-365)."""
 
     @staticmethod
     def forward(ctx, h, prepared, cfg, *weights):
@@ -30,15 +30,22 @@ class _EdgeMLPLayerFunction(torch.autograd.Function):
     def backward(ctx, grad_out):
         h, out, *weights = ctx.saved_tensors
         cfg, prepared = ctx.cfg, ctx.prepared
-        if cfg["n_hidden"] != 0:
-            raise NotImplementedError("backward is built for edge MLPs without hidden layers (RGCN-style) only")
+        if cfg["n_hidden"] not in (0, 1):
+            raise NotImplementedError("backward is built for edge MLPs with at most one hidden layer")
         grad_out = grad_out.contiguous()
         grad_h = torch.empty_like(h) if ctx.needs_input_grad[0] else None
         grad_w = [torch.empty_like(w) for w in weights]
-        _ffi.check(_ffi.lib().tfgnn_b200_rgcn_bwd(
-            prepared.handle, prepared.transposed().handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights),
-            cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], out.data_ptr(), grad_out.data_ptr(),
-            grad_h.data_ptr() if grad_h is not None else None, _ffi.ptr_array(grad_w), stream_ptr()))
+        gh = grad_h.data_ptr() if grad_h is not None else None
+        if cfg["n_hidden"] == 0:
+            _ffi.check(_ffi.lib().tfgnn_b200_rgcn_bwd(
+                prepared.handle, prepared.transposed().handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights),
+                cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], out.data_ptr(), grad_out.data_ptr(), gh,
+                _ffi.ptr_array(grad_w), stream_ptr()))
+        else:
+            _ffi.check(_ffi.lib().tfgnn_b200_edge_mlp_bwd(
+                prepared.handle, prepared.transposed().handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights),
+                1, cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], out.data_ptr(), grad_out.data_ptr(), gh,
+                _ffi.ptr_array(grad_w), stream_ptr()))
         return (grad_h, None, None, *grad_w)
 
 
@@ -117,12 +124,9 @@ class GNN_Edge_MLP(MessagePassing):
         self._check_types(prepared)
         ptrs, tensors = self._mlp_weight_ptrs()
         if torch.is_grad_enabled() and (h.requires_grad or any(t.requires_grad for t in tensors)):
-            fused_backward = (int(self._num_edge_MLP_hidden_layers) == 0 and self._aggregation_fn.name != "max"
-                              and not self._message_activation_before_aggregation and int(h.shape[1]) % 4 == 0
-                              and self._hidden_dim % 4 == 0)
-            if not fused_backward:
-                # hidden layers / max aggregation / activation before aggregation: the reference's literal op order with
-                # per-op backward kernels (layers/differentiable.py)
+            if not (self._has_fused_backward(int(h.shape[1])) and not self._message_activation_before_aggregation):
+                # two or more hidden layers / max aggregation / activation before aggregation: the reference's literal op
+                # order with per-op backward kernels (layers/differentiable.py)
                 from ..differentiable import edge_mlp_family_forward
                 return edge_mlp_family_forward(self, h, prepared)
             cfg = dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers), flags=self._flags(),
@@ -134,6 +138,13 @@ class GNN_Edge_MLP(MessagePassing):
             self._hidden_dim, self._flags(), self._aggregation_fn.code, self._activation_fn.code,
             _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
         return out
+
+    def _has_fused_backward(self, D: int) -> bool:
+        """The edge MLPs tfgnn_b200_rgcn_bwd (no hidden layer) and tfgnn_b200_edge_mlp_bwd (one hidden layer, the class
+        defaults of GNN_Edge_MLP and RGIN) differentiate, activation before aggregation aside."""
+        n = int(self._num_edge_MLP_hidden_layers)
+        return ((n == 0 or (n == 1 and self._hidden_dim <= 512)) and self._aggregation_fn.name != "max"
+                and D % 4 == 0 and self._hidden_dim % 4 == 0)
 
     def call_with_layernorm(self, inputs: MessagePassingInput, gamma: torch.Tensor, beta: torch.Tensor, epsilon: float,
                             prepared: Optional[PreparedBatch] = None) -> torch.Tensor:

@@ -7,9 +7,10 @@ import torch
 
 from ... import _ffi
 from ...runtime import PreparedBatch, stream_ptr
-from .gnn_edge_mlp import GNN_Edge_MLP
+from ...utils.param_helpers import get_activation_function
+from .gnn_edge_mlp import GNN_Edge_MLP, _EdgeMLPLayerFunction
 from ..differentiable import edge_mlp_family_forward
-from ..node_ops import _needs_grad
+from ..node_ops import _needs_grad, dense
 from .message_passing import MessagePassingInput, Variable, register_message_passing_implementation
 
 
@@ -48,7 +49,21 @@ class RGIN(GNN_Edge_MLP):
         h, prepared = self._device_inputs(inputs, prepared)
         self._check_types(prepared)
         if _needs_grad(h, *[v.value for v in self.variables]):
-            # training: the reference's literal op order with per-op backward kernels (layers/differentiable.py)
+            if self._has_fused_backward(int(h.shape[1])):
+                # the inference forward's op sequence, each op with its fused backward: edge MLP (activation-before is
+                # ignored, rgin.py:88-106), then the aggregation MLP and the activation
+                aggr = [v.value for v in (self._aggregation_mlp or [])]
+                act = self._activation_fn.code if (self._activation_fn is not None and not aggr) else _ffi.ACT[None]
+                cfg = dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers),
+                           flags=self._flags() & ~_ffi.FLAG_ACT_BEFORE_AGG, agg=self._aggregation_fn.code, act=act,
+                           path=_ffi.PATH[self._path])
+                out = _EdgeMLPLayerFunction.apply(h, prepared, cfg, *self._mlp_weight_ptrs()[1])
+                relu = get_activation_function("relu")
+                for i, W in enumerate(aggr):
+                    out = dense(out, W, None, self._activation_fn if i == len(aggr) - 1 else relu)
+                return out
+            # two or more hidden layers / max aggregation: the reference's literal op order with per-op backward kernels
+            # (layers/differentiable.py)
             return edge_mlp_family_forward(
                 self, h, prepared, activation_before=False,
                 aggr_kernels=[v.value for v in self._aggregation_mlp] if self._aggregation_mlp is not None else None)

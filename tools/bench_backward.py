@@ -1,10 +1,15 @@
 """Measurement of the backward pass (SURVEY.md §8f-1) at bench.py's workloads: forward and backward device time of one
 RGCN, GGNN or GNN-FiLM layer through the autograd hook, CUDA events, inputs resident in HBM.
   python tools/bench_backward.py [--workload cfg2] [--steps 10] [--warmup 3] [--shards N] [--film-literal]
+                                 [--kind rgin|gnn_edge_mlp [--literal]]
 For GNN-FiLM the line also carries the device memory in use after the steps (the library's pool and torch's allocator keep
 their high-water marks, so this is the peak of the run, inputs included).
 With --film-literal: a reduced FiLM graph on which the literal per-edge path (layers/differentiable.py) fits, 250k nodes /
 6 x 666,667 edges / D = H = 320, with the fused and the literal training step alternated in one process.
+With --kind rgin|gnn_edge_mlp: that layer (class defaults, one hidden layer in the edge MLPs; RGIN normalised as in
+PPI_RGIN.json) on the workload's graph, with D = H = the workload's hidden_dim; the line carries the device memory in use and
+the literal path's saved activations computed from shapes.  Adding --literal runs the fused and the literal path alternated
+on a reduced graph (250k nodes / 4 x 1M edges / D = H = 256).
 With --shards N: the per-rank compute of training on N target-range shards (DESIGN.md §6), on ONE GPU and without
 communication: for each shard, the build of its owned-transpose batch (TFGNN_PREPARE_TRANSPOSE_OWNED) and the backward of
 the layer on the shard from the full [V, D] table; one JSON line per workload.
@@ -34,16 +39,26 @@ def main():
     ap.add_argument("--shards", type=int, default=0, help="time the backward of each of N target-range shards")
     ap.add_argument("--film-literal", action="store_true",
                     help="fused vs literal GNN-FiLM training step on a reduced graph the literal path fits")
+    ap.add_argument("--kind", choices=sorted(EDGE_MLP_KINDS),
+                    help="time this layer kind (class defaults, one hidden layer of width H) on the workload's graph "
+                         "instead of the workload's own layer")
+    ap.add_argument("--literal", action="store_true",
+                    help="with --kind: fused vs literal training step on a reduced graph the literal path fits")
     args = ap.parse_args()
     if args.film_literal:
         return bench_film_literal(args)
+    if args.literal:
+        if not args.kind:
+            ap.error("--literal needs --kind")
+        return bench_edge_mlp_literal(args)
     wl = bench.WORKLOADS[args.workload]
     V, H, L = wl["V"], wl["H"], len(wl["E"])
     h_np, adjs_np, w_np = bench.make_inputs(wl, seed=0)
-    kind = wl["kind"]
+    kind = args.kind or wl["kind"]
+    wl = dict(wl, kind=kind)
     cls = get_message_passing_class(kind)
     params = cls.get_default_hyperparameters()
-    params.update(wl.get("params", {}))
+    params.update(EDGE_MLP_KINDS[kind] if args.kind else wl.get("params", {}))
     params.update(hidden_dim=H)
     layer = cls(params)
     torch.manual_seed(1)
@@ -75,14 +90,32 @@ def main():
             fwd_ms.append(e0.elapsed_time(e1))
             bwd_ms.append(e1.elapsed_time(e2))
     M = sum(wl["E"])
-    alg_fwd = bench.algorithmic_bytes(kind, V, wl["E"], H, H, params)
     rec = {
         "workload": wl["desc"], "kind": kind, "forward_ms": float(np.median(fwd_ms)), "backward_ms": float(np.median(bwd_ms)),
-        "edges_per_s_fwd_bwd": M / ((np.median(fwd_ms) + np.median(bwd_ms)) * 1e-3),
-        "forward_algorithmic_bytes": alg_fwd, "card": card(), "note": NOTES.get(kind, NOTES["rgcn"])}
-    if kind == "gnn_film":
+        "edges_per_s_fwd_bwd": M / ((np.median(fwd_ms) + np.median(bwd_ms)) * 1e-3), "steps": args.steps,
+        "card": card(), "note": NOTES.get(kind, NOTES["rgcn"])}
+    if args.kind:
+        rec["params"] = EDGE_MLP_KINDS[kind]
+        rec["literal_saved_activations_GB_from_shapes"] = literal_footprint_gb(M, H, H, params)
+    else:
+        rec["forward_algorithmic_bytes"] = bench.algorithmic_bytes(kind, V, wl["E"], H, H, params)
+    if kind in ("gnn_film",) + tuple(EDGE_MLP_KINDS):
         rec["device_memory_used_GB"] = device_used_gb()
     print(json.dumps(rec), flush=True)
+
+
+# --kind: class defaults (one hidden layer in the edge MLPs); RGIN with PPI_RGIN.json's normalisation
+EDGE_MLP_KINDS = {"rgin": {"normalize_by_num_incoming": True}, "gnn_edge_mlp": {}}
+
+
+def literal_footprint_gb(M, D, H, params):
+    """Saved activations of the literal per-edge path (layers/differentiable.py, edge_mlp_family_forward) for one
+    one-hidden-layer edge-MLP layer over M edges, from the shapes of its op sequence (not measured): the gathered source
+    rows [E, D] (with target-state input also the target rows and their [E, 2D] concat), the hidden layer's output
+    [E, H], the output layer's [E, H], the normalised messages [E, H] and the [M, H] concat of all types."""
+    target = params.get("use_target_state_as_input", False)
+    per_edge = (4 * D if target else D) + 2 * H + (H if params.get("normalize_by_num_incoming") else 0) + H
+    return 4.0 * M * per_edge / 1e9
 
 
 NOTES = {
@@ -90,6 +123,11 @@ NOTES = {
             "autograd hook overhead included; not tuned (two-kernel form, SIMT dW)",
     "ggnn": "backward = recomputed GRU inputs + gate backward + TN GEMMs for the GRU kernels + the RGCN-style message backward; "
             "autograd hook overhead included",
+    "rgin": "one hidden layer: backward = recompute Xs (= h U^s) and A_l (hidden_relu CSR reduce), dW2 (TN, fp32 FFMA), "
+            "dA (tensor-core GEMM), dXs over the source-keyed CSR (one warp per (type, source)), dU (TN), grad_h "
+            "(tensor-core GEMM, K = L*H); autograd hook overhead included",
+    "gnn_edge_mlp": "as rgin, plus Xt = h_v U^t, the per-column count of active edges in the recompute pass, "
+                    "dXt = dA * count, dU^t (TN) and the target rows of grad_h (accumulating GEMM)",
     "gnn_film": "backward = per type: recompute [A_l | T_l] (CSR reduce), dQ_l and dgamma_l (tensor-core GEMMs with the dZ "
                 "multiply in the epilogue), dW_l and dF_l (TN GEMMs, fp32 FFMA), dA_l and the target-side terms "
                 "(tensor-core GEMMs); then one source-keyed CSR reduce for dh; autograd hook overhead included",
@@ -167,6 +205,60 @@ def bench_film_literal(args):
                 ms[name][1].append(e1.elapsed_time(e2))
     print(json.dumps({
         "workload": wl["desc"], "kind": "gnn_film", "steps": args.steps, "card": card(),
+        "paths": {k: {"forward_ms": float(np.median(f)), "backward_ms": float(np.median(b)),
+                      "device_memory_used_GB": mem[k]} for k, (f, b) in ms.items()},
+        "note": "alternated step by step in one process; memory = device memory in use after the step with the library's "
+                "pool and torch's allocator cache emptied before it (their high-water mark for that path, inputs included)"}),
+        flush=True)
+
+
+def bench_edge_mlp_literal(args):
+    """Fused (tfgnn_b200_edge_mlp_bwd) vs literal (layers/differentiable.py) training step of an RGIN or GNN_Edge_MLP layer
+    with one hidden layer, alternated step by step, on a reduced graph the literal path fits."""
+    from tf2_gnn_b200.layers.differentiable import edge_mlp_family_forward
+    kind = args.kind
+    wl = dict(V=250_000, E=[1_000_000] * 4, H=256, kind=kind, graph="er",
+              desc=f"{kind} reduced graph: 250k nodes / 4M edges / 4 edge types, D = H = 256 (class defaults, "
+                   f"{EDGE_MLP_KINDS[kind] or 'nothing'} changed)")
+    V, H, L = wl["V"], wl["H"], len(wl["E"])
+    h_np, adjs_np, _ = bench.make_inputs(wl, seed=0)
+    cls = get_message_passing_class(kind)
+    layer = cls(dict(cls.get_default_hyperparameters(), hidden_dim=H, **EDGE_MLP_KINDS[kind]))
+    torch.manual_seed(1)
+    layer.build(MessagePassingInput((None, H), tuple((None, 2) for _ in range(L))))
+    for v in layer.variables:
+        v.requires_grad_()
+    dev = torch.device("cuda", 0)
+    h = torch.from_numpy(h_np).to(dev).requires_grad_()
+    adj = tuple(torch.from_numpy(a).to(dev) for a in adjs_np)
+    g = torch.rand((V, H), device=dev) * 2 - 1
+    prepared = PreparedBatch(adj, V)
+    prepared.transposed()
+    literal_kw = dict(activation_before=False, aggr_kernels=None) if kind == "rgin" else {}
+    paths = {"fused": lambda: layer(MessagePassingInput(h, adj), prepared=prepared),
+             "literal": lambda: edge_mlp_family_forward(layer, h, prepared, **literal_kw)}
+    ms = {k: ([], []) for k in paths}
+    mem = {k: 0.0 for k in paths}
+    for i in range(args.warmup + args.steps):
+        for name, fwd in paths.items():
+            release_memory()
+            e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            h.grad = None
+            for v in layer.variables:
+                v.value.grad = None
+            e0.record()
+            out = fwd()
+            e1.record()
+            out.backward(g)
+            e2.record()
+            torch.cuda.synchronize()
+            mem[name] = max(mem[name], device_used_gb())
+            del out
+            if i >= args.warmup:
+                ms[name][0].append(e0.elapsed_time(e1))
+                ms[name][1].append(e1.elapsed_time(e2))
+    print(json.dumps({
+        "workload": wl["desc"], "kind": kind, "steps": args.steps, "card": card(),
         "paths": {k: {"forward_ms": float(np.median(f)), "backward_ms": float(np.median(b)),
                       "device_memory_used_GB": mem[k]} for k, (f, b) in ms.items()},
         "note": "alternated step by step in one process; memory = device memory in use after the step with the library's "
