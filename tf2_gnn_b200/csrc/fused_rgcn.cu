@@ -13,7 +13,8 @@
 // The accumulators of a 64 x BN half tile take BN registers per thread, and with 17 warps a thread has 96 (five warps share
 // an SM quarter's register file), so a tile is at most 64 columns wide: wider layers take several N passes over the same
 // gathered ring slots (the ring then holds all L types of the tile).  Layers with 64 < H <= 256 (H % 32 == 0) outside
-// split-tile mode take fused_rgcn_rows_kernel instead: 64-row tiles of all H columns in one pass (see there).
+// split-tile mode take fused_rgcn_rows_kernel instead: one pass over all H columns, a CTA pair splitting each 128-row tile
+// by columns (see there).
 //
 // Warp roles (544 threads):
 //   0-7: two consumer warpgroups (split, MMA, epilogue) | 8: TMA | 9-16: gather.
@@ -309,13 +310,14 @@ __device__ __forceinline__ void gather_warp_main(const FusedParams& p, int lane,
 // Epilogue of one 64 x BN half tile (rows m0 + 64 cw + ..., columns n0 + ...) from the accumulator registers: row norm / bias /
 // activation, the fused LayerNorm (single N pass: the tile holds whole rows), stores.  Thread (warp w, lane) holds rows
 // 16 w + lane / 4 + {0, 8} and, of each 8-column group, columns 2 (lane % 4) + {0, 1}: a lane quad writes 32 contiguous bytes.
-// FOLDED: the caller has already added the correction accumulator into the main one (the same single addition).
+// FOLDED: the caller has already added the correction accumulator into the main one (the same single addition).  Only the
+// row tiling folds, and it never runs the fused LayerNorm (H <= 64 keeps fused_rgcn_kernel), so that code is left out.
 template <int BN, bool FOLDED = false>
 __device__ __forceinline__ void fused_epilogue(const FusedParams& p, const HalfTileAcc<BN>& c, long long m0, int n0, int cw,
                                                int t) {
   const int w = t >> 5, lane = t & 31, cq = 2 * (lane & 3);
   const uint64_t pol_stream = ptx::policy_evict_first();
-  const bool ln = p.epi.ln_gamma != nullptr;
+  const bool ln = !FOLDED && p.epi.ln_gamma != nullptr;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const long long row = m0 + 64 * cw + 16 * w + (lane >> 2) + 8 * h;
@@ -537,16 +539,20 @@ fused_rgcn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   }
 }
 
-// ---- row tiling (64 < H <= 256, H % 32 == 0): a tile is 64 target rows x all H columns, contracted in ONE pass -----------
-// Both consumer warpgroups read the same 64 rows of A and own H / 2 = BN columns each (main + correction: BN registers per
-// thread, 128 at H = 256).  The registers come from setmaxnreg: the kernel launches at 128 per thread (512 threads) and the
-// TMA / gather warpgroups hand theirs to the consumers.  A ring slot (64 rows, one edge type) is released as soon as its
-// K blocks are consumed, so the gather runs up to a whole tile ahead of the MMAs.  The two CTAs of a cluster take
-// neighbouring tiles and walk the same (type, K block) sequence in lockstep: each producer loads half of every weight
-// stage (the tf32-hi rows from CTA 0, the correction rows from CTA 1) and multicasts it into both CTAs, so a weight tile
-// crosses L2 -> SM once per 128 target rows.  Gather and ring stay per CTA; with an odd tile count the last cluster's
-// second CTA runs every stage on an empty tile and stores nothing.  The K order of every output element (type, K block,
-// k8 step; main and correction added in the epilogue) is that of fused_rgcn_kernel, so both give the same bits.
+// ---- row tiling (64 < H <= 256, H % 32 == 0): the N dimension in ONE pass ------------------------------------------------
+// The two CTAs of a cluster share each 128-row x H tile ("unit"), split by columns: CTA r gathers rows [64 r, 64 r + 64) of
+// the unit into its own ring slot (64 rows, one edge type) and produces columns [r BN, r BN + BN) of all 128 rows, BN = H / 2.
+// For every K block each producer loads its 64 ring rows once and multicasts them into both CTAs' stage (at row 64 r of a
+// 128-row A tile), and loads only its own BN columns of the pre-split weights.  So an SM receives 16 KB of A and 2 BN x 128 B
+// of weights per K block (48 KB at H = 256), and each weight byte it receives serves 128 rows.  Consumer warpgroup w splits
+// rows [64 w, 64 w + 64) of A and contracts them with this CTA's BN columns (main + correction: BN registers per thread, 128
+// at H = 256).  The registers come from setmaxnreg: the kernel launches at 128 per thread (512 threads) and the TMA / gather
+// warpgroups hand theirs to the consumers.  A ring slot is released as soon as its last K block has landed, so the gather
+// runs up to a whole unit ahead of the MMAs.  Both CTAs walk the same (type, K block) sequence in lockstep: every stage is
+// written by both producers, so it is refilled once all four consumer warpgroups of the pair have released it.  With an odd
+// 64-row tile count the last cluster's second CTA gathers an empty tile; both CTAs still store their columns of the first
+// 64 rows.  The K order of every output element (type, K block, k8 step; main and correction added in the epilogue) is that
+// of fused_rgcn_kernel, so both give the same bits.
 //
 // Warp roles (512 threads, warpgroup-aligned):
 //   0-7: two consumer warpgroups | 8: TMA | 9-15: gather (64 / 7 rows each: 9 or 10).
@@ -566,11 +572,11 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int H = 2 * BN;
-  constexpr int w_tile_bytes = H * kFuBK * 4;     // one of the two weight halves (hi or correction), all H columns
-  constexpr int stage_bytes = 2 * kRtATileBytes + 2 * w_tile_bytes;
+  constexpr int b_tile_bytes = BN * kFuBK * 4;    // this CTA's columns of one weight half (hi or correction)
+  constexpr int stage_bytes = 2 * kFuATileBytes + 2 * b_tile_bytes;
   const int S = p.num_stages;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);
-  uint64_t* full = bars;                          // this CTA's A and both weight halves landed
+  uint64_t* full = bars;                          // both CTAs' rows of A and this CTA's weights landed
   uint64_t* empty = bars + S;                     // the MMAs of all four consumer warpgroups of the cluster retired
   uint64_t* slot_ready = bars + 2 * S;
   uint64_t* slot_free = bars + 2 * S + kFuMaxSlots;
@@ -579,7 +585,7 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const uint32_t srank = ptx::cluster_ctarank();
-  // one unit = the cluster's pair of 64-row tiles; this CTA's tile is 2 unit + srank
+  // one unit = the cluster's 128-row tile; this CTA gathers its 64-row tile 2 unit + srank
   const long long total_units = (p.m_tiles + 1) / 2;
   const long long unit0 = blockIdx.x / 2, unit_step = gridDim.x / 2;
   const int kSlots = p.num_slots;
@@ -619,11 +625,14 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
               // both CTAs' copies of the stage are free (the multicast below writes into the peer's as well)
               ptx::mbar_wait_cluster(&empty[s], ph ^ 1);
               uint8_t* st = smem + (size_t)s * stage_bytes;
-              ptx::mbar_arrive_expect_tx(&full[s], kRtATileBytes + 2 * w_tile_bytes);
-              ptx::tma_load_2d_hint(st, &map_a, &full[s], kb * kFuBK, ring_row0 + slot * kRtBM, pol_keep);
+              // this CTA's full[s] counts both producers' rows of A and its own weight columns
+              ptx::mbar_arrive_expect_tx(&full[s], kFuATileBytes + 2 * b_tile_bytes);
+              ptx::tma_load_2d_multicast_hint(st + (int)srank * kRtATileBytes, &map_a, &full[s], kb * kFuBK,
+                                              ring_row0 + slot * kRtBM, (uint16_t)0x3, pol_keep);
               const int kcol = (l * p.kb_per_type + kb) * kFuBK;
-              ptx::tma_load_2d_multicast_hint(st + 2 * kRtATileBytes + (int)srank * w_tile_bytes, &map_b, &full[s], kcol,
-                                              (int)srank * H, (uint16_t)0x3, pol_keep);
+              ptx::tma_load_2d_hint(st + 2 * kFuATileBytes, &map_b, &full[s], kcol, (int)srank * BN, pol_keep);
+              ptx::tma_load_2d_hint(st + 2 * kFuATileBytes + b_tile_bytes, &map_b, &full[s], kcol, H + (int)srank * BN,
+                                    pol_keep);
             }
           }
         }
@@ -641,7 +650,7 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
 #undef TFGNN_RT_GATHER
     }
   } else {
-    // ================= consumers: warpgroup cw -> columns [cw BN, cw BN + BN) of the tile's 64 rows =================
+    // ================= consumers: warpgroup cw -> rows [64 cw, 64 cw + 64) x this CTA's BN columns =================
     ptx::setmaxnreg_inc<kRtConsumerRegs>();
     const int cw = wg, t = threadIdx.x & 127;
     const uint32_t empty0_cta0 = ptx::mapa_shared(ptx::smem_u32(&empty[0]), 0u);
@@ -662,8 +671,10 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
           const int s = it % S;
           const uint32_t ph = (it / S) & 1;
           ptx::mbar_wait_backoff(&full[s], ph, p.sleep_crit);
-          // the last K block of the slot has landed: its lines are dead.  This warpgroup discards half of the rows from L2
-          // (never written back to HBM), and the slot goes back to the gather warps.
+          // The last K block of this CTA's slot has landed here, and only this CTA's producer reads the slot (the peer gets
+          // the rows through the multicast, from the same L2 read): its lines are dead.  This warpgroup discards half of the
+          // rows from L2 (never written back to HBM), and the slot goes back to the gather warps.  Split-tile mode
+          // (fused_rgcn_kernel) cannot discard, because there the peer CTA reads the shared slot itself.
           const bool slot_done = kb == p.kb_per_type - 1;
           if (slot_done && p.discard_ring) {
             const char* sb = reinterpret_cast<const char*>(
@@ -672,16 +683,15 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
             for (int i = t; i < lines; i += 128) ptx::discard_l2_128(sb + (size_t)i * 128);
           }
           const uint32_t st = ptx::smem_u32(smem + (size_t)s * stage_bytes);
-          split_a_half<128, kRtBM>(st, cw, t, p.corr_bf16);   // each warpgroup splits 32 of the 64 shared rows
+          split_a_half<128>(st, cw, t, p.corr_bf16);   // this warpgroup's 64 rows only
           ptx::fence_proxy_async_smem();
-          ptx::warpgroup_pair_sync(1);                        // ... and both halves are split before either MMA reads them
+          ptx::warpgroup_sync(1 + cw);
           if (slot_done && t == 0) ptx::mbar_arrive(&slot_free[slot]);
-          const uint32_t w = st + 2 * kRtATileBytes + (uint32_t)(cw * BN * 128);
           ptx::wgmma_fence();
-          mma_kblock_at<BN, 128>(c, st, st + kRtATileBytes, w, w + w_tile_bytes, p.corr_bf16, first);
+          mma_kblock<BN, 128>(c, st, st + 2 * kFuATileBytes, cw, p.corr_bf16, first);
           ptx::wgmma_commit();
-          // The stage goes back to both producers as soon as its MMAs retire, before the next stage is waited for: with
-          // two 80 KB stages, holding it one more block (wait_group 1) would leave a single stage load in flight.
+          // The stage goes back to both producers as soon as its MMAs retire, before the next stage is waited for.  On cfg2
+          // this measured as fast as three stages (gather depth 4 instead of 8) that keep one K block of MMAs in flight.
           ptx::wgmma_wait<0>();
           release_stage(s);
           first = false;
@@ -691,8 +701,9 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
       // main + correction first: the correction registers are free for the epilogue
 #pragma unroll
       for (int j = 0; j < BN / 2; ++j) c.main[j] += c.corr[j];
-      // rows past V (the idle CTA of the last cluster: all of them) are not stored
-      fused_epilogue<BN, true>(p, c, (2 * unit + srank) * kRtBM, cw * BN, 0, t);
+      // rows past V (the second half of the last unit with an odd tile count: all of them) are not stored.  The warpgroup's
+      // row offset goes into m0 (cw = 0) so that the epilogue needs no extra register for it.
+      fused_epilogue<BN, true>(p, c, unit * kFuBM + 64 * cw, (int)srank * BN, 0, t);
     }
   }
   __syncwarp();
@@ -806,8 +817,9 @@ void restore_l2_persist_carveout() {
 }
 
 constexpr int kFuMaxGrid = 160;
-// Row tiling: 3 slots of 64 rows by default (26 MB of ring at D = 256 on 132 SMs).  On cfg2 (H100 SXM, 400 W) 3 slots ran
-// the layer in 12.05 ms and 4 slots in 12.96 ms: the smaller ring leaves more of L2 to the weights and the source rows.
+// Row tiling: 3 slots of 64 rows by default (26 MB of ring at D = 256 on 132 SMs).  On cfg2 (H100 SXM, 400 W) 2 slots ran
+// within 1 % of 3, and 4 and 5 slots 6 % and 13 % slower (DESIGN.md §4): the smaller ring leaves more of L2 to the weights
+// and the source rows.
 static int fused_num_slots(int L, bool multi_pass, bool rows = false) {
   static const int env_slots = [] { const char* e = getenv("TFGNN_B200_RING_SLOTS"); return e ? atoi(e) : 0; }();
   if (multi_pass) return L + 1;
@@ -925,7 +937,8 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
   const int split_env = split_str ? atoi(split_str) : 1;
   const bool split = !want_ln && split_env != 0 && 2 * p.m_tiles <= sms && H % 32 == 0 &&
                      (fused_block_n(H / 2) == H / 2 || L + 1 <= kFuMaxSlots);
-  // Row tiling (fused_rgcn_rows_kernel): 64 x H tiles in one N pass, for the full-size launch of the layers wider than one
+  // Row tiling (fused_rgcn_rows_kernel): 128 x H tiles in one N pass, split by columns over a CTA pair (m_tiles counts the
+  // 64-row halves each CTA gathers), for the full-size launch of the layers wider than one
   // 64-column tile up to H = 256.  Split-tile mode, the fused LayerNorm (H <= 64) and H > 256 keep fused_rgcn_kernel.
   const bool rows = !split && !want_ln && H > kFuMaxBN && H <= kRtMaxH && H % 32 == 0;
   p.split = split ? 1 : 0;
@@ -954,8 +967,8 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
   const int row_bytes = D * 4;
   const int want_q = q_env >= 1 && q_env <= kFuMaxQ ? q_env : kFuMaxQ;
   const int gather_warps = rows ? kRtGatherWarps : kFuGatherWarps;
-  // row tiling: A and its correction operand (64 rows each) + the hi and correction rows of all H weight columns
-  const int stage_bytes = rows ? 2 * kRtATileBytes + 2 * H * kFuBK * 4 : 2 * kFuATileBytes + 2 * p.block_n * kFuBK * 4;
+  // A and its correction operand (128 rows each) + the hi and correction rows of the CTA's block_n weight columns
+  const int stage_bytes = 2 * kFuATileBytes + 2 * p.block_n * kFuBK * 4;
   auto q_for = [&](int s_) { return (kFuSmemLimit - fixed_bytes - s_ * stage_bytes) / (gather_warps * row_bytes); };
   int stages = stage_env >= 2 ? stage_env : 4;
   while (stages > 2 && q_for(stages) < want_q) --stages;
@@ -985,8 +998,7 @@ int launch_fused_rgcn(const float* h, int D, const int* row_ptr, const int* src,
   {
     cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)(2 * H)};
     cuuint64_t strides[1] = {(cuuint64_t)Kp * sizeof(float)};
-    // row tiling: one box is the hi (or the correction) half of the stage, all H rows
-    cuuint32_t box[2] = {(cuuint32_t)kFuBK, (cuuint32_t)(rows ? H : p.block_n)};
+    cuuint32_t box[2] = {(cuuint32_t)kFuBK, (cuuint32_t)p.block_n};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = encode(&map_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(packedB), dims, strides, box,
                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,

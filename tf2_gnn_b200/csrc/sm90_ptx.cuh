@@ -160,8 +160,6 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 __device__ __forceinline__ void reg_fence(float& x) { asm volatile("" : "+f"(x)::"memory"); }
 // Barrier over the 128 threads of one warpgroup (id 1..15; 0 is __syncthreads).
 __device__ __forceinline__ void warpgroup_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
-// Barrier over the 256 threads of two warpgroups.
-__device__ __forceinline__ void warpgroup_pair_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
 
 // Shared-memory matrix descriptor of a K-major tile with 128-byte (ROW_BYTES = 128: 32 tf32 per row, 8-row groups 1024 B
 // apart) or 64-byte swizzle (ROW_BYTES = 64, groups 512 B apart): start[0,14) LBO[16,30) SBO[32,46) layout[62,64)

@@ -16,15 +16,14 @@ struct HalfTileAcc {
   float corr[BN / 2];
 };
 
-// Splits this warpgroup's half of the raw fp32 A tile (TILE_ROWS rows of ROW_BYTES at a_tile, TMA-swizzled; warpgroup wg
-// takes rows [wg * TILE_ROWS / 2, (wg + 1) * TILE_ROWS / 2)) in place: the tile becomes tf32(a), and the tile at
-// a_tile + TILE_ROWS * ROW_BYTES the correction operand - tf32(a - tf32(a)), or with corr_bf16 the bf16 pair
-// (a | a - tf32(a)) (sm90_ptx.cuh).  Position-preserving, so independent of the swizzle.
-template <int ROW_BYTES, int TILE_ROWS = 128>
+// Splits this warpgroup's 64 rows of the raw fp32 A tile (128 rows of ROW_BYTES at a_tile, TMA-swizzled) in place: the
+// tile becomes tf32(a), and the tile at a_tile + 128 * ROW_BYTES the correction operand - tf32(a - tf32(a)), or with
+// corr_bf16 the bf16 pair (a | a - tf32(a)) (sm90_ptx.cuh).  Position-preserving, so independent of the swizzle.
+template <int ROW_BYTES>
 __device__ __forceinline__ void split_a_half(uint32_t a_tile, int wg, int t, int corr_bf16) {
-  const uint32_t a_s = a_tile + (uint32_t)(wg * (TILE_ROWS / 2) * ROW_BYTES) + (uint32_t)t * 16u;
-  const uint32_t lo_s = a_s + (uint32_t)(TILE_ROWS * ROW_BYTES);
-  constexpr int kIt = TILE_ROWS / 2 * ROW_BYTES / 16 / 128;
+  const uint32_t a_s = a_tile + (uint32_t)(wg * 64 * ROW_BYTES) + (uint32_t)t * 16u;
+  const uint32_t lo_s = a_s + 128u * ROW_BYTES;
+  constexpr int kIt = 64 * ROW_BYTES / 16 / 128;
   float4 xs[kIt];
 #pragma unroll
   for (int i = 0; i < kIt; ++i) xs[i] = ptx::lds_f4(a_s + (uint32_t)i * 2048u);
@@ -50,14 +49,14 @@ __device__ __forceinline__ void split_a_half(uint32_t a_tile, int wg, int t, int
 
 // Issues (does not wait for) the MMAs of one K block of ROW_BYTES / 4 floats: B is the pre-split weight tile (BN rows of
 // tf32 hi at b_tile, BN rows of the correction operand right after it).  first: the block starts the tile's accumulation.
-// mma_kblock_at: the same with every operand placed explicitly (64 rows of A hi / correction, BN rows of B hi / correction).
 template <int BN, int ROW_BYTES>
-__device__ __forceinline__ void mma_kblock_at(HalfTileAcc<BN>& c, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
-                                              int corr_bf16, bool first) {
+__device__ __forceinline__ void mma_kblock(HalfTileAcc<BN>& c, uint32_t a_tile, uint32_t b_tile, int wg, int corr_bf16,
+                                           bool first) {
+  const uint32_t a_hi = a_tile + (uint32_t)(wg * 64 * ROW_BYTES);
   const uint64_t da_hi = ptx::gmma_desc_k<ROW_BYTES>(a_hi);
-  const uint64_t da_lo = ptx::gmma_desc_k<ROW_BYTES>(a_lo);
-  const uint64_t db_hi = ptx::gmma_desc_k<ROW_BYTES>(b_hi);
-  const uint64_t db_lo = ptx::gmma_desc_k<ROW_BYTES>(b_lo);
+  const uint64_t da_lo = ptx::gmma_desc_k<ROW_BYTES>(a_hi + 128u * ROW_BYTES);
+  const uint64_t db_hi = ptx::gmma_desc_k<ROW_BYTES>(b_tile);
+  const uint64_t db_lo = ptx::gmma_desc_k<ROW_BYTES>(b_tile + (uint32_t)(BN * ROW_BYTES));
 #pragma unroll
   for (int k = 0; k < ROW_BYTES / 32; ++k) {
     const uint64_t adv = (uint64_t)(k * 32 >> 4);   // 8 tf32 (or 16 bf16) = 32 B along K inside the swizzle row
@@ -70,13 +69,6 @@ __device__ __forceinline__ void mma_kblock_at(HalfTileAcc<BN>& c, uint32_t a_hi,
     }
     ptx::wgmma_tf32<BN>(c.main, da_hi + adv, db_hi + adv, acc);
   }
-}
-template <int BN, int ROW_BYTES>
-__device__ __forceinline__ void mma_kblock(HalfTileAcc<BN>& c, uint32_t a_tile, uint32_t b_tile, int wg, int corr_bf16,
-                                           bool first) {
-  const uint32_t a_hi = a_tile + (uint32_t)(wg * 64 * ROW_BYTES);
-  mma_kblock_at<BN, ROW_BYTES>(c, a_hi, a_hi + 128u * ROW_BYTES, b_tile, b_tile + (uint32_t)(BN * ROW_BYTES), corr_bf16,
-                               first);
 }
 
 // After wgmma_wait<0>: pins the accumulators so no access is moved above the wait.
