@@ -42,20 +42,21 @@ int unsupported(const std::string& msg) {
 bool valid_act(int a) { return a >= TFGNN_ACT_NONE && a <= TFGNN_ACT_SIGMOID; }
 bool valid_agg(int a) { return a >= TFGNN_AGG_SUM && a <= TFGNN_AGG_SQRT_N; }
 
-// Node-level contraction C = epi(A B) with B [K,N] row-major in device memory.
-// tc_scratch: buffer for the tensor-core operand packing (may be null -> SIMT only).
+// Node-level contraction C = epi(A B) with B [K,N] row-major in device memory.  The tensor-core path packs B into slot
+// kPackSlot of `batch`, or without a batch into a pool buffer freed after the GEMM.
 int node_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int N,
-                     int K, const GemmEpilogue& epi, int path, tfgnn_batch* batch, int tc_slot,
-                     cudaStream_t st) {
+                     int K, const GemmEpilogue& epi, int path, tfgnn_batch* batch, cudaStream_t st) {
   bool want_tc = (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
   const bool mul_ok = epi.mul == nullptr || (epi.ldm % 4 == 0 && (reinterpret_cast<uintptr_t>(epi.mul) & 15) == 0);
   if (want_tc && mul_ok && gemm_tc_supported(M, N, K, A, lda, C, ldc)) {   // the packing kernel takes any ldb
     void* packed = nullptr;
-    int rc = batch_scratch(batch, tc_slot, gemm_tc_packed_bytes(N, K), &packed);
+    const size_t bytes = gemm_tc_packed_bytes(N, K);
+    int rc = batch ? batch_scratch(batch, kPackSlot, bytes, &packed) : pool_alloc(&packed, bytes, st);
     if (rc) return rc;
     rc = launch_pack_weights_tc(B, ldb, K, N, (float*)packed, st);
-    if (rc) return rc;
-    return launch_gemm_tc(A, lda, (const float*)packed, C, ldc, M, N, K, epi, st);
+    if (!rc) rc = launch_gemm_tc(A, lda, (const float*)packed, C, ldc, M, N, K, epi, st);
+    if (!batch) pool_free(packed, st);
+    return rc;
   }
   if (path == TFGNN_PATH_SORTED_TC)
     return unsupported("TFGNN_PATH_SORTED_TC: shape not supported by the tensor-core GEMM (need N%16==0, K%32==0)");
@@ -102,7 +103,7 @@ static int rgcn_pipelined(tfgnn_batch* b, const float* h, int D, const float* Wc
   const size_t a_chunk_elems = (size_t)kPipeChunkRows * K;
   rc = batch_scratch(b, 2, a_chunk_elems * tfgnn_batch::kPipeBufs * sizeof(float), &A);
   if (rc) return rc;
-  rc = batch_scratch(b, 6, gemm_tc_packed_bytes(H, K), &packed);
+  rc = batch_scratch(b, kPackSlot, gemm_tc_packed_bytes(H, K), &packed);
   if (rc) return rc;
   rc = launch_pack_weights_tc(Wcat, H, K, H, (float*)packed, st);
   if (rc) return rc;
@@ -212,7 +213,7 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
     static const bool fused_auto = [] { const char* e = getenv("TFGNN_B200_FUSED"); return !e || atoi(e) != 0; }();
     if (fused_ok && (path == TFGNN_PATH_FUSED_TC || (path == TFGNN_PATH_AUTO && fused_auto))) {
       void *packed = nullptr, *ring = nullptr;
-      rc = batch_scratch(b, 6, gemm_tc_packed_bytes(H, K), &packed);
+      rc = batch_scratch(b, kPackSlot, gemm_tc_packed_bytes(H, K), &packed);
       if (rc) return rc;
       rc = batch_scratch(b, 15, fused_rgcn_ring_bytes(D, L, H), &ring);
       if (rc) return rc;
@@ -267,7 +268,7 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
     GemmEpilogue epi;
     epi.act = activation;
     epi.row_norm = row_norm; epi.row_ptr = b->row_ptr; epi.V = V; epi.L = L;
-    return node_gemm((const float*)A, K, (const float*)Wcat, H, out, ldo, V, H, K, epi, path, b, 6, st);
+    return node_gemm((const float*)A, K, (const float*)Wcat, H, out, ldo, V, H, K, epi, path, b, st);
   }
 
   if (path == TFGNN_PATH_ATOMIC)
@@ -284,14 +285,14 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
     rc = launch_pack_horizontal(first, L, 0, D, H, H, (float*)Wcat, LH, st);
     if (rc) return rc;
     GemmEpilogue none;
-    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, 6, st);
+    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
     if (rc) return rc;
     if (use_target) {
       rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Tt);
       if (rc) return rc;
       rc = launch_pack_horizontal(first, L, D, D, H, H, (float*)Wcat, LH, st);
       if (rc) return rc;
-      rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, 6, st);
+      rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, st);
       if (rc) return rc;
     }
     EdgeReduceParams p;
@@ -318,14 +319,14 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
     rc = launch_pack_horizontal(first, L, 0, D, H, H, (float*)Wcat, LH, st);
     if (rc) return rc;
     GemmEpilogue none;
-    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)Xs, LH, Vs, LH, D, none, path, b, 6, st);
+    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)Xs, LH, Vs, LH, D, none, path, b, st);
     if (rc) return rc;
     if (use_target) {
       rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Xt);
       if (rc) return rc;
       rc = launch_pack_horizontal(first, L, D, D, H, H, (float*)Wcat, LH, st);
       if (rc) return rc;
-      rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Xt, LH, V, LH, D, none, path, b, 6, st);
+      rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Xt, LH, V, LH, D, none, path, b, st);
       if (rc) return rc;
     }
     rc = batch_scratch(b, 5, (size_t)V * LH * sizeof(float), &A);
@@ -345,7 +346,7 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
     GemmEpilogue epi;
     epi.act = activation;
     epi.row_norm = row_norm; epi.row_ptr = b->row_ptr; epi.V = V; epi.L = L;
-    return node_gemm((const float*)A, LH, (const float*)W2, H, out, ldo, V, H, LH, epi, path, b, 6, st);
+    return node_gemm((const float*)A, LH, (const float*)W2, H, out, ldo, V, H, LH, epi, path, b, st);
   }
 
   // edge MLP with >= 2 hidden layers, or hidden layers combined with max-aggregation /

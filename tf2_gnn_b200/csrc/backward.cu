@@ -12,28 +12,11 @@
 // On a target-range shard (DESIGN.md §6) everything but the dh reduce covers the owned rows only; the dh reduce runs over the
 // shard's TFGNN_PREPARE_TRANSPOSE_OWNED CSR (all global sources, local target ids), so each shard writes its contribution
 // to the full grad_h table and the contributions of all shards sum to the unsharded gradient.
+#include <initializer_list>
+
 #include "layers.cuh"
 
 namespace tfgnn {
-
-__device__ __forceinline__ float act_grad_from_output(float y, int act) {
-  switch (act) {
-    case TFGNN_ACT_RELU: return y > 0.f ? 1.f : 0.f;
-    case TFGNN_ACT_TANH: return 1.f - y * y;
-    case TFGNN_ACT_LEAKY_RELU: return y > 0.f ? 1.f : kLeakyReluAlpha;
-    case TFGNN_ACT_ELU: return y > 0.f ? 1.f : y + 1.f;                               // d/dx (e^x - 1) = y + 1
-    case TFGNN_ACT_SELU: return y > 0.f ? kSeluScale : y + kSeluScale * kSeluAlpha;   // scale*alpha*e^x = y + scale*alpha
-    case TFGNN_ACT_SIGMOID: return y * (1.f - y);
-    default: return 1.f;
-  }
-}
-// gelu (utils/activation.py:7-14, tanh approximation) is not invertible from its output: derivative from the
-// recomputed PRE-activation x.
-__device__ __forceinline__ float gelu_grad_from_input(float x) {
-  const float c = 0.7978845608028654f;
-  const float t = tanhf(c * (x + 0.044715f * x * x * x));
-  return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * c * (1.0f + 3.0f * 0.044715f * x * x);
-}
 
 __global__ void act_grad_kernel(const float* __restrict__ g, const float* __restrict__ out, long long V, int H,
                                 int act, const int* __restrict__ row_ptr, int L, int row_norm,
@@ -218,29 +201,32 @@ __global__ void reduce_partials_kernel(const float* __restrict__ Cpart, int chun
 
 // ---- GGNN: Keras GRUCell (reset_after=True) backward, ggnn.py:84-87 -------------------------------------------------
 // forward: z = sig(gx_z+gh_z), r = sig(gx_r+gh_r), hh = tanh(gx_h + r*gh_h), h' = z*h + (1-z)*hh.
-// In place: gx <- dL/dgx, gh <- dL/dgh (each thread reads its six pre-activations before it writes),
-// dh_direct = dL/dh' * z (the path of h through the convex combination).
-__global__ void gru_gate_bwd_kernel(float* __restrict__ gx, float* __restrict__ gh, const float* __restrict__ h, int ldh,
-                                    const float* __restrict__ grad_out, long long V, int H,
+// dgx = dL/dgx, dgh = dL/dgh, dh_direct = dL/dh' * z (the path of h through the convex combination).  dgx / dgh may be
+// gx / gh (GGNN's backward works in place): each thread reads its six pre-activations before it writes.
+__global__ void gru_gate_bwd_kernel(const float* gx, const float* gh, const float* __restrict__ h, int ldh,
+                                    const float* __restrict__ grad_out, long long V, int H, float* dgx, float* dgh,
                                     float* __restrict__ dh_direct) {
   const long long total = V * H;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const long long v = i / H;
     const int c = (int)(i - v * H);
-    float* x = gx + v * 3 * H;
-    float* y = gh + v * 3 * H;
+    const float* x = gx + v * 3 * H;
+    const float* y = gh + v * 3 * H;
     const float ghh = y[2 * H + c];
+    const float hv = h[v * ldh + c];
     const float z = 1.0f / (1.0f + expf(-(x[c] + y[c])));
     const float r = 1.0f / (1.0f + expf(-(x[H + c] + y[H + c])));
     const float hh = tanhf(x[2 * H + c] + r * ghh);
     const float g = grad_out[i];
     const float da = g * (1.0f - z) * (1.0f - hh * hh);   // d/d(pre-tanh)
-    const float daz = g * (h[v * ldh + c] - hh) * z * (1.0f - z);
+    const float daz = g * (hv - hh) * z * (1.0f - z);
     const float dar = da * ghh * r * (1.0f - r);
-    x[c] = daz;          y[c] = daz;
-    x[H + c] = dar;      y[H + c] = dar;
-    x[2 * H + c] = da;   y[2 * H + c] = da * r;
+    float* ox = dgx + v * 3 * H;
+    float* oy = dgh + v * 3 * H;
+    ox[c] = daz;          oy[c] = daz;
+    ox[H + c] = dar;      oy[H + c] = dar;
+    ox[2 * H + c] = da;   oy[2 * H + c] = da * r;
     dh_direct[i] = g * z;
   }
 }
@@ -269,11 +255,6 @@ __global__ void add3_kernel(float* __restrict__ acc, const float* __restrict__ a
     acc[i] = acc[i] + a[i] + b[i];
 }
 
-static int grid_cap(long long n) {
-  int g = ceil_div(n, 256);
-  return g < 1 ? 1 : (g > 132 * 32 ? 132 * 32 : g);
-}
-
 // (b, bt) of a backward call: the unsharded pair (bt = TFGNN_PREPARE_TRANSPOSE of the same graph) or a target-range shard
 // and its TFGNN_PREPARE_TRANSPOSE_OWNED batch over the same range.
 static int check_backward_pair(const tfgnn_batch* b, const tfgnn_batch* bt) {
@@ -286,6 +267,157 @@ static int check_backward_pair(const tfgnn_batch* b, const tfgnn_batch* bt) {
   else
     TFGNN_REQUIRE(bt->V == b->V && bt->L == b->L && bt->V_src == b->V && (!bt->owned_transpose || bt->own_count == b->V),
                   "forward and transposed batches must describe the same graph");
+  return 0;
+}
+
+// A buffer from the library pool, freed (stream-ordered, after the work queued so far) when it goes out of scope.
+struct PoolBuffer {
+  cudaStream_t st;
+  void* p = nullptr;
+  ~PoolBuffer() { pool_free(p, st); }
+  int alloc(size_t bytes) { return pool_alloc(&p, bytes, st); }
+  float* f() const { return (float*)p; }
+};
+
+static PtrTable one_table(const void* p) {
+  PtrTable t{};
+  t.p[0] = p;
+  return t;
+}
+
+static int tn_chunks(long long M) { return (int)((M + kTnChunk - 1) / kTnChunk); }
+// floats of the partial buffer of weight_grad over M rows
+static size_t tn_partial_floats(long long M, int Kd, int N) { return (size_t)tn_chunks(M) * Kd * N; }
+
+// Weight gradient X^T Y for X [M, Kd], Y [M, N]: partial sums over fixed kTnChunk-row chunks, then summed in chunk order, so
+// the result is bitwise reproducible.  `part` holds tn_partial_floats(M, Kd, N).  The rows of X^T Y come in blocks of D:
+// block j goes to rows [row0 + (j / L) D, row0 + (j / L + 1) D) of dW_{j % L}.
+static int weight_grad(const float* X, int ldx, const float* Y, int ldy, long long M, int Kd, int N, float* part,
+                       PtrTable dW, int L, int D, int row0, cudaStream_t st) {
+  const int chunks = tn_chunks(M);
+  gemm_tn_partial_kernel<<<dim3(ceil_div(Kd, kTnTile), ceil_div(N, kTnTile), chunks), 256, 0, st>>>(X, ldx, Y, ldy, M, Kd,
+                                                                                                      N, part);
+  TFGNN_LAUNCH_CHECK();
+  for (int k0 = 0; k0 < Kd; k0 += L * D) {
+    reduce_partials_kernel<<<grid_for((long long)L * D * N), 256, 0, st>>>(part, chunks, L, D, N, dW, Kd, k0,
+                                                                            row0 + k0 / L);
+    TFGNN_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+// The transposes of a table of L weights W_l (H columns each), as packed for gemm_transposed: rows
+// [row0 + p D, row0 + (p + 1) D) of every W_l for p < parts, transposed.  Side by side: WT [H, parts L D] with block (p, l) at
+// column (p L + l) D.  Stacked (parts = 1): WT [L H, D] with block l at row l H.
+struct TransposedWeights {
+  PtrTable W;
+  int L, D, H;
+  int parts = 1, row0 = 0;
+  bool stacked = false;
+};
+
+// C [M, N] = X WT (epilogue `epi`, node GEMM) after packing WT (pack_transposed_kernel): X [M, H] multiplies every type's
+// block side by side; stacked, X [M, L H] holds one block per type and the product sums over the types.
+static int gemm_transposed(const float* X, int ldx, const TransposedWeights& w, float* WT, float* C, int ldc, long long M,
+                           int N, const GemmEpilogue& epi, tfgnn_batch* b, cudaStream_t st) {
+  if (w.stacked) {
+    for (int l = 0; l < w.L; ++l) {
+      pack_transposed_kernel<<<grid_for((long long)w.D * w.H), 256, 0, st>>>(one_table(w.W.p[l]), 1, w.D, w.H,
+                                                                             WT + (size_t)l * w.H * w.D, w.D, 0, w.row0);
+      TFGNN_LAUNCH_CHECK();
+    }
+    return node_gemm(X, ldx, WT, w.D, C, ldc, M, N, w.L * w.H, epi, TFGNN_PATH_AUTO, b, st);
+  }
+  const int LD = w.L * w.D;
+  for (int p = 0; p < w.parts; ++p) {
+    pack_transposed_kernel<<<grid_for((long long)LD * w.H), 256, 0, st>>>(w.W, w.L, w.D, w.H, WT, w.parts * LD, p * LD,
+                                                                          w.row0 + p * w.D);
+    TFGNN_LAUNCH_CHECK();
+  }
+  return node_gemm(X, ldx, WT, w.parts * LD, C, ldc, M, N, w.H, epi, TFGNN_PATH_AUTO, b, st);
+}
+
+// n gradient buffers p[0], p[step], p[2 step], .. of `floats` floats each
+struct GradBuffers {
+  float* const* p;
+  int n;
+  size_t floats;
+  int step = 1;
+};
+
+// The contribution of a backward call without owned rows (an empty shard) or without edge types: every weight gradient and
+// grad_h (when given, grad_h_floats floats) are cleared.
+static int zero_contribution(std::initializer_list<GradBuffers> weights, float* grad_h, size_t grad_h_floats,
+                             cudaStream_t st) {
+  for (const GradBuffers& g : weights)
+    for (int i = 0; i < g.n; ++i) {
+      float* p = g.p[(size_t)i * g.step];
+      TFGNN_REQUIRE(p, "a weight-gradient pointer is NULL");
+      TFGNN_CUDA(cudaMemsetAsync(p, 0, g.floats * sizeof(float), st));
+    }
+  if (grad_h && grad_h_floats) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, grad_h_floats * sizeof(float), st));
+  return 0;
+}
+
+static int enter_both(tfgnn_batch* b, tfgnn_batch* bt, cudaStream_t st) {
+  const int rc = batch_enter(b, st);
+  return rc ? rc : batch_enter(bt, st);
+}
+
+// The start of a fused layer backward with owned rows and edge types: enters both batches and forms
+// dZ = dOut * act'(out) * rn(v) [V, H] in slot 8 of b.  For gelu, act' needs the pre-activation: `preact(z)` recomputes it
+// (the layer's forward without activation) into a pool buffer that is freed once dZ is formed, so no scratch pointer is held
+// across that nested forward call, which may regrow any slot.
+template <class Preact>
+static int begin_backward(tfgnn_batch* b, tfgnn_batch* bt, const float* out, const float* grad_out, int H, int activation,
+                          int aggregation, cudaStream_t st, float** dz, Preact preact) {
+  const long long V = b->V;
+  int rc = enter_both(b, bt, st);
+  if (rc) return rc;
+  PoolBuffer z{st};
+  if (activation == TFGNN_ACT_GELU) {
+    rc = z.alloc((size_t)V * H * sizeof(float));
+    if (!rc) rc = preact(z.f());
+    if (rc) return rc;
+    out = z.f();
+  }
+  void* d = nullptr;
+  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &d);
+  if (rc) return rc;
+  *dz = (float*)d;
+  act_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_out, out, V, H, activation, b->row_ptr, b->L,
+                                                   agg_row_norm(aggregation), *dz);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+// grad_h[u] = sum over the edges LEAVING u of every type l of dA_l[v] (at dA + v ldx + l D): the merged reduce over bt's
+// source-keyed CSR.  On a shard that is its owned transpose: Vs segments per type (every global source; rows without an
+// owned edge get zeros), values = local target ids = rows of dA.
+static int reduce_over_sources(const tfgnn_batch* bt, const float* dA, int ldx, int D, long long Vs, float* grad_h,
+                               cudaStream_t st) {
+  EdgeReduceParams p;
+  p.X = dA; p.ldx = ldx; p.x_type_stride = D;
+  p.row_ptr = bt->row_ptr; p.src = bt->src_sorted;
+  p.out = grad_h; p.ldo = D;
+  p.V = (int)Vs; p.L = bt->L; p.C = D;
+  return launch_edge_reduce(p, /*merged=*/true, st);
+}
+
+// column sums of X [V, N] in fixed-order chunks -> out [N]   (bias / gamma / beta gradients).  `part` holds
+// tn_chunks(V) * N floats; without it the call takes a pool buffer.
+static int column_sums(const float* X, long long V, int N, float* out, float* part, cudaStream_t st) {
+  const int chunks = tn_chunks(V);
+  PoolBuffer own{st};
+  if (!part) {
+    const int rc = own.alloc((size_t)chunks * N * sizeof(float));
+    if (rc) return rc;
+    part = own.f();
+  }
+  colsum_partial_kernel<<<dim3(ceil_div(N, 128), chunks), 128, 0, st>>>(X, V, N, part);
+  TFGNN_LAUNCH_CHECK();
+  colsum_reduce_kernel<<<ceil_div(N, 128), 128, 0, st>>>(part, chunks, N, out);
+  TFGNN_LAUNCH_CHECK();
   return 0;
 }
 
@@ -303,10 +435,7 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
   const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
-  {
-    const int rc = check_backward_pair(b, bt);
-    if (rc) return rc;
-  }
+  if (int rc = check_backward_pair(b, bt)) return rc;
   if (flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION)
     return unsupported("rgcn_bwd: activation-before-aggregation is not built yet");
   const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // W_l is then [2D, H]: rows [0,D) source, [D,2D) target
@@ -314,14 +443,8 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   if (D % 4 != 0 || H % 4 != 0) return unsupported("rgcn_bwd needs D and H to be multiples of 4");
   TFGNN_REQUIRE(L == 0 || (W && grad_W), "weight / weight-gradient table is NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  if (V == 0 || L == 0) {   // no owned rows (an empty shard) or no edge types: zero contribution
-    for (int l = 0; l < L && V == 0; ++l) {
-      TFGNN_REQUIRE(grad_W[l], "a weight-gradient pointer is NULL");
-      TFGNN_CUDA(cudaMemsetAsync(grad_W[l], 0, (size_t)(use_target ? 2 * D : D) * H * sizeof(float), st));
-    }
-    if (grad_h && Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
-    return 0;
-  }
+  if (V == 0 || L == 0)   // no owned rows (an empty shard) or no edge types: zero contribution
+    return zero_contribution({{grad_W, L, (size_t)(use_target ? 2 * D : D) * H}}, grad_h, (size_t)Vs * D, st);
   TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
   const float* h_tgt = h + (size_t)lo * D;   // rows of the owned targets (target-state input)
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
@@ -333,36 +456,20 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     wt.p[l] = W[l];
     gwt.p[l] = grad_W[l];
   }
-  void *dz = nullptr, *A = nullptr, *WT = nullptr, *part = nullptr;
-  int rc = batch_enter(b, st);
+  // 1. dZ = dOut * act'(out) * rn(v)
+  float* dz = nullptr;
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, &dz, [&](float* z) {
+    return edge_mlp_core(b, h, D, W, 0, H, flags, aggregation, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, z, H, st);
+  });
   if (rc) return rc;
-  rc = batch_enter(bt, st);
-  if (rc) return rc;
-  // 1a. gelu: act'(pre-activation).  The pre-activation is recomputed by the forward kernel without activation
-  // BEFORE any other scratch pointer of this function is taken: the nested forward call may re-grow (= free and
-  // re-allocate) the slots it shares with this function (2, 3, 6), which would leave them dangling.
-  if (activation == TFGNN_ACT_GELU) {
-    void* z = nullptr;
-    rc = batch_scratch(b, 12, (size_t)V * H * sizeof(float), &z);
-    if (rc) return rc;
-    rc = edge_mlp_core(b, h, D, W, 0, H, flags, aggregation, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, (float*)z, H, st);
-    if (rc) return rc;
-    out = (const float*)z;
-  }
-  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &dz);
-  if (rc) return rc;
+  void *A = nullptr, *WT = nullptr, *part = nullptr;
   rc = batch_scratch(b, 2, (size_t)V * K * sizeof(float), &A);     // A (forward operand), then dA
   if (rc) return rc;
   rc = batch_scratch(b, 3, (size_t)K * H * sizeof(float), &WT);
   if (rc) return rc;
-  const int chunks = (int)((V + kTnChunk - 1) / kTnChunk);
-  rc = batch_scratch(b, 9, (size_t)chunks * K * H * sizeof(float), &part);
+  rc = batch_scratch(b, 9, tn_partial_floats(V, K, H) * sizeof(float), &part);
   if (rc) return rc;
 
-  // 1b. dZ = dOut * act'(out) * rn(v)
-  act_grad_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_out, out, V, H, activation, b->row_ptr, L,
-                                                   agg_row_norm(aggregation), (float*)dz);
-  TFGNN_LAUNCH_CHECK();
   // 2. A_l (recomputed, normalised) and dW = A^T dZ
   {
     EdgeReduceParams p;
@@ -372,49 +479,25 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     p.V = (int)V; p.L = L; p.C = D; p.normalize = normalize;
     rc = launch_edge_reduce(p, /*merged=*/false, st);
     if (rc) return rc;
-    if (use_target) {
-      rc = launch_target_term(h_tgt, D, b->row_ptr, (int)V, L, D, normalize, (float*)A, K, LD, st);
-      if (rc) return rc;
-    }
-    dim3 grid((K + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
-    gemm_tn_partial_kernel<<<grid, 256, 0, st>>>((const float*)A, K, (const float*)dz, H, V, K, H, (float*)part);
-    TFGNN_LAUNCH_CHECK();
-    reduce_partials_kernel<<<grid_cap((long long)LD * H), 256, 0, st>>>((const float*)part, chunks, L, D, H, gwt, K, 0, 0);
-    TFGNN_LAUNCH_CHECK();
-    if (use_target) {
-      reduce_partials_kernel<<<grid_cap((long long)LD * H), 256, 0, st>>>((const float*)part, chunks, L, D, H, gwt, K, LD,
-                                                                        D);
-      TFGNN_LAUNCH_CHECK();
-    }
   }
-  if (!grad_h) return 0;
-  // 3. dA = dZ Wcat^T (overwrites A), scaled per (v,l)
-  pack_transposed_kernel<<<grid_cap((long long)LD * H), 256, 0, st>>>(wt, L, D, H, (float*)WT, K, 0, 0);
-  TFGNN_LAUNCH_CHECK();
   if (use_target) {
-    pack_transposed_kernel<<<grid_cap((long long)LD * H), 256, 0, st>>>(wt, L, D, H, (float*)WT, K, LD, D);
-    TFGNN_LAUNCH_CHECK();
-  }
-  GemmEpilogue none;
-  rc = node_gemm((const float*)dz, H, (const float*)WT, K, (float*)A, K, V, K, H, none, TFGNN_PATH_AUTO, b, 6, st);
-  if (rc) return rc;
-  if (normalize) {
-    scale_by_type_kernel<<<grid_cap(V * LD), 256, 0, st>>>((float*)A, K, V, L, D, b->row_ptr);
-    TFGNN_LAUNCH_CHECK();
-  }
-  // 4. dh[u] = sum over the edges LEAVING u (source-keyed CSR), all types merged.  On a shard: Vs segments per type (every
-  // global source, rows without an owned edge get zeros), values = local target ids = rows of dA
-  {
-    EdgeReduceParams p;
-    p.X = (const float*)A; p.ldx = K; p.x_type_stride = D;
-    p.row_ptr = bt->row_ptr; p.src = bt->src_sorted;
-    p.out = grad_h; p.ldo = D;
-    p.V = (int)Vs; p.L = L; p.C = D;
-    rc = launch_edge_reduce(p, /*merged=*/true, st);
+    rc = launch_target_term(h_tgt, D, b->row_ptr, (int)V, L, D, normalize, (float*)A, K, LD, st);
     if (rc) return rc;
   }
+  rc = weight_grad((const float*)A, K, dz, H, V, K, H, (float*)part, gwt, L, D, 0, st);
+  if (rc || !grad_h) return rc;
+  // 3. dA = dZ Wcat^T (overwrites A), scaled per (v,l)
+  rc = gemm_transposed(dz, H, {wt, L, D, H, use_target ? 2 : 1}, (float*)WT, (float*)A, K, V, K, GemmEpilogue{}, b, st);
+  if (rc) return rc;
+  if (normalize) {
+    scale_by_type_kernel<<<grid_for(V * LD), 256, 0, st>>>((float*)A, K, V, L, D, b->row_ptr);
+    TFGNN_LAUNCH_CHECK();
+  }
+  // 4. dh[u] = sum over the edges LEAVING u
+  rc = reduce_over_sources(bt, (const float*)A, K, D, Vs, grad_h, st);
+  if (rc) return rc;
   if (use_target) {   // 5. the target half: grad_h[lo + v] += sum_l coeff(v,l) * dT_l[v]
-    target_term_bwd_kernel<<<grid_cap(V * D), 256, 0, st>>>((const float*)A + LD, K, b->row_ptr, V, L, D, normalize,
+    target_term_bwd_kernel<<<grid_for(V * D), 256, 0, st>>>((const float*)A + LD, K, b->row_ptr, V, L, D, normalize,
                                                             grad_h + (size_t)lo * D);
     TFGNN_LAUNCH_CHECK();
   }
@@ -437,10 +520,7 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   // V = owned target rows, Vs = rows of h and grad_h; the GRU state of local row v is h[lo + v]
   const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
-  {
-    const int rc = check_backward_pair(b, bt);
-    if (rc) return rc;
-  }
+  if (int rc = check_backward_pair(b, bt)) return rc;
   if (flags & TFGNN_FLAG_USE_TARGET_STATE) return unsupported("ggnn_bwd: target-state input is not built yet");
   if (aggregation == TFGNN_AGG_MAX) return unsupported("ggnn_bwd: max aggregation is not built yet");
   if (H % 4 != 0) return unsupported("ggnn_bwd needs hidden_dim to be a multiple of 4");
@@ -448,28 +528,20 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   TFGNN_REQUIRE(grad_gru_kernel && grad_gru_recurrent_kernel && grad_gru_bias, "GRU gradient pointer is NULL");
   TFGNN_REQUIRE(L == 0 || grad_W, "weight-gradient table is NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  if (V == 0) {   // no owned rows (an empty shard): zero contribution
-    const size_t n3 = (size_t)H * 3 * H;
-    TFGNN_CUDA(cudaMemsetAsync(grad_gru_kernel, 0, n3 * sizeof(float), st));
-    TFGNN_CUDA(cudaMemsetAsync(grad_gru_recurrent_kernel, 0, n3 * sizeof(float), st));
-    TFGNN_CUDA(cudaMemsetAsync(grad_gru_bias, 0, (size_t)2 * 3 * H * sizeof(float), st));
-    for (int l = 0; l < L; ++l) {
-      TFGNN_REQUIRE(grad_W[l], "a weight-gradient pointer is NULL");
-      TFGNN_CUDA(cudaMemsetAsync(grad_W[l], 0, (size_t)D * H * sizeof(float), st));
-    }
-    if (Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
-    return 0;
-  }
+  const int N3 = 3 * H;
+  if (V == 0)   // no owned rows (an empty shard): zero contribution
+    return zero_contribution({{&grad_gru_kernel, 1, (size_t)H * N3},
+                              {&grad_gru_recurrent_kernel, 1, (size_t)H * N3},
+                              {&grad_gru_bias, 1, (size_t)2 * N3},
+                              {grad_W, L, (size_t)D * H}},
+                             grad_h, (size_t)Vs * D, st);
   TFGNN_REQUIRE(h && grad_out, "NULL pointer");
   TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
   const float* h_tgt = h + (size_t)lo * D;
-  const int N3 = 3 * H;
-  const int chunks = (int)((V + kTnChunk - 1) / kTnChunk);
+  const int chunks = tn_chunks(V);
   void *agg = nullptr, *gx = nullptr, *gh = nullptr, *dagg = nullptr, *wT = nullptr, *part = nullptr, *dhd = nullptr,
        *tmp = nullptr;
-  int rc = batch_enter(b, st);
-  if (rc) return rc;
-  rc = batch_enter(bt, st);
+  int rc = enter_both(b, bt, st);
   if (rc) return rc;
   rc = batch_scratch(b, 11, (size_t)V * H * sizeof(float), &agg);
   if (rc) return rc;
@@ -481,7 +553,7 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   if (rc) return rc;
   rc = batch_scratch(b, 7, (size_t)N3 * H * sizeof(float), &wT);
   if (rc) return rc;
-  rc = batch_scratch(b, 10, (size_t)chunks * ((size_t)H * N3 + N3) * sizeof(float), &part);
+  rc = batch_scratch(b, 10, (tn_partial_floats(V, H, N3) + (size_t)chunks * N3) * sizeof(float), &part);
   if (rc) return rc;
   rc = batch_scratch(b, 4, (size_t)V * H * sizeof(float), &dhd);
   if (rc) return rc;
@@ -491,52 +563,55 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   rc = edge_mlp_core(b, h, D, W, 0, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION, aggregation, TFGNN_ACT_NONE,
                      TFGNN_PATH_AUTO, (float*)agg, H, st);
   if (rc) return rc;
-  GemmEpilogue e0, e1, none;
+  GemmEpilogue e0, e1;
   e0.bias = gru_bias;
   e1.bias = gru_bias + N3;
-  rc = node_gemm((const float*)agg, H, gru_kernel, N3, (float*)gx, N3, V, N3, H, e0, TFGNN_PATH_AUTO, b, 6, st);
+  rc = node_gemm((const float*)agg, H, gru_kernel, N3, (float*)gx, N3, V, N3, H, e0, TFGNN_PATH_AUTO, b, st);
   if (rc) return rc;
-  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, N3, (float*)gh, N3, V, N3, H, e1, TFGNN_PATH_AUTO, b, 6, st);
+  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, N3, (float*)gh, N3, V, N3, H, e1, TFGNN_PATH_AUTO, b, st);
   if (rc) return rc;
-  // 2. gates
-  gru_gate_bwd_kernel<<<grid_cap(V * H), 256, 0, st>>>((float*)gx, (float*)gh, h_tgt, D, grad_out, V, H, (float*)dhd);
+  // 2. gates, in place
+  gru_gate_bwd_kernel<<<grid_for(V * H), 256, 0, st>>>((const float*)gx, (const float*)gh, h_tgt, D, grad_out, V, H,
+                                                       (float*)gx, (float*)gh, (float*)dhd);
   TFGNN_LAUNCH_CHECK();
   // 3. bias gradients: rows 0 / 1 of gru_bias belong to gx / gh
-  float* cpart = (float*)part + (size_t)chunks * H * N3;
-  for (int which = 0; which < 2; ++which) {
-    dim3 grid((N3 + 127) / 128, chunks);
-    colsum_partial_kernel<<<grid, 128, 0, st>>>((const float*)(which ? gh : gx), V, N3, cpart);
-    TFGNN_LAUNCH_CHECK();
-    colsum_reduce_kernel<<<(N3 + 127) / 128, 128, 0, st>>>(cpart, chunks, N3, grad_gru_bias + (size_t)which * N3);
-    TFGNN_LAUNCH_CHECK();
-  }
+  float* cpart = (float*)part + tn_partial_floats(V, H, N3);
+  rc = column_sums((const float*)gx, V, N3, grad_gru_bias, cpart, st);
+  if (rc) return rc;
+  rc = column_sums((const float*)gh, V, N3, grad_gru_bias + N3, cpart, st);
+  if (rc) return rc;
   // 4. dK = agg^T dgx, dU = h^T dgh
-  for (int which = 0; which < 2; ++which) {
-    PtrTable gt{};
-    gt.p[0] = which ? grad_gru_recurrent_kernel : grad_gru_kernel;
-    dim3 grid((H + kTnTile - 1) / kTnTile, (N3 + kTnTile - 1) / kTnTile, chunks);
-    gemm_tn_partial_kernel<<<grid, 256, 0, st>>>(which ? h_tgt : (const float*)agg, which ? D : H,
-                                                 (const float*)(which ? gh : gx), N3, V, H, N3, (float*)part);
-    TFGNN_LAUNCH_CHECK();
-    reduce_partials_kernel<<<grid_cap((long long)H * N3), 256, 0, st>>>((const float*)part, chunks, 1, H, N3, gt);
-    TFGNN_LAUNCH_CHECK();
-  }
+  rc = weight_grad((const float*)agg, H, (const float*)gx, N3, V, H, N3, (float*)part, one_table(grad_gru_kernel), 1, H, 0,
+                   st);
+  if (rc) return rc;
+  rc = weight_grad(h_tgt, D, (const float*)gh, N3, V, H, N3, (float*)part, one_table(grad_gru_recurrent_kernel), 1, H, 0,
+                   st);
+  if (rc) return rc;
   // 5. dagg = dgx K^T, dh_rec = dgh U^T
-  for (int which = 0; which < 2; ++which) {
-    PtrTable wt{};
-    wt.p[0] = which ? gru_recurrent_kernel : gru_kernel;
-    pack_transposed_kernel<<<grid_cap((long long)H * N3), 256, 0, st>>>(wt, 1, H, N3, (float*)wT);   // [3H, H]
-    TFGNN_LAUNCH_CHECK();
-    rc = node_gemm((const float*)(which ? gh : gx), N3, (const float*)wT, H, (float*)(which ? tmp : dagg), H, V, H, N3,
-                   none, TFGNN_PATH_AUTO, b, 6, st);
-    if (rc) return rc;
-  }
+  rc = gemm_transposed((const float*)gx, N3, {one_table(gru_kernel), 1, H, N3}, (float*)wT, (float*)dagg, H, V, H,
+                       GemmEpilogue{}, b, st);
+  if (rc) return rc;
+  rc = gemm_transposed((const float*)gh, N3, {one_table(gru_recurrent_kernel), 1, H, N3}, (float*)wT, (float*)tmp, H, V,
+                       H, GemmEpilogue{}, b, st);
+  if (rc) return rc;
   // 6. messages: dagg -> grad_h (through the edges) and grad_W
   rc = tfgnn_b200_rgcn_bwd(b, bt, h, D, W, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION, aggregation, TFGNN_ACT_NONE,
                            (const float*)dagg, (const float*)dagg, grad_h, grad_W, stream);
   if (rc) return rc;
   // 7. grad_h[lo + v] += dh_direct + dh_rec
-  add3_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dhd, (const float*)tmp, V * H);
+  add3_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dhd, (const float*)tmp, V * H);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int tfgnn_b200_gru_gate_bwd(const float* gx, const float* gh, const float* h, const float* grad_out,
+                                       int64_t num_rows, int32_t H, float* grad_gx, float* grad_gh, float* grad_h_direct,
+                                       void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && H > 0, "bad gru_gate_bwd sizes");
+  if (num_rows == 0) return 0;
+  TFGNN_REQUIRE(gx && gh && h && grad_out && grad_gx && grad_gh && grad_h_direct, "NULL pointer");
+  gru_gate_bwd_kernel<<<grid_for(num_rows * H), 256, 0, (cudaStream_t)stream>>>(gx, gh, h, H, grad_out, num_rows, H,
+                                                                               grad_gx, grad_gh, grad_h_direct);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -592,56 +667,35 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
   const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
-  {
-    const int rc = check_backward_pair(b, bt);
-    if (rc) return rc;
-  }
+  if (int rc = check_backward_pair(b, bt)) return rc;
   TFGNN_REQUIRE(L == 0 || (mlp_weights && film_weights && grad_W && grad_film), "weight / weight-gradient table is NULL");
   const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // W_l is then [2D, H]: rows [0,D) source, [D,2D) target
   const int KT = use_target ? 2 * D : D;                          // columns of [A_l | T_l], rows of W_l
   for (int l = 0; l < L; ++l)
     TFGNN_REQUIRE(mlp_weights[l] && film_weights[l] && grad_W[l] && grad_film[l], "a weight pointer is NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  if (V == 0 || L == 0) {   // no owned rows (an empty shard) or no edge types: zero contribution
-    for (int l = 0; l < L; ++l) {
-      TFGNN_CUDA(cudaMemsetAsync(grad_W[l], 0, (size_t)KT * H * sizeof(float), st));
-      TFGNN_CUDA(cudaMemsetAsync(grad_film[l], 0, (size_t)D * 2 * H * sizeof(float), st));
-    }
-    if (grad_h && Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
-    return 0;
-  }
+  if (V == 0 || L == 0)   // no owned rows (an empty shard) or no edge types: zero contribution
+    return zero_contribution({{grad_W, L, (size_t)KT * H}, {grad_film, L, (size_t)D * 2 * H}}, grad_h, (size_t)Vs * D, st);
   TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
   const float* h_tgt = h + (size_t)lo * D;   // rows of the owned targets (FiLM parameters, target-state input)
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
   const int LD = L * D;
-  int rc = batch_enter(b, st);
+  // 1. dZ = dOut * act'(out) * rn(v)
+  float* dz = nullptr;
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, &dz, [&](float* z) {
+    return tfgnn_b200_film_fwd(b, h, D, mlp_weights, 0, film_weights, H, flags, aggregation, TFGNN_ACT_NONE,
+                               TFGNN_PATH_AUTO, z, stream);
+  });
   if (rc) return rc;
-  rc = batch_enter(bt, st);
-  if (rc) return rc;
-  // 1a. gelu: act'(pre-activation).  The pre-activation is recomputed by the forward entry without activation BEFORE any
-  // other scratch pointer of this function is taken: the nested forward may re-grow (= free and re-allocate) slots 2, 3,
-  // 4, 6, 11 and 12, which would leave pointers taken earlier dangling.  Slot 10 is not among them.
-  if (activation == TFGNN_ACT_GELU) {
-    void* z = nullptr;
-    rc = batch_scratch(b, 10, (size_t)V * H * sizeof(float), &z);
-    if (rc) return rc;
-    rc = tfgnn_b200_film_fwd(b, h, D, mlp_weights, 0, film_weights, H, flags, aggregation, TFGNN_ACT_NONE,
-                             TFGNN_PATH_AUTO, (float*)z, stream);
-    if (rc) return rc;
-    out = (const float*)z;
-  }
-  void *dz = nullptr, *AT = nullptr, *dQ = nullptr, *dGB = nullptr, *part = nullptr;
+  void *AT = nullptr, *dQ = nullptr, *dGB = nullptr, *part = nullptr;
   void *dA = nullptr, *dHt = nullptr, *WT = nullptr, *FT = nullptr;
-  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &dz);
-  if (rc) return rc;
   rc = batch_scratch(b, 4, (size_t)V * KT * sizeof(float), &AT);   // [A_l | T_l], later dT_l
   if (rc) return rc;
   rc = batch_scratch(b, 5, (size_t)V * H * sizeof(float), &dQ);
   if (rc) return rc;
   rc = batch_scratch(b, 11, (size_t)V * 2 * H * sizeof(float), &dGB);   // [dgamma_l | dbeta_l]
   if (rc) return rc;
-  const int chunks = (int)((V + kTnChunk - 1) / kTnChunk);
-  rc = batch_scratch(b, 9, (size_t)chunks * D * 2 * H * sizeof(float), &part);   // KT * H <= D * 2H
+  rc = batch_scratch(b, 9, tn_partial_floats(V, D, 2 * H) * sizeof(float), &part);   // KT * H <= D * 2H
   if (rc) return rc;
   if (grad_h) {
     rc = batch_scratch(b, 2, (size_t)V * LD * sizeof(float), &dA);
@@ -654,12 +708,8 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     if (rc) return rc;
   }
 
-  // 1b. dZ = dOut * act'(out) * rn(v)
-  act_grad_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_out, out, V, H, activation, b->row_ptr, L,
-                                                   agg_row_norm(aggregation), (float*)dz);
-  TFGNN_LAUNCH_CHECK();
   GemmEpilogue none, by_dz;
-  by_dz.mul = (const float*)dz;
+  by_dz.mul = dz;
   by_dz.ldm = H;
   for (int l = 0; l < L; ++l) {
     const int* rp = b->row_ptr + (size_t)l * V;   // the V segments of type l
@@ -680,71 +730,45 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
       }
     }
     // 3. dQ_l = dZ * (h_v Fgamma_l);  dgamma_l = dZ * ([A_l | T_l] W_l);  dbeta_l = c dZ
-    rc = node_gemm(h_tgt, D, Fl, 2 * H, (float*)dQ, H, V, H, D, by_dz, TFGNN_PATH_AUTO, b, 6, st);
+    rc = node_gemm(h_tgt, D, Fl, 2 * H, (float*)dQ, H, V, H, D, by_dz, TFGNN_PATH_AUTO, b, st);
     if (rc) return rc;
-    rc = node_gemm((const float*)AT, KT, Wl, H, (float*)dGB, 2 * H, V, H, KT, by_dz, TFGNN_PATH_AUTO, b, 6, st);
+    rc = node_gemm((const float*)AT, KT, Wl, H, (float*)dGB, 2 * H, V, H, KT, by_dz, TFGNN_PATH_AUTO, b, st);
     if (rc) return rc;
-    film_beta_grad_kernel<<<grid_cap(V * H), 256, 0, st>>>((const float*)dz, rp, V, H, (float*)dGB);
+    film_beta_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(dz, rp, V, H, (float*)dGB);
     TFGNN_LAUNCH_CHECK();
     // 4. dW_l = [A_l | T_l]^T dQ_l,  dF_l = h_v^T [dgamma_l | dbeta_l]
-    {
-      PtrTable gw{}, gf{};
-      gw.p[0] = grad_W[l];
-      gf.p[0] = grad_film[l];
-      dim3 gridw((KT + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
-      gemm_tn_partial_kernel<<<gridw, 256, 0, st>>>((const float*)AT, KT, (const float*)dQ, H, V, KT, H, (float*)part);
-      TFGNN_LAUNCH_CHECK();
-      reduce_partials_kernel<<<grid_cap((long long)KT * H), 256, 0, st>>>((const float*)part, chunks, 1, KT, H, gw);
-      TFGNN_LAUNCH_CHECK();
-      dim3 gridf((D + kTnTile - 1) / kTnTile, (2 * H + kTnTile - 1) / kTnTile, chunks);
-      gemm_tn_partial_kernel<<<gridf, 256, 0, st>>>(h_tgt, D, (const float*)dGB, 2 * H, V, D, 2 * H, (float*)part);
-      TFGNN_LAUNCH_CHECK();
-      reduce_partials_kernel<<<grid_cap((long long)D * 2 * H), 256, 0, st>>>((const float*)part, chunks, 1, D, 2 * H, gf);
-      TFGNN_LAUNCH_CHECK();
-    }
+    rc = weight_grad((const float*)AT, KT, (const float*)dQ, H, V, KT, H, (float*)part, one_table(grad_W[l]), 1, KT, 0, st);
+    if (rc) return rc;
+    rc = weight_grad(h_tgt, D, (const float*)dGB, 2 * H, V, D, 2 * H, (float*)part, one_table(grad_film[l]), 1, D, 0, st);
+    if (rc) return rc;
     if (!grad_h) continue;
     // 5. dA_l = dQ_l W^s_l^T into columns [l*D, (l+1)*D) of dA (scaled by s after the loop)
-    PtrTable wt{}, ft{};
-    wt.p[0] = Wl;
-    ft.p[0] = Fl;
-    pack_transposed_kernel<<<grid_cap((long long)KT * H), 256, 0, st>>>(wt, 1, KT, H, (float*)WT);   // [H, KT]
-    TFGNN_LAUNCH_CHECK();
-    rc = node_gemm((const float*)dQ, H, (const float*)WT, KT, (float*)dA + (size_t)l * D, LD, V, D, H, none,
-                   TFGNN_PATH_AUTO, b, 6, st);
+    rc = gemm_transposed((const float*)dQ, H, {one_table(Wl), 1, KT, H}, (float*)WT, (float*)dA + (size_t)l * D, LD, V, D,
+                         none, b, st);
     if (rc) return rc;
     // 6. target side: dHt (+)= [dgamma_l | dbeta_l] F_l^T (+ coeff(v,l) dQ_l W^t_l^T)
-    pack_transposed_kernel<<<grid_cap((long long)D * 2 * H), 256, 0, st>>>(ft, 1, D, 2 * H, (float*)FT);   // [2H, D]
-    TFGNN_LAUNCH_CHECK();
     GemmEpilogue sum_types;
     sum_types.accumulate = l > 0;
-    rc = node_gemm((const float*)dGB, 2 * H, (const float*)FT, D, (float*)dHt, D, V, D, 2 * H, sum_types, TFGNN_PATH_AUTO,
-                   b, 6, st);
+    rc = gemm_transposed((const float*)dGB, 2 * H, {one_table(Fl), 1, D, 2 * H}, (float*)FT, (float*)dHt, D, V, D,
+                         sum_types, b, st);
     if (rc) return rc;
-    if (use_target) {   // dT_l overwrites [A_l | T_l] (read for the last time by the dW_l pass above)
-      rc = node_gemm((const float*)dQ, H, (const float*)WT + D, KT, (float*)AT, KT, V, D, H, none, TFGNN_PATH_AUTO, b, 6,
-                     st);
+    if (use_target) {   // dT_l overwrites [A_l | T_l] (read for the last time by the dW_l pass above); W^t_l^T is packed
+      rc = node_gemm((const float*)dQ, H, (const float*)WT + D, KT, (float*)AT, KT, V, D, H, none, TFGNN_PATH_AUTO, b, st);
       if (rc) return rc;
-      target_term_bwd_kernel<<<grid_cap(V * D), 256, 0, st>>>((const float*)AT, KT, rp, V, 1, D, normalize, (float*)dHt);
+      target_term_bwd_kernel<<<grid_for(V * D), 256, 0, st>>>((const float*)AT, KT, rp, V, 1, D, normalize, (float*)dHt);
       TFGNN_LAUNCH_CHECK();
     }
   }
   if (!grad_h) return 0;
   if (normalize) {
-    scale_by_type_kernel<<<grid_cap(V * LD), 256, 0, st>>>((float*)dA, LD, V, L, D, b->row_ptr);
+    scale_by_type_kernel<<<grid_for(V * LD), 256, 0, st>>>((float*)dA, LD, V, L, D, b->row_ptr);
     TFGNN_LAUNCH_CHECK();
   }
-  // 7. grad_h[u] = sum over the edges LEAVING u (source-keyed CSR; on a shard its owned transpose over all Vs sources)
-  {
-    EdgeReduceParams p;
-    p.X = (const float*)dA; p.ldx = LD; p.x_type_stride = D;
-    p.row_ptr = bt->row_ptr; p.src = bt->src_sorted;
-    p.out = grad_h; p.ldo = D;
-    p.V = (int)Vs; p.L = L; p.C = D;
-    rc = launch_edge_reduce(p, /*merged=*/true, st);
-    if (rc) return rc;
-  }
+  // 7. grad_h[u] = sum over the edges LEAVING u
+  rc = reduce_over_sources(bt, (const float*)dA, LD, D, Vs, grad_h, st);
+  if (rc) return rc;
   // 8. grad_h[lo + v] += target-side terms
-  add_kernel<<<grid_cap(V * D), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dHt, V * D);
+  add_kernel<<<grid_for(V * D), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dHt, V * D);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -948,10 +972,7 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
   // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
   const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
-  {
-    const int rc = check_backward_pair(b, bt);
-    if (rc) return rc;
-  }
+  if (int rc = check_backward_pair(b, bt)) return rc;
   TFGNN_REQUIRE(L == 0 || (mlp_weights && grad_weights), "weight / weight-gradient table is NULL");
   const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // U_l is then [2D, H]: rows [0,D) source, [D,2D) target
   const int KU = use_target ? 2 * D : D;                          // rows of U_l
@@ -964,37 +985,21 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
     gw2.p[l] = grad_weights[2 * l + 1];
   }
   cudaStream_t st = (cudaStream_t)stream;
-  if (V == 0 || L == 0) {   // no owned rows (an empty shard) or no edge types: zero contribution
-    for (int l = 0; l < L; ++l) {
-      TFGNN_CUDA(cudaMemsetAsync(grad_weights[2 * l], 0, (size_t)KU * H * sizeof(float), st));
-      TFGNN_CUDA(cudaMemsetAsync(grad_weights[2 * l + 1], 0, (size_t)H * H * sizeof(float), st));
-    }
-    if (grad_h && Vs > 0) TFGNN_CUDA(cudaMemsetAsync(grad_h, 0, (size_t)Vs * D * sizeof(float), st));
-    return 0;
-  }
+  if (V == 0 || L == 0)   // no owned rows (an empty shard) or no edge types: zero contribution
+    return zero_contribution({{grad_weights, L, (size_t)KU * H, 2}, {grad_weights + 1, L, (size_t)H * H, 2}}, grad_h,
+                             (size_t)Vs * D, st);
   TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
   const float* h_tgt = h + (size_t)lo * D;   // rows of the owned targets (target-state input)
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
   const int LH = L * H;
-  int rc = batch_enter(b, st);
+  // 1. dZ = dOut * act'(out) * rn(v)
+  float* dz = nullptr;
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, &dz, [&](float* z) {
+    return edge_mlp_core(b, h, D, mlp_weights, 1, H, flags, aggregation, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, z, H, st);
+  });
   if (rc) return rc;
-  rc = batch_enter(bt, st);
-  if (rc) return rc;
-  // 1a. gelu: act'(pre-activation).  The pre-activation is recomputed by the forward entry without activation BEFORE any
-  // other scratch pointer of this function is taken: the nested forward may re-grow (= free and re-allocate) slots 2, 3,
-  // 4, 5, 6 and 7, which would leave pointers taken earlier dangling.  Slot 12 is not among them.
-  if (activation == TFGNN_ACT_GELU) {
-    void* z = nullptr;
-    rc = batch_scratch(b, 12, (size_t)V * H * sizeof(float), &z);
-    if (rc) return rc;
-    rc = edge_mlp_core(b, h, D, mlp_weights, 1, H, flags, aggregation, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, (float*)z, H, st);
-    if (rc) return rc;
-    out = (const float*)z;
-  }
-  void *dz = nullptr, *Xs = nullptr, *Xt = nullptr, *A = nullptr, *cnt = nullptr, *dXs = nullptr, *Wp = nullptr,
-       *W2T = nullptr, *part = nullptr;
-  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &dz);
-  if (rc) return rc;
+  void *Xs = nullptr, *Xt = nullptr, *A = nullptr, *cnt = nullptr, *dXs = nullptr, *Wp = nullptr, *W2T = nullptr,
+       *part = nullptr;
   rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &Xs);   // the forward's slots for Xs, Xt, A, Wcat, W2
   if (rc) return rc;
   rc = batch_scratch(b, 5, (size_t)V * LH * sizeof(float), &A);      // A, then dA
@@ -1011,27 +1016,22 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
     rc = batch_scratch(b, 11, (size_t)V * LH * sizeof(float), &cnt);   // cnt, then dXt
     if (rc) return rc;
   }
-  const int chunks = (int)((V + kTnChunk - 1) / kTnChunk), chunks_s = (int)((Vs + kTnChunk - 1) / kTnChunk);
   {
-    const size_t a = (size_t)chunks * LH * H, c = (size_t)chunks_s * D * H;
+    const size_t a = tn_partial_floats(V, LH, H), c = tn_partial_floats(Vs, D, H);
     rc = batch_scratch(b, 9, (a > c ? a : c) * sizeof(float), &part);
     if (rc) return rc;
   }
 
-  // 1b. dZ = dOut * act'(out) * rn(v)
-  act_grad_kernel<<<grid_cap(V * H), 256, 0, st>>>(grad_out, out, V, H, activation, b->row_ptr, L,
-                                                   agg_row_norm(aggregation), (float*)dz);
-  TFGNN_LAUNCH_CHECK();
   // 2. Xs, Xt and A_l (+ cnt_l) recomputed with the forward's GEMMs and summation order
   GemmEpilogue none;
   rc = launch_pack_horizontal(us, L, 0, D, H, H, (float*)Wp, LH, st);
   if (rc) return rc;
-  rc = node_gemm(h, D, (const float*)Wp, LH, (float*)Xs, LH, Vs, LH, D, none, TFGNN_PATH_AUTO, b, 6, st);
+  rc = node_gemm(h, D, (const float*)Wp, LH, (float*)Xs, LH, Vs, LH, D, none, TFGNN_PATH_AUTO, b, st);
   if (rc) return rc;
   if (use_target) {
     rc = launch_pack_horizontal(us, L, D, D, H, H, (float*)Wp, LH, st);
     if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Wp, LH, (float*)Xt, LH, V, LH, D, none, TFGNN_PATH_AUTO, b, 6, st);
+    rc = node_gemm(h_tgt, D, (const float*)Wp, LH, (float*)Xt, LH, V, LH, D, none, TFGNN_PATH_AUTO, b, st);
     if (rc) return rc;
     rc = launch_hidden_relu_count((const float*)Xs, (const float*)Xt, b->row_ptr, b->src_sorted, (int)V, L, H, normalize,
                                   (float*)A, (float*)cnt, st);
@@ -1046,20 +1046,13 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
     if (rc) return rc;
   }
   // 3. dW2_l = A_l^T dZ
-  {
-    dim3 grid((LH + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
-    gemm_tn_partial_kernel<<<grid, 256, 0, st>>>((const float*)A, LH, (const float*)dz, H, V, LH, H, (float*)part);
-    TFGNN_LAUNCH_CHECK();
-    reduce_partials_kernel<<<grid_cap((long long)LH * H), 256, 0, st>>>((const float*)part, chunks, L, H, H, gw2);
-    TFGNN_LAUNCH_CHECK();
-  }
+  rc = weight_grad((const float*)A, LH, dz, H, V, LH, H, (float*)part, gw2, L, H, 0, st);
+  if (rc) return rc;
   // 4. dA = dZ [W2_0; ..]^T (overwrites A), dA_l[v] *= s_{v,l}
-  pack_transposed_kernel<<<grid_cap((long long)LH * H), 256, 0, st>>>(w2, L, H, H, (float*)W2T);   // [H, LH]
-  TFGNN_LAUNCH_CHECK();
-  rc = node_gemm((const float*)dz, H, (const float*)W2T, LH, (float*)A, LH, V, LH, H, none, TFGNN_PATH_AUTO, b, 6, st);
+  rc = gemm_transposed(dz, H, {w2, L, H, H}, (float*)W2T, (float*)A, LH, V, LH, none, b, st);
   if (rc) return rc;
   if (normalize) {
-    scale_by_type_kernel<<<grid_cap(V * LH), 256, 0, st>>>((float*)A, LH, V, L, H, b->row_ptr);
+    scale_by_type_kernel<<<grid_for(V * LH), 256, 0, st>>>((float*)A, LH, V, L, H, b->row_ptr);
     TFGNN_LAUNCH_CHECK();
   }
   // 5. dXs over the source-keyed CSR (on a shard: its owned transpose, every global source, local target ids);
@@ -1068,52 +1061,28 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
                                   (int)Vs, L, H, (float*)dXs, st);
   if (rc) return rc;
   if (use_target) {
-    mul_inplace_kernel<<<grid_cap(V * LH), 256, 0, st>>>((float*)cnt, (const float*)A, V * LH);
+    mul_inplace_kernel<<<grid_for(V * LH), 256, 0, st>>>((float*)cnt, (const float*)A, V * LH);
     TFGNN_LAUNCH_CHECK();
   }
   // 6. dU^s_l = h^T dXs_l over all Vs rows, dU^t_l = h_v^T dXt_l over the owned rows (rows [D, 2D) of U_l)
   for (int l = 0; l < L; ++l) {
-    PtrTable gu{};
-    gu.p[0] = grad_weights[2 * l];
-    dim3 grid_s((D + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks_s);
-    gemm_tn_partial_kernel<<<grid_s, 256, 0, st>>>(h, D, (const float*)dXs + (size_t)l * H, LH, Vs, D, H, (float*)part);
-    TFGNN_LAUNCH_CHECK();
-    reduce_partials_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>((const float*)part, chunks_s, 1, D, H, gu);
-    TFGNN_LAUNCH_CHECK();
+    const PtrTable gu = one_table(grad_weights[2 * l]);
+    rc = weight_grad(h, D, (const float*)dXs + (size_t)l * H, LH, Vs, D, H, (float*)part, gu, 1, D, 0, st);
+    if (rc) return rc;
     if (use_target) {
-      dim3 grid_t((D + kTnTile - 1) / kTnTile, (H + kTnTile - 1) / kTnTile, chunks);
-      gemm_tn_partial_kernel<<<grid_t, 256, 0, st>>>(h_tgt, D, (const float*)cnt + (size_t)l * H, LH, V, D, H,
-                                                     (float*)part);
-      TFGNN_LAUNCH_CHECK();
-      reduce_partials_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>((const float*)part, chunks, 1, D, H, gu, 0, 0, D);
-      TFGNN_LAUNCH_CHECK();
+      rc = weight_grad(h_tgt, D, (const float*)cnt + (size_t)l * H, LH, V, D, H, (float*)part, gu, 1, D, D, st);
+      if (rc) return rc;
     }
   }
   if (!grad_h) return 0;
   // 7. grad_h = dXs [U^s_0^T; ..] (K = L*H), then the owned rows += dXt [U^t_0^T; ..]
-  for (int l = 0; l < L; ++l) {
-    PtrTable ul{};
-    ul.p[0] = mlp_weights[2 * l];
-    pack_transposed_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>(ul, 1, D, H, (float*)Wp + (size_t)l * H * D, D);
-    TFGNN_LAUNCH_CHECK();
-  }
-  rc = node_gemm((const float*)dXs, LH, (const float*)Wp, D, grad_h, D, Vs, D, LH, none, TFGNN_PATH_AUTO, b, 6, st);
-  if (rc) return rc;
-  if (use_target) {
-    for (int l = 0; l < L; ++l) {
-      PtrTable ul{};
-      ul.p[0] = mlp_weights[2 * l];
-      pack_transposed_kernel<<<grid_cap((long long)D * H), 256, 0, st>>>(ul, 1, D, H, (float*)Wp + (size_t)l * H * D, D,
-                                                                         0, D);
-      TFGNN_LAUNCH_CHECK();
-    }
-    GemmEpilogue acc;
-    acc.accumulate = 1;
-    rc = node_gemm((const float*)cnt, LH, (const float*)Wp, D, grad_h + (size_t)lo * D, D, V, D, LH, acc,
-                   TFGNN_PATH_AUTO, b, 6, st);
-    if (rc) return rc;
-  }
-  return 0;
+  rc = gemm_transposed((const float*)dXs, LH, {us, L, D, H, 1, 0, /*stacked=*/true}, (float*)Wp, grad_h, D, Vs, D, none,
+                       b, st);
+  if (rc || !use_target) return rc;
+  GemmEpilogue acc;
+  acc.accumulate = 1;
+  return gemm_transposed((const float*)cnt, LH, {us, L, D, H, 1, D, /*stacked=*/true}, (float*)Wp, grad_h + (size_t)lo * D,
+                         D, V, D, acc, b, st);
 }
 
 // =====================================================================================================================
@@ -1122,14 +1091,6 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
 // tf.GradientTape (models/graph_task_model.py:338-365).
 // =====================================================================================================================
 namespace tfgnn {
-
-// dZ = dY * act'(.) for a Dense layer: derivative from the OUTPUT (every activation but gelu) or from the recomputed
-// pre-activation (gelu).
-__global__ void dense_act_grad_kernel(const float* __restrict__ g, const float* __restrict__ y, long long n, int act,
-                                      float* __restrict__ dz) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    dz[i] = g[i] * (act == TFGNN_ACT_GELU ? gelu_grad_from_input(y[i]) : act_grad_from_output(y[i], act));
-}
 
 // LayerNormalization backward, one warp per row:
 //   xhat = (x - mean) * rstd;  dxhat = g * gamma;
@@ -1221,21 +1182,6 @@ __global__ void axpby_kernel(const float* __restrict__ a, float alpha, const flo
     out[i] = b ? alpha * a[i] + beta * b[i] : alpha * a[i];
 }
 
-// column sums of X [V, N] in fixed-order chunks -> out [N]   (bias / gamma / beta gradients)
-static int column_sums(const float* X, long long V, int N, float* out, cudaStream_t st) {
-  const int chunks = (int)((V + kTnChunk - 1) / kTnChunk);
-  void* part = nullptr;
-  int rc = pool_alloc(&part, (size_t)chunks * N * sizeof(float), st);
-  if (rc) return rc;
-  dim3 grid((N + 127) / 128, chunks);
-  colsum_partial_kernel<<<grid, 128, 0, st>>>(X, V, N, (float*)part);
-  TFGNN_LAUNCH_CHECK();
-  colsum_reduce_kernel<<<(N + 127) / 128, 128, 0, st>>>((const float*)part, chunks, N, out);
-  TFGNN_LAUNCH_CHECK();
-  pool_free(part, st);
-  return 0;
-}
-
 }  // namespace tfgnn
 
 // Backward of out = act(x W + bias): grad_x = dZ W^T (tensor-core GEMM), grad_W = x^T dZ (TN GEMM, fixed-order partials),
@@ -1252,49 +1198,33 @@ extern "C" int tfgnn_b200_dense_bwd(const float* x, const float* W, const float*
     return 0;
   }
   TFGNN_REQUIRE(x && W && out && grad_out, "NULL pointer");
-  void *dz = nullptr, *pre = nullptr, *wT = nullptr, *part = nullptr;
-  int rc = pool_alloc(&dz, (size_t)V * N * sizeof(float), st);
+  PoolBuffer dz{st}, pre{st};
+  int rc = dz.alloc((size_t)V * N * sizeof(float));
   if (rc) return rc;
   const float* y = out;
   if (activation == TFGNN_ACT_GELU) {   // derivative needs the pre-activation: recompute x W + bias
-    rc = pool_alloc(&pre, (size_t)V * N * sizeof(float), st);
-    if (!rc) rc = tfgnn_b200_dense_bias_fwd(x, W, bias, (float*)pre, V, K, N, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, stream);
-    if (rc) { pool_free(dz, st); pool_free(pre, st); return rc; }
-    y = (const float*)pre;
+    rc = pre.alloc((size_t)V * N * sizeof(float));
+    if (!rc) rc = tfgnn_b200_dense_bias_fwd(x, W, bias, pre.f(), V, K, N, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, stream);
+    if (rc) return rc;
+    y = pre.f();
   }
-  dense_act_grad_kernel<<<grid_cap(V * N), 256, 0, st>>>(grad_out, y, V * N, activation, (float*)dz);
-  g_launch_count.fetch_add(1);
+  rc = tfgnn_b200_activation_bwd(y, grad_out, V * N, activation, dz.f(), stream);
+  if (rc) return rc;
   if (grad_W) {
-    const int chunks = (int)((V + kTnChunk - 1) / kTnChunk);
-    rc = pool_alloc(&part, (size_t)chunks * K * N * sizeof(float), st);
-    if (!rc) {
-      PtrTable gt{};
-      gt.p[0] = grad_W;
-      dim3 grid((K + kTnTile - 1) / kTnTile, (N + kTnTile - 1) / kTnTile, chunks);
-      gemm_tn_partial_kernel<<<grid, 256, 0, st>>>(x, K, (const float*)dz, N, V, K, N, (float*)part);
-      g_launch_count.fetch_add(1);
-      reduce_partials_kernel<<<grid_cap((long long)K * N), 256, 0, st>>>((const float*)part, chunks, 1, K, N, gt);
-      g_launch_count.fetch_add(1);
-    }
+    PoolBuffer part{st};
+    rc = part.alloc(tn_partial_floats(V, K, N) * sizeof(float));
+    if (!rc) rc = weight_grad(x, K, dz.f(), N, V, K, N, part.f(), one_table(grad_W), 1, K, 0, st);
+    if (rc) return rc;
   }
-  if (!rc && grad_bias) rc = column_sums((const float*)dz, V, N, grad_bias, st);
-  if (!rc && grad_x) {
-    rc = pool_alloc(&wT, (size_t)N * K * sizeof(float), st);
-    if (!rc) {
-      PtrTable wt{};
-      wt.p[0] = W;
-      pack_transposed_kernel<<<grid_cap((long long)K * N), 256, 0, st>>>(wt, 1, K, N, (float*)wT);   // [N, K]
-      g_launch_count.fetch_add(1);
-      rc = tfgnn_b200_dense_fwd((const float*)dz, (const float*)wT, grad_x, V, N, K, TFGNN_ACT_NONE, TFGNN_PATH_AUTO,
-                                stream);
-    }
+  if (grad_bias) {
+    rc = column_sums(dz.f(), V, N, grad_bias, nullptr, st);
+    if (rc) return rc;
   }
-  if (!rc) rc = check_cuda(cudaGetLastError(), "dense_bwd kernels", __FILE__, __LINE__);
-  pool_free(dz, st);
-  pool_free(pre, st);
-  pool_free(wT, st);
-  pool_free(part, st);
-  return rc;
+  if (!grad_x) return 0;
+  PoolBuffer wT{st};
+  rc = wT.alloc((size_t)N * K * sizeof(float));
+  if (rc) return rc;
+  return gemm_transposed(dz.f(), N, {one_table(W), 1, K, N}, wT.f(), grad_x, K, V, K, GemmEpilogue{}, nullptr, st);
 }
 
 extern "C" int tfgnn_b200_layer_norm_bwd(const float* x, const float* gamma, const float* grad_out, int64_t V, int32_t H,
@@ -1308,16 +1238,16 @@ extern "C" int tfgnn_b200_layer_norm_bwd(const float* x, const float* gamma, con
     return 0;
   }
   TFGNN_REQUIRE(x && gamma && grad_out, "NULL pointer");
-  void* t = nullptr;
-  int rc = pool_alloc(&t, (size_t)V * H * sizeof(float), st);
+  PoolBuffer t{st};
+  int rc = t.alloc((size_t)V * H * sizeof(float));
   if (rc) return rc;
-  layer_norm_bwd_kernel<<<ceil_div(V * 32, 256), 256, 0, st>>>(x, gamma, grad_out, V, H, epsilon, grad_x, (float*)t);
-  g_launch_count.fetch_add(1);
-  rc = check_cuda(cudaGetLastError(), "layer_norm_bwd_kernel", __FILE__, __LINE__);
-  if (!rc && grad_gamma) rc = column_sums((const float*)t, V, H, grad_gamma, st);
-  if (!rc && grad_beta) rc = column_sums(grad_out, V, H, grad_beta, st);
-  pool_free(t, st);
-  return rc;
+  layer_norm_bwd_kernel<<<ceil_div(V * 32, 256), 256, 0, st>>>(x, gamma, grad_out, V, H, epsilon, grad_x, t.f());
+  TFGNN_LAUNCH_CHECK();
+  if (grad_gamma) {
+    rc = column_sums(t.f(), V, H, grad_gamma, nullptr, st);
+    if (rc) return rc;
+  }
+  return grad_beta ? column_sums(grad_out, V, H, grad_beta, nullptr, st) : 0;
 }
 
 // tf.nn.dropout (gnn.py:285-289, graph_global_exchange.py:98-101).  The mask is a pure function of (seed, offset, element
@@ -1327,7 +1257,7 @@ extern "C" int tfgnn_b200_dropout(const float* x, int64_t n, float rate, uint64_
   TFGNN_REQUIRE(n >= 0 && rate >= 0.0f && rate < 1.0f, "dropout rate must lie in [0, 1)");
   if (n == 0) return 0;
   TFGNN_REQUIRE(x && out, "NULL pointer");
-  dropout_kernel<<<grid_cap((n + 3) / 4), 256, 0, (cudaStream_t)stream>>>(x, n, rate, seed, offset, out);
+  dropout_kernel<<<grid_for((n + 3) / 4), 256, 0, (cudaStream_t)stream>>>(x, n, rate, seed, offset, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -1337,7 +1267,7 @@ extern "C" int tfgnn_b200_axpby(const float* a, float alpha, const float* b, flo
   TFGNN_REQUIRE(n >= 0, "negative size");
   if (n == 0) return 0;
   TFGNN_REQUIRE(a && out, "NULL pointer");
-  axpby_kernel<<<grid_cap(n), 256, 0, (cudaStream_t)stream>>>(a, alpha, b, beta, n, out);
+  axpby_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(a, alpha, b, beta, n, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }

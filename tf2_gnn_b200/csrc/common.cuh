@@ -59,6 +59,25 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   }
 }
 
+// act'(x) from the OUTPUT y = act(x), for every activation but gelu
+__device__ __forceinline__ float act_grad_from_output(float y, int act) {
+  switch (act) {
+    case TFGNN_ACT_RELU: return y > 0.f ? 1.f : 0.f;
+    case TFGNN_ACT_TANH: return 1.f - y * y;
+    case TFGNN_ACT_LEAKY_RELU: return y > 0.f ? 1.f : kLeakyReluAlpha;
+    case TFGNN_ACT_ELU: return y > 0.f ? 1.f : y + 1.f;                               // d/dx (e^x - 1) = y + 1
+    case TFGNN_ACT_SELU: return y > 0.f ? kSeluScale : y + kSeluScale * kSeluAlpha;   // scale*alpha*e^x = y + scale*alpha
+    case TFGNN_ACT_SIGMOID: return y * (1.f - y);
+    default: return 1.f;
+  }
+}
+// gelu (tanh approximation) is not invertible from its output: its derivative comes from the PRE-activation x
+__device__ __forceinline__ float gelu_grad_from_input(float x) {
+  const float c = 0.7978845608028654f;
+  const float t = tanhf(c * (x + 0.044715f * x * x * x));
+  return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * c * (1.0f + 3.0f * 0.044715f * x * x);
+}
+
 template <int ACT>
 __device__ __forceinline__ float apply_act_t(float x) {
   return apply_act(x, ACT);
@@ -108,6 +127,12 @@ struct CountTable {
 };
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// Blocks of 256 threads for a grid-stride loop over n items: at most 32 per SM of the H100's 132.
+inline int grid_for(long long n) {
+  const int g = ceil_div(n, 256);
+  return g < 1 ? 1 : (g > 132 * 32 ? 132 * 32 : g);
+}
 
 }  // namespace tfgnn
 

@@ -105,11 +105,6 @@ __global__ void layer_norm_kernel(const float* __restrict__ x, const float* __re
   for (int c = lane; c < H; c += 32) out[row * H + c] = (xr[c] - mean) * inv * gamma[c] + beta[c];
 }
 
-static int grid_for(long long n, int cap = 132 * 32) {
-  int b = ceil_div(n, 256);
-  return b < 1 ? 1 : (b > cap ? cap : b);
-}
-
 }  // namespace tfgnn
 
 using namespace tfgnn;
@@ -193,28 +188,11 @@ extern "C" int tfgnn_b200_layer_norm(const float* x, const float* gamma, const f
 // one TensorFlow op of that sequence.
 namespace tfgnn {
 
-__device__ __forceinline__ float act_grad_out(float y, int act) {   // derivative from the OUTPUT y = act(x)
-  switch (act) {
-    case TFGNN_ACT_RELU: return y > 0.f ? 1.f : 0.f;
-    case TFGNN_ACT_TANH: return 1.f - y * y;
-    case TFGNN_ACT_LEAKY_RELU: return y > 0.f ? 1.f : kLeakyReluAlpha;
-    case TFGNN_ACT_ELU: return y > 0.f ? 1.f : y + 1.f;
-    case TFGNN_ACT_SELU: return y > 0.f ? kSeluScale : y + kSeluScale * kSeluAlpha;
-    case TFGNN_ACT_SIGMOID: return y * (1.f - y);
-    default: return 1.f;
-  }
-}
-__device__ __forceinline__ float gelu_grad_in(float x) {            // gelu: derivative from the INPUT
-  const float c = 0.7978845608028654f;
-  const float t = tanhf(c * (x + 0.044715f * x * x * x));
-  return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * c * (1.0f + 3.0f * 0.044715f * x * x);
-}
-
 // grad_in = grad_out * act'(.): `ref` is the forward OUTPUT for every activation but gelu, whose `ref` is the forward INPUT
 __global__ void activation_bwd_kernel(const float* __restrict__ ref, const float* __restrict__ g, long long n, int act,
                                       float* __restrict__ out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    out[i] = g[i] * (act == TFGNN_ACT_GELU ? gelu_grad_in(ref[i]) : act_grad_out(ref[i], act));
+    out[i] = g[i] * (act == TFGNN_ACT_GELU ? gelu_grad_from_input(ref[i]) : act_grad_from_output(ref[i], act));
 }
 
 // out[m, :] = x[m, :] * f(s[m]),  f = s (mode 0), 1/(s + 1e-7) (mode 1: gnn_edge_mlp.py:102-106), 1/max(s,1) (mode 2:
@@ -372,35 +350,6 @@ __global__ void head_dot_kernel(const float* __restrict__ a, const float* __rest
   }
 }
 
-// Keras GRUCell(reset_after=True) gate backward given gx = inputs K + b0, gh = h U + b1 (not modified): dgx, dgh, and the
-// direct path dL/dh' * z through the convex combination.
-__global__ void gru_gate_bwd_out_kernel(const float* __restrict__ gx, const float* __restrict__ gh, const float* __restrict__ h,
-                                        const float* __restrict__ grad_out, long long V, int H, float* __restrict__ dgx,
-                                        float* __restrict__ dgh, float* __restrict__ dh_direct) {
-  const long long total = V * H;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const long long v = i / H;
-    const int c = (int)(i - v * H);
-    const float* x = gx + v * 3 * H;
-    const float* y = gh + v * 3 * H;
-    const float ghh = y[2 * H + c];
-    const float z = 1.0f / (1.0f + expf(-(x[c] + y[c])));
-    const float r = 1.0f / (1.0f + expf(-(x[H + c] + y[H + c])));
-    const float hh = tanhf(x[2 * H + c] + r * ghh);
-    const float g = grad_out[i];
-    const float da = g * (1.0f - z) * (1.0f - hh * hh);
-    const float daz = g * (h[i] - hh) * z * (1.0f - z);
-    const float dar = da * ghh * r * (1.0f - r);
-    float* ox = dgx + v * 3 * H;
-    float* oy = dgh + v * 3 * H;
-    ox[c] = daz;          oy[c] = daz;
-    ox[H + c] = dar;      oy[H + c] = dar;
-    ox[2 * H + c] = da;   oy[2 * H + c] = da * r;
-    dh_direct[i] = g * z;
-  }
-}
-
 }  // namespace tfgnn
 
 extern "C" int tfgnn_b200_softmax_apply(const float* scores, const float* seg_max_per_elem, const float* seg_sum_per_elem,
@@ -429,18 +378,6 @@ extern "C" int tfgnn_b200_head_dot(const float* a, const float* b, int64_t M, in
   if (M == 0) return 0;
   TFGNN_REQUIRE(a && b && out, "NULL pointer");
   head_dot_kernel<<<grid_for(M * num_heads), 256, 0, (cudaStream_t)stream>>>(a, b, M, num_heads, head_dim, out);
-  TFGNN_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" int tfgnn_b200_gru_gate_bwd(const float* gx, const float* gh, const float* h, const float* grad_out,
-                                       int64_t num_rows, int32_t H, float* grad_gx, float* grad_gh, float* grad_h_direct,
-                                       void* stream) {
-  TFGNN_REQUIRE(num_rows >= 0 && H > 0, "bad gru_gate_bwd sizes");
-  if (num_rows == 0) return 0;
-  TFGNN_REQUIRE(gx && gh && h && grad_out && grad_gx && grad_gh && grad_h_direct, "NULL pointer");
-  gru_gate_bwd_out_kernel<<<grid_for(num_rows * H), 256, 0, (cudaStream_t)stream>>>(gx, gh, h, grad_out, num_rows, H,
-                                                                                   grad_gx, grad_gh, grad_h_direct);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }

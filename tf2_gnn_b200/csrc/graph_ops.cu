@@ -8,7 +8,6 @@
 //   segment_softmax         per (graph, head): w = exp((s - max) - log(sum exp(s - max)))   dpu_utils unsorted_segment_softmax
 //   weighted_segment_sum    out[g, k*d + c] = sum_{v in g} w[v,k] * r[v, k*d + c]   (or plain sum / mean)
 //   gathered_add            out[v] = act((a[v] + b[index[v]]) * scale)              exchange combine (mean, MLP hidden)
-//   gru_gate                Keras GRUCell gate math with the input-side pre-activations indexed per row
 //   dense_bias_fwd          Dense with bias (readout MLPs with use_biases, GRU cell halves)
 // All HBM-bound and tiny next to the message-passing layers; deterministic (fixed reduction orders).
 #include "layers.cuh"
@@ -95,25 +94,6 @@ __global__ void gathered_add_kernel(const float* __restrict__ a, const float* __
   }
 }
 
-// Keras GRUCell(reset_after=True) gates; the input-side pre-activations gx live in a table indexed per row
-// (graph-level gx gathered by node_to_graph_map: the GRU exchange computes graph_repr K + b0 once per GRAPH).
-__global__ void gru_gate_indexed_kernel(const float* __restrict__ gx, const int* __restrict__ gx_index,
-                                        const float* __restrict__ gh, const float* __restrict__ h, long long V, int H,
-                                        float* __restrict__ out) {
-  const long long total = V * H;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const long long v = i / H;
-    const int c = (int)(i - v * H);
-    const float* x = gx + (gx_index ? (long long)__ldg(gx_index + v) : v) * 3 * H;
-    const float* r_ = gh + v * 3 * H;
-    const float z = 1.0f / (1.0f + expf(-(x[c] + r_[c])));
-    const float r = 1.0f / (1.0f + expf(-(x[H + c] + r_[H + c])));
-    const float hh = tanhf(x[2 * H + c] + r * r_[2 * H + c]);
-    out[i] = z * h[i] + (1.0f - z) * hh;
-  }
-}
-
 __global__ void clamp_kernel(float* __restrict__ x, long long n, float lo, float hi, int has_lo, int has_hi) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float v = x[i];
@@ -121,11 +101,6 @@ __global__ void clamp_kernel(float* __restrict__ x, long long n, float lo, float
     if (has_hi) v = fminf(v, hi);
     x[i] = v;
   }
-}
-
-static int go_grid(long long n) {
-  int g = ceil_div(n, 256);
-  return g < 1 ? 1 : (g > 132 * 32 ? 132 * 32 : g);
 }
 
 }  // namespace tfgnn
@@ -142,7 +117,7 @@ extern "C" int tfgnn_b200_graph_offsets(const int32_t* node_to_graph_map, int64_
   int rc = pool_alloc((void**)&bad, sizeof(int), st);
   if (rc) return rc;
   TFGNN_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
-  graph_offsets_kernel<<<go_grid(num_nodes + 1), 256, 0, st>>>(node_to_graph_map, num_nodes, num_graphs, graph_ptr, bad);
+  graph_offsets_kernel<<<grid_for(num_nodes + 1), 256, 0, st>>>(node_to_graph_map, num_nodes, num_graphs, graph_ptr, bad);
   TFGNN_LAUNCH_CHECK();
   int host_bad = 0;
   if (validate) {
@@ -190,19 +165,8 @@ extern "C" int tfgnn_b200_gathered_add(const float* a, const float* b, const int
   TFGNN_REQUIRE(num_rows >= 0 && H > 0 && valid_act(activation), "bad gathered_add arguments");
   if (num_rows == 0) return 0;
   TFGNN_REQUIRE(a && b && out, "NULL pointer");
-  gathered_add_kernel<<<go_grid(num_rows * H), 256, 0, (cudaStream_t)stream>>>(a, b, index, num_rows, H, scale,
+  gathered_add_kernel<<<grid_for(num_rows * H), 256, 0, (cudaStream_t)stream>>>(a, b, index, num_rows, H, scale,
                                                                               activation, out);
-  TFGNN_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" int tfgnn_b200_gru_gate_fwd(const float* gx, const int32_t* gx_row_index, const float* gh, const float* h,
-                                       int64_t num_rows, int32_t H, float* out, void* stream) {
-  TFGNN_REQUIRE(num_rows >= 0 && H > 0, "bad gru_gate sizes");
-  if (num_rows == 0) return 0;
-  TFGNN_REQUIRE(gx && gh && h && out, "NULL pointer");
-  gru_gate_indexed_kernel<<<go_grid(num_rows * H), 256, 0, (cudaStream_t)stream>>>(gx, gx_row_index, gh, h, num_rows,
-                                                                                  H, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -212,7 +176,7 @@ extern "C" int tfgnn_b200_clamp(float* x, int64_t n, float lower, float upper, i
   TFGNN_REQUIRE(n >= 0, "negative size");
   if (n == 0 || (!has_lower && !has_upper)) return 0;
   TFGNN_REQUIRE(x != nullptr, "NULL pointer");
-  clamp_kernel<<<go_grid(n), 256, 0, (cudaStream_t)stream>>>(x, n, lower, upper, has_lower, has_upper);
+  clamp_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(x, n, lower, upper, has_lower, has_upper);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }

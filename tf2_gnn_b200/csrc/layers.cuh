@@ -8,8 +8,10 @@ int unsupported(const std::string& msg);
 bool valid_act(int a);
 bool valid_agg(int a);
 int agg_row_norm(int aggregation);
+// the batch scratch slot that holds a GEMM's tensor-core-packed weights for the duration of that GEMM
+constexpr int kPackSlot = 6;
 int node_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int N, int K,
-              const GemmEpilogue& epi, int path, tfgnn_batch* batch, int tc_slot, cudaStream_t st);
+              const GemmEpilogue& epi, int path, tfgnn_batch* batch, cudaStream_t st);
 int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                   uint32_t flags, int aggregation, int activation, int path, float* out, int ldo, cudaStream_t st);
 // literal per-edge path (literal.cu); FB = optional FiLM table [V, L*2H] (gamma | beta per type)

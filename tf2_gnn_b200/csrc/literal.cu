@@ -105,11 +105,6 @@ __global__ void finalize_kernel(float* __restrict__ out, long long V, int H, int
   }
 }
 
-static int cap_grid(long long n) {
-  int g = ceil_div(n, 256);
-  return g < 1 ? 1 : (g > 132 * 32 ? 132 * 32 : g);
-}
-
 int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                      uint32_t flags, int aggregation, int activation, const float* FB, int ldf, int path, float* out,
                      int ldo, cudaStream_t st) {
@@ -135,14 +130,14 @@ int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* 
   if (rc) return rc;
   rc = batch_scratch(b, 4, (size_t)maxE * sizeof(int), &tgt_of);
   if (rc) return rc;
-  fill2d_kernel<<<cap_grid(V * H), 256, 0, st>>>(out, V, H, ldo, use_max ? kLowestFloat : 0.f);
+  fill2d_kernel<<<grid_for(V * H), 256, 0, st>>>(out, V, H, ldo, use_max ? kLowestFloat : 0.f);
   TFGNN_LAUNCH_CHECK();
   for (int l = 0; l < L; ++l) {
     const long long E = b->E[l];
     if (E == 0) continue;
-    expand_targets_kernel<<<cap_grid(V), 256, 0, st>>>(b->row_ptr, V, l, (int*)tgt_of);
+    expand_targets_kernel<<<grid_for(V), 256, 0, st>>>(b->row_ptr, V, l, (int*)tgt_of);
     TFGNN_LAUNCH_CHECK();
-    gather_concat_kernel<<<cap_grid(E * 32), 256, 0, st>>>(h, h_tgt, D, b->row_ptr, b->src_sorted, V, l,
+    gather_concat_kernel<<<grid_for(E * 32), 256, 0, st>>>(h, h_tgt, D, b->row_ptr, b->src_sorted, V, l,
                                                          (const int*)tgt_of, use_target, (float*)X0, D_in);
     TFGNN_LAUNCH_CHECK();
     float* cur = (float*)X0;
@@ -151,18 +146,18 @@ int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* 
     for (int i = 0; i < n_layers; ++i) {
       GemmEpilogue epi;
       epi.act = i < n_hidden ? TFGNN_ACT_RELU : TFGNN_ACT_NONE;   // dpu_utils MLP: ReLU hidden, linear output
-      rc = node_gemm(cur, k_in, mlp_weights[l * n_layers + i], H, nxt, H, E, H, k_in, epi, path, b, 6, st);
+      rc = node_gemm(cur, k_in, mlp_weights[l * n_layers + i], H, nxt, H, E, H, k_in, epi, path, b, st);
       if (rc) return rc;
       float* t = cur; cur = nxt; nxt = t;
       k_in = H;
     }
-    edge_post_kernel<<<cap_grid(E * H), 256, 0, st>>>(cur, H, b->row_ptr, V, l, (const int*)tgt_of, normalize, FB, ldf,
+    edge_post_kernel<<<grid_for(E * H), 256, 0, st>>>(cur, H, b->row_ptr, V, l, (const int*)tgt_of, normalize, FB, ldf,
                                                      act_before ? activation : TFGNN_ACT_NONE);
     TFGNN_LAUNCH_CHECK();
-    segment_reduce_sorted_kernel<<<cap_grid(V * H), 256, 0, st>>>(cur, H, b->row_ptr, V, l, use_max, out, ldo);
+    segment_reduce_sorted_kernel<<<grid_for(V * H), 256, 0, st>>>(cur, H, b->row_ptr, V, l, use_max, out, ldo);
     TFGNN_LAUNCH_CHECK();
   }
-  finalize_kernel<<<cap_grid(V * H), 256, 0, st>>>(out, V, H, ldo, b->row_ptr, L, agg_row_norm(aggregation),
+  finalize_kernel<<<grid_for(V * H), 256, 0, st>>>(out, V, H, ldo, b->row_ptr, L, agg_row_norm(aggregation),
                                                   act_before ? TFGNN_ACT_NONE : activation);
   TFGNN_LAUNCH_CHECK();
   return 0;

@@ -5,15 +5,16 @@ namespace tfgnn {
 
 // Keras GRUCell, reset_after=True (ggnn.py:84-87): gx = agg K + b0, gh = h U + b1 (both [V,3H]),
 // z = sigmoid(gx_z+gh_z), r = sigmoid(gx_r+gh_r), hh = tanh(gx_h + r*gh_h), h' = z*h + (1-z)*hh.
-__global__ void gru_gate_kernel(const float* __restrict__ gx, const float* __restrict__ gh,
-                                const float* __restrict__ h, int ldh, long long V, int H,
-                                float* __restrict__ out) {
+// gx_index (optional) picks row gx_index[v] of gx for row v: the GRU exchange computes graph_repr K + b0 once per GRAPH.
+// out may overlap h (an in-place state update): each thread reads its h element before it writes.
+__global__ void gru_gate_kernel(const float* __restrict__ gx, const int* __restrict__ gx_index,
+                                const float* __restrict__ gh, const float* h, int ldh, long long V, int H, float* out) {
   const long long total = V * H;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const long long v = i / H;
     const int c = (int)(i - v * H);
-    const float* x = gx + v * 3 * H;
+    const float* x = gx + (gx_index ? (long long)__ldg(gx_index + v) : v) * 3 * H;
     const float* r_ = gh + v * 3 * H;
     const float z = 1.0f / (1.0f + expf(-(x[c] + r_[c])));
     const float r = 1.0f / (1.0f + expf(-(x[H + c] + r_[H + c])));
@@ -58,7 +59,7 @@ extern "C" int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     const bool in_place = out < h + (size_t)b->V_src * D && h < out + (size_t)V * H;
     if (want && !in_place && gemm_tc_gru_supported(V, H, (const float*)agg, H, h_tgt0, D, out, H)) {
       void* packed = nullptr;
-      rc = batch_scratch(b, 6, gemm_tc_gru_packed_bytes(H), &packed);
+      rc = batch_scratch(b, kPackSlot, gemm_tc_gru_packed_bytes(H), &packed);
       if (rc) return rc;
       return launch_gemm_tc_gru((const float*)agg, H, h_tgt0, D, gru_kernel, gru_recurrent_kernel, gru_bias, (float*)packed,
                                 out, H, V, H, st);
@@ -71,14 +72,22 @@ extern "C" int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   GemmEpilogue ex, eh;
   ex.bias = gru_bias;
   eh.bias = gru_bias + 3 * H;
-  rc = node_gemm((const float*)agg, H, gru_kernel, 3 * H, (float*)gx, 3 * H, V, 3 * H, H, ex, path, b, 6, st);
+  rc = node_gemm((const float*)agg, H, gru_kernel, 3 * H, (float*)gx, 3 * H, V, 3 * H, H, ex, path, b, st);
   if (rc) return rc;
   const float* h_tgt = h + (size_t)b->tgt_off * D;
-  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, 3 * H, (float*)gh, 3 * H, V, 3 * H, H, eh, path, b, 6, st);
+  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, 3 * H, (float*)gh, 3 * H, V, 3 * H, H, eh, path, b, st);
   if (rc) return rc;
-  int blocks = ceil_div(V * H, 256);
-  if (blocks > 132 * 32) blocks = 132 * 32;
-  gru_gate_kernel<<<blocks, 256, 0, st>>>((const float*)gx, (const float*)gh, h_tgt, D, V, H, out);
+  gru_gate_kernel<<<grid_for(V * H), 256, 0, st>>>((const float*)gx, nullptr, (const float*)gh, h_tgt, D, V, H, out);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int tfgnn_b200_gru_gate_fwd(const float* gx, const int32_t* gx_row_index, const float* gh, const float* h,
+                                       int64_t num_rows, int32_t H, float* out, void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && H > 0, "bad gru_gate sizes");
+  if (num_rows == 0) return 0;
+  TFGNN_REQUIRE(gx && gh && h && out, "NULL pointer");
+  gru_gate_kernel<<<grid_for(num_rows * H), 256, 0, (cudaStream_t)stream>>>(gx, gx_row_index, gh, h, H, num_rows, H, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -117,7 +126,7 @@ extern "C" int tfgnn_b200_rgin_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     GemmEpilogue epi;
     epi.act = last ? activation : TFGNN_ACT_RELU;
     float* dst = last ? out : nxt;
-    rc = node_gemm(cur, H, aggr_weights[i], H, dst, H, V, H, H, epi, path, b, 6, st);
+    rc = node_gemm(cur, H, aggr_weights[i], H, dst, H, V, H, H, epi, path, b, st);
     if (rc) return rc;
     float* t = cur; cur = nxt; nxt = t;
     if (!last) cur = dst;
@@ -201,7 +210,7 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     if (rc) return rc;
     GemmEpilogue raw;
     raw.finalize = 0;
-    rc = node_gemm((const float*)T, K, (const float*)Fb, H, out, H, V, H, K, raw, path, b, 6, st);
+    rc = node_gemm((const float*)T, K, (const float*)Fb, H, out, H, V, H, K, raw, path, b, st);
     if (rc) return rc;
     if (use_target && normalize) {   // coeff(v,l) h_v with the normalised coefficient (the beta operand used the raw count)
       rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, 1, (float*)T, K, 0, st);
@@ -218,7 +227,7 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     if (rc) return rc;
     rc = launch_pack_horizontal(film, L, 0, D, H, 2 * H, (float*)Fg, LHw, st);   // first H columns of every F_l [D, 2H]
     if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Fg, LHw, (float*)Gall, LHw, V, LHw, D, none, path, b, 6, st);
+    rc = node_gemm(h_tgt, D, (const float*)Fg, LHw, (float*)Gall, LHw, V, LHw, D, none, path, b, st);
     if (rc) return rc;
     for (int l = 0; l < L; ++l) {
       GemmEpilogue chain;
@@ -232,7 +241,7 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
         chain.row_norm = agg_row_norm(aggregation); chain.row_ptr = b->row_ptr; chain.V = V; chain.L = L;
       }
       rc = node_gemm((const float*)A + (size_t)l * D, K, reinterpret_cast<const float*>(first.p[l]), H, out, H, V, H, D,
-                     chain, path, b, 6, st);
+                     chain, path, b, st);
       if (rc) return rc;
       if (use_target) {
         if (l == L - 1) {
@@ -241,7 +250,7 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
           chain.row_norm = agg_row_norm(aggregation); chain.row_ptr = b->row_ptr; chain.V = V; chain.L = L;
         }
         rc = node_gemm((const float*)T + (size_t)l * D, K, reinterpret_cast<const float*>(first.p[l]) + (size_t)D * H, H,
-                       out, H, V, H, D, chain, path, b, 6, st);
+                       out, H, V, H, D, chain, path, b, st);
         if (rc) return rc;
       }
     }
@@ -259,7 +268,7 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     // hidden layers in the edge MLP: FiLM parameters at node level, messages on the literal per-edge path
     rc = launch_pack_horizontal(film, L, 0, D, 2 * H, 2 * H, (float*)Fcat, 2 * LH, st);
     if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Fcat, 2 * LH, (float*)FB, 2 * LH, V, 2 * LH, D, none, path, b, 6, st);
+    rc = node_gemm(h_tgt, D, (const float*)Fcat, 2 * LH, (float*)FB, 2 * LH, V, 2 * LH, D, none, path, b, st);
     if (rc) return rc;
     return edge_mlp_literal(b, h, D, mlp_weights, num_hidden_layers, H, flags, aggregation, activation,
                             (const float*)FB, 2 * LH, path, out, H, st);
@@ -267,20 +276,20 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   // projected source messages P_l = h W^s_l  (gnn_edge_mlp.py:100 hoisted to node level)
   rc = launch_pack_horizontal(first, L, 0, D, H, H, (float*)Wcat, LH, st);
   if (rc) return rc;
-  rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, 6, st);
+  rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
   if (rc) return rc;
   if (use_target) {
     rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Tt);
     if (rc) return rc;
     rc = launch_pack_horizontal(first, L, D, D, H, H, (float*)Wcat, LH, st);
     if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, 6, st);
+    rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, st);
     if (rc) return rc;
   }
   // FiLM parameters [gamma_l | beta_l] = h F_l depend on (target, type) only (gnn_film.py:99-103)
   rc = launch_pack_horizontal(film, L, 0, D, 2 * H, 2 * H, (float*)Fcat, 2 * LH, st);
   if (rc) return rc;
-  rc = node_gemm(h_tgt, D, (const float*)Fcat, 2 * LH, (float*)FB, 2 * LH, V, 2 * LH, D, none, path, b, 6, st);
+  rc = node_gemm(h_tgt, D, (const float*)Fcat, 2 * LH, (float*)FB, 2 * LH, V, 2 * LH, D, none, path, b, st);
   if (rc) return rc;
   EdgeReduceParams p;
   p.X = (const float*)P; p.ldx = LH; p.x_type_stride = H;
@@ -437,7 +446,7 @@ extern "C" int tfgnn_b200_rgat_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
       none.score_src = (float*)ss; none.score_tgt = (float*)stt; none.score_att = at;
       none.score_H = H; none.score_K = K; none.score_d = d;
     }
-    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, 6, st);
+    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
     if (rc) return rc;
     if (!fuse_scores) {
       const long long total = Vs * L * K;
