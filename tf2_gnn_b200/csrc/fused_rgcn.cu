@@ -655,10 +655,14 @@ fused_rgcn_rows_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
     const int cw = wg, t = threadIdx.x & 127;
     const uint32_t empty0_cta0 = ptx::mapa_shared(ptx::smem_u32(&empty[0]), 0u);
     const uint32_t empty0_cta1 = ptx::mapa_shared(ptx::smem_u32(&empty[0]), 1u);
-    auto release_stage = [&](int s) {   // one arrival per consumer warpgroup on the stage's barrier in BOTH CTAs
+    // One arrival per consumer warpgroup on the stage's barrier in BOTH CTAs.  A plain arrive: the stage's only readers are
+    // this warpgroup's retired MMAs (wgmma.wait_group 0), and its split stores were read by them, so nothing is left for a
+    // cluster-scope release to order before the producers' refill.  The release form costs a GPU-scope memory barrier per
+    // arrive (MEMBAR.ALL.GPU), which also waits for the epilogue stores and L2 discards still in flight.
+    auto release_stage = [&](int s) {
       if (t == 0) {
-        ptx::mbar_arrive_cluster_release(empty0_cta0 + (uint32_t)s * 8u);
-        ptx::mbar_arrive_cluster_release(empty0_cta1 + (uint32_t)s * 8u);
+        ptx::mbar_arrive_cluster(empty0_cta0 + (uint32_t)s * 8u);
+        ptx::mbar_arrive_cluster(empty0_cta1 + (uint32_t)s * 8u);
       }
     };
     HalfTileAcc<BN> c;
