@@ -7,7 +7,8 @@
 //     valid when the message is linear in h_u and the aggregation is sum/mean/sqrt_n with the
 //     activation after it (RGCN/GGNN defaults, every PPI/QM9 RGCN config).
 //   transform-then-aggregate  P = h [W_0|..|W_{L-1}];  out[v] = agg_{l,e} f(P_l[src_e], v, l)
-//     for max-aggregation / activation-before-aggregation (per-edge non-linearity).
+//     for max-aggregation / activation-before-aggregation (per-edge non-linearity); its backward
+//     (backward.cu) recomputes P through the same transform_aggregate_tables and differentiates f per edge.
 //   hoisted hidden layer      A_l[v] = scale * sum_e relu(U^s_l h_u + U^t_l h_v); out = act(A W2cat)
 #include <cstdlib>
 #include <mutex>
@@ -149,6 +150,45 @@ int agg_row_norm(int aggregation) {
   return aggregation == TFGNN_AGG_MEAN ? 1 : aggregation == TFGNN_AGG_SQRT_N ? 2 : 0;
 }
 
+// The node-level half of the transform-then-aggregate form (no hidden layer; max aggregation and / or activation before
+// aggregation): P = h [W_0|..|W_{L-1}] over the Vs source rows (slot 2) and, with target-state input, T = h_tgt [W^t_0|..]
+// over the owned rows (slot 4), W_l = W.p[l].  *p becomes the merged edge reduce that forms the layer from them, out / ldo
+// unset:  out[v] = act_final(agg_e act_edge((P_l[u] + T_l[v]) s)).  The backward recomputes both through this function.
+int transform_aggregate_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& W, int H, uint32_t flags,
+                               int aggregation, int activation, int path, EdgeReduceParams* p, cudaStream_t st) {
+  const int V = (int)b->V, Vs = (int)b->V_src, L = b->L, LH = L * H;
+  const bool act_before = flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION;
+  void *P = nullptr, *Tt = nullptr, *Wcat = nullptr;
+  int rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &P);
+  if (rc) return rc;
+  rc = batch_scratch(b, 3, (size_t)D * LH * sizeof(float), &Wcat);
+  if (rc) return rc;
+  rc = launch_pack_horizontal(W, L, 0, D, H, H, (float*)Wcat, LH, st);
+  if (rc) return rc;
+  GemmEpilogue none;
+  rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
+  if (rc) return rc;
+  if (flags & TFGNN_FLAG_USE_TARGET_STATE) {
+    rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Tt);
+    if (rc) return rc;
+    rc = launch_pack_horizontal(W, L, D, D, H, H, (float*)Wcat, LH, st);
+    if (rc) return rc;
+    rc = node_gemm(h + (size_t)b->tgt_off * D, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, st);
+    if (rc) return rc;
+  }
+  *p = EdgeReduceParams{};
+  p->X = (const float*)P; p->ldx = LH; p->x_type_stride = H;
+  p->T = (const float*)Tt; p->ldt = LH; p->t_type_stride = H;
+  p->row_ptr = b->row_ptr; p->src = b->src_sorted;
+  p->V = V; p->L = L; p->C = H;
+  p->normalize = (flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING) != 0;
+  p->edge_act = act_before ? activation : TFGNN_ACT_NONE;
+  p->reduce_max = aggregation == TFGNN_AGG_MAX;
+  p->row_norm = agg_row_norm(aggregation);
+  p->final_act = act_before ? TFGNN_ACT_NONE : activation;
+  return 0;
+}
+
 // Edge-MLP family core.  Writes act/agg result to out[V, ldo].
 int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights,
                          int n_hidden, int H, uint32_t flags, int aggregation, int activation, int path,
@@ -276,35 +316,10 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
 
   if (n_hidden == 0) {
     // ---- transform-then-aggregate (max aggregation and/or activation before aggregation) ----
-    const int LH = L * H;
-    void *P = nullptr, *Tt = nullptr, *Wcat = nullptr;
-    int rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &P);
-    if (rc) return rc;
-    rc = batch_scratch(b, 3, (size_t)D * LH * sizeof(float), &Wcat);
-    if (rc) return rc;
-    rc = launch_pack_horizontal(first, L, 0, D, H, H, (float*)Wcat, LH, st);
-    if (rc) return rc;
-    GemmEpilogue none;
-    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
-    if (rc) return rc;
-    if (use_target) {
-      rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Tt);
-      if (rc) return rc;
-      rc = launch_pack_horizontal(first, L, D, D, H, H, (float*)Wcat, LH, st);
-      if (rc) return rc;
-      rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, st);
-      if (rc) return rc;
-    }
     EdgeReduceParams p;
-    p.X = (const float*)P; p.ldx = LH; p.x_type_stride = H;
-    p.T = (const float*)Tt; p.ldt = LH; p.t_type_stride = H;
-    p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-    p.out = out; p.ldo = ldo; p.V = V; p.L = L; p.C = H;
-    p.normalize = normalize;
-    p.edge_act = act_before ? activation : TFGNN_ACT_NONE;
-    p.reduce_max = aggregation == TFGNN_AGG_MAX;
-    p.row_norm = row_norm;
-    p.final_act = act_before ? TFGNN_ACT_NONE : activation;
+    int rc = transform_aggregate_tables(b, h, D, first, H, flags, aggregation, activation, path, &p, st);
+    if (rc) return rc;
+    p.out = out; p.ldo = ldo;
     return launch_edge_reduce(p, /*merged=*/true, st);
   }
 

@@ -8,7 +8,8 @@
 //   dA      = dZ [W_0;..;W_{L-1}]^T, then dA_l[v] *= s_{v,l}   (3xTF32 wgmma GEMM + row/type scale)
 //   dh[u]   = sum_l sum_{(u,v) in A_l} dA_l[v]                (CSR reduce over the SOURCE-keyed CSR: no atomics)
 // Supported: 0 hidden layers, source or source+target state input, sum / mean / sqrt_n aggregation, activation after the
-// aggregation, every activation of the reference's table (gelu through a recomputed pre-activation).
+// aggregation, every activation of the reference's table (gelu through a recomputed pre-activation).  Max aggregation and
+// activation before the aggregation take the transform-then-aggregate backward (transform_aggregate_bwd, below).
 // On a target-range shard (DESIGN.md §6) everything but the dh reduce covers the owned rows only; the dh reduce runs over the
 // shard's TFGNN_PREPARE_TRANSPOSE_OWNED CSR (all global sources, local target ids), so each shard writes its contribution
 // to the full grad_h table and the contributions of all shards sum to the unsharded gradient.
@@ -18,9 +19,11 @@
 
 namespace tfgnn {
 
+// ties (max aggregation): the tie count n of every (v, c); dz is then divided by it, as tf.math.unsorted_segment_max's
+// gradient divides by its count (segment_max_bwd_kernel), and is 0 where n = 0 (a target without edges carries no gradient).
 __global__ void act_grad_kernel(const float* __restrict__ g, const float* __restrict__ out, long long V, int H,
                                 int act, const int* __restrict__ row_ptr, int L, int row_norm,
-                                float* __restrict__ dz) {
+                                float* __restrict__ dz, const float* __restrict__ ties = nullptr) {
   const long long total = V * H;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -33,7 +36,8 @@ __global__ void act_grad_kernel(const float* __restrict__ g, const float* __rest
       s = 1.f / (row_norm == 1 ? n : sqrtf(n));
     }
     // for gelu `out` holds the recomputed pre-activation
-    dz[i] = g[i] * (act == TFGNN_ACT_GELU ? gelu_grad_from_input(out[i]) : act_grad_from_output(out[i], act)) * s;
+    const float d = g[i] * (act == TFGNN_ACT_GELU ? gelu_grad_from_input(out[i]) : act_grad_from_output(out[i], act)) * s;
+    dz[i] = ties ? (ties[i] > 0.f ? d / ties[i] : 0.f) : d;
   }
 }
 
@@ -421,6 +425,87 @@ static int column_sums(const float* X, long long V, int N, float* out, float* pa
   return 0;
 }
 
+// Backward of the transform-then-aggregate form (no hidden layer, max aggregation and / or activation before aggregation;
+// DESIGN.md §6).  Per edge e = (u -> v) of type l: x_e = (P_l[u] + T_l[v]) s, y_e = act_edge(x_e), z[v] = agg_e y_e,
+// out = act_final(rn(v) z), with P = h [W_0|..], T = h_tgt [W^t_0|..] (target-state input, else 0):
+//   1. P, T recomputed by the forward's node GEMMs (transform_aggregate_tables); for max, z and the tie count n in one pass
+//      of the forward's edge reduce
+//   2. dZ = dOut * act_final'(z) / n  (max)   or   dOut * rn(v)  (sum / mean / sqrt_n: act_final is the identity)
+//   3. w_e = dZ[v] * [y_e == z[v]] (max) * act_edge'(x_e) (activation before) * s;  dP_l[u] = sum_{e leaving u} w_e over
+//      the source-keyed CSR, dT_l[v] = sum_{e into v} w_e over the forward's CSR (edge_grad_kernel, one template)
+//   4. dW_l = h^T dP_l,  dW^t_l = h_tgt^T dT_l   (TN, fixed 8192-row chunks)
+//   5. grad_h = dP [W_0^T; ..] (+ dT [W^t_0^T; ..] on the owned rows)
+// Every temporary is [V or Vs, L*H] at most.  On a shard, dP and grad_h cover every source (bt is the owned transpose), dT and
+// the target term the owned rows.
+static int transform_aggregate_bwd(tfgnn_batch* b, tfgnn_batch* bt, const float* h, int D, const PtrTable& wt,
+                                   float* const* grad_W, int H, uint32_t flags, int aggregation, int activation,
+                                   const float* out, const float* grad_out, float* grad_h, cudaStream_t st) {
+  const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
+  const int L = b->L, LH = L * H;
+  const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;
+  const bool use_max = aggregation == TFGNN_AGG_MAX;
+  int rc = enter_both(b, bt, st);
+  if (rc) return rc;
+  // 1. P, T and (max) z, n
+  EdgeReduceParams f;
+  rc = transform_aggregate_tables(b, h, D, wt, H, flags, aggregation, activation, TFGNN_PATH_AUTO, &f, st);
+  if (rc) return rc;
+  const int final_act = f.final_act;
+  PoolBuffer zn{st}, dP{st}, dT{st};
+  if (use_max) {
+    rc = zn.alloc((size_t)2 * V * H * sizeof(float));   // z, then n
+    if (rc) return rc;
+    EdgeReduceParams p = f;
+    p.out = zn.f(); p.ldo = H; p.final_act = TFGNN_ACT_NONE; p.ties = zn.f() + (size_t)V * H;
+    rc = launch_edge_reduce(p, /*merged=*/true, st);
+    if (rc) return rc;
+  }
+  const float* z = use_max ? zn.f() : nullptr;
+  void *dz = nullptr, *part = nullptr, *WT = nullptr;
+  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &dz);
+  if (rc) return rc;
+  rc = batch_scratch(b, 9, tn_partial_floats(Vs, D, H) * sizeof(float), &part);   // Vs >= V
+  if (rc) return rc;
+  rc = batch_scratch(b, 3, (size_t)LH * D * sizeof(float), &WT);
+  if (rc) return rc;
+  // 2. dZ (act_final' from the saved output, or for gelu from z)
+  act_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_out, final_act == TFGNN_ACT_GELU ? z : out, V, H, final_act,
+                                                   b->row_ptr, L, f.row_norm, (float*)dz,
+                                                   use_max ? z + (size_t)V * H : nullptr);
+  TFGNN_LAUNCH_CHECK();
+  // 3. dP over the source-keyed CSR, dT over the forward's
+  rc = dP.alloc((size_t)Vs * LH * sizeof(float));
+  if (rc) return rc;
+  rc = launch_edge_grad(f, z, (const float*)dz, bt->row_ptr, bt->src_sorted, (int)Vs, dP.f(), st);
+  if (rc) return rc;
+  if (use_target) {
+    rc = dT.alloc((size_t)V * LH * sizeof(float));
+    if (rc) return rc;
+    rc = launch_edge_grad(f, z, (const float*)dz, nullptr, nullptr, 0, dT.f(), st);
+    if (rc) return rc;
+  }
+  // 4. dW_l over all Vs rows, dW^t_l (rows [D, 2D) of W_l) over the owned rows
+  const float* h_tgt = h + (size_t)lo * D;
+  for (int l = 0; l < L; ++l) {
+    const PtrTable gw = one_table(grad_W[l]);
+    rc = weight_grad(h, D, dP.f() + (size_t)l * H, LH, Vs, D, H, (float*)part, gw, 1, D, 0, st);
+    if (rc) return rc;
+    if (use_target) {
+      rc = weight_grad(h_tgt, D, dT.f() + (size_t)l * H, LH, V, D, H, (float*)part, gw, 1, D, D, st);
+      if (rc) return rc;
+    }
+  }
+  if (!grad_h) return 0;
+  // 5. grad_h = dP [W_0^T; ..] (K = L*H), then the owned rows += dT [W^t_0^T; ..]
+  rc = gemm_transposed(dP.f(), LH, {wt, L, D, H, 1, 0, /*stacked=*/true}, (float*)WT, grad_h, D, Vs, D, GemmEpilogue{},
+                       b, st);
+  if (rc || !use_target) return rc;
+  GemmEpilogue acc;
+  acc.accumulate = 1;
+  return gemm_transposed(dT.f(), LH, {wt, L, D, H, 1, D, /*stacked=*/true}, (float*)WT, grad_h + (size_t)lo * D, D, V, D,
+                         acc, b, st);
+}
+
 }  // namespace tfgnn
 
 using namespace tfgnn;
@@ -436,11 +521,11 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
   if (int rc = check_backward_pair(b, bt)) return rc;
-  if (flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION)
-    return unsupported("rgcn_bwd: activation-before-aggregation is not built yet");
   const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // W_l is then [2D, H]: rows [0,D) source, [D,2D) target
-  if (aggregation == TFGNN_AGG_MAX) return unsupported("rgcn_bwd: max aggregation is not built yet");
+  const bool transform_aggregate = aggregation == TFGNN_AGG_MAX || (flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION);
   if (D % 4 != 0 || H % 4 != 0) return unsupported("rgcn_bwd needs D and H to be multiples of 4");
+  if (transform_aggregate && H > 512)
+    return unsupported("rgcn_bwd: max aggregation / activation before aggregation above hidden_dim 512 is not built");
   TFGNN_REQUIRE(L == 0 || (W && grad_W), "weight / weight-gradient table is NULL");
   cudaStream_t st = (cudaStream_t)stream;
   if (V == 0 || L == 0)   // no owned rows (an empty shard) or no edge types: zero contribution
@@ -456,6 +541,8 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     wt.p[l] = W[l];
     gwt.p[l] = grad_W[l];
   }
+  if (transform_aggregate)
+    return transform_aggregate_bwd(b, bt, h, D, wt, grad_W, H, flags, aggregation, activation, out, grad_out, grad_h, st);
   // 1. dZ = dOut * act'(out) * rn(v)
   float* dz = nullptr;
   int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, &dz, [&](float* z) {
@@ -522,8 +609,9 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   const int L = b->L;
   if (int rc = check_backward_pair(b, bt)) return rc;
   if (flags & TFGNN_FLAG_USE_TARGET_STATE) return unsupported("ggnn_bwd: target-state input is not built yet");
-  if (aggregation == TFGNN_AGG_MAX) return unsupported("ggnn_bwd: max aggregation is not built yet");
   if (H % 4 != 0) return unsupported("ggnn_bwd needs hidden_dim to be a multiple of 4");
+  if (aggregation == TFGNN_AGG_MAX && H > 512)
+    return unsupported("ggnn_bwd: max aggregation above hidden_dim 512 is not built");
   TFGNN_REQUIRE(grad_h, "NULL pointer");
   TFGNN_REQUIRE(grad_gru_kernel && grad_gru_recurrent_kernel && grad_gru_bias, "GRU gradient pointer is NULL");
   TFGNN_REQUIRE(L == 0 || grad_W, "weight-gradient table is NULL");

@@ -29,10 +29,17 @@ struct EdgeReduceParams {
   int reduce_max = 0;   // unsorted_segment_max instead of sum
   int row_norm = 0;     // MERGED only: 1 = mean, 2 = sqrt_n (counts over all types)
   int final_act = 0;    // MERGED only: activation after aggregation          message_passing.py:176-177
+  float* ties = nullptr;  // MERGED max only: [v, c] (leading dimension ldo) = number of messages equal to the maximum
 };
 
 // max_blocks > 0 caps the grid (grid-stride over segments) so another kernel can co-reside on the SMs.
 int launch_edge_reduce(const EdgeReduceParams& p, bool merged, cudaStream_t st, int max_blocks = 0);
+// Gradient of the merged transform-then-aggregate reduce f (max and / or activation before aggregation) with respect to its
+// per-type tables, for z = its maximum ([V, C]; max only, else NULL) and dz = the gradient of its result ([V, C], the tie
+// count of max divided out).  With the source-keyed CSR (row_ptr_t, tgt over Vs sources): dP = d/d f.X into out [Vs, L*C];
+// with row_ptr_t NULL: dT = d/d f.T over f's own CSR into out [V, L*C].
+int launch_edge_grad(const EdgeReduceParams& f, const float* z, const float* dz, const int* row_ptr_t, const int* tgt,
+                     int Vs, float* out, cudaStream_t st);
 int launch_target_term(const float* h, int ldh, const int* row_ptr, int V, int L, int D, int normalize,
                        float* out, int ldo, int col0, cudaStream_t st);
 int launch_edge_scatter_atomic(const tfgnn_batch* b, const float* X, int ldx, int C, int normalize,

@@ -183,9 +183,10 @@ extern "C" int tfgnn_b200_layer_norm(const float* x, const float* gamma, const f
 
 // ---- primitives of the differentiable generic path (layers/differentiable.py, SURVEY.md section 8f-1) -----------------
 // The reference differentiates EVERY message-passing variant with tf.GradientTape through its literal op sequence
-// (message_passing.py:95-218).  Variants without a fused backward (hidden-layer edge MLPs, RGIN, GNN-FiLM, max aggregation,
-// activation before aggregation) train through the same op sequence here: each op below is the forward or the backward of
-// one TensorFlow op of that sequence.
+// (message_passing.py:95-218).  Variants without a fused backward (edge MLPs with two or more hidden layers, one hidden
+// layer combined with max aggregation or activation before aggregation, hidden layers in GNN-FiLM's MLPs, GNN-FiLM with max
+// aggregation or activation before aggregation) train through the same op sequence here: each op below is the forward or the
+// backward of one TensorFlow op of that sequence.
 namespace tfgnn {
 
 // grad_in = grad_out * act'(.): `ref` is the forward OUTPUT for every activation but gelu, whose `ref` is the forward INPUT

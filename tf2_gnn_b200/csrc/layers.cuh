@@ -12,6 +12,9 @@ int agg_row_norm(int aggregation);
 constexpr int kPackSlot = 6;
 int node_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int N, int K,
               const GemmEpilogue& epi, int path, tfgnn_batch* batch, cudaStream_t st);
+// P (slot 2), T (slot 4) and the merged edge reduce of the transform-then-aggregate form (api.cu)
+int transform_aggregate_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& W, int H, uint32_t flags,
+                               int aggregation, int activation, int path, EdgeReduceParams* p, cudaStream_t st);
 int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                   uint32_t flags, int aggregation, int activation, int path, float* out, int ldo, cudaStream_t st);
 // literal per-edge path (literal.cu); FB = optional FiLM table [V, L*2H] (gamma | beta per type)

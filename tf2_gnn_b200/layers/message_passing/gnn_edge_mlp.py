@@ -124,9 +124,9 @@ class GNN_Edge_MLP(MessagePassing):
         self._check_types(prepared)
         ptrs, tensors = self._mlp_weight_ptrs()
         if torch.is_grad_enabled() and (h.requires_grad or any(t.requires_grad for t in tensors)):
-            if not (self._has_fused_backward(int(h.shape[1])) and not self._message_activation_before_aggregation):
-                # two or more hidden layers / max aggregation / activation before aggregation: the reference's literal op
-                # order with per-op backward kernels (layers/differentiable.py)
+            if not self._has_fused_backward(int(h.shape[1]), self._message_activation_before_aggregation):
+                # two or more hidden layers / one hidden layer with max aggregation or activation before aggregation: the
+                # reference's literal op order with per-op backward kernels (layers/differentiable.py)
                 from ..differentiable import edge_mlp_family_forward
                 return edge_mlp_family_forward(self, h, prepared)
             cfg = dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers), flags=self._flags(),
@@ -139,12 +139,18 @@ class GNN_Edge_MLP(MessagePassing):
             _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
         return out
 
-    def _has_fused_backward(self, D: int) -> bool:
-        """The edge MLPs tfgnn_b200_rgcn_bwd (no hidden layer) and tfgnn_b200_edge_mlp_bwd (one hidden layer, the class
-        defaults of GNN_Edge_MLP and RGIN) differentiate, activation before aggregation aside."""
-        n = int(self._num_edge_MLP_hidden_layers)
-        return ((n == 0 or (n == 1 and self._hidden_dim <= 512)) and self._aggregation_fn.name != "max"
-                and D % 4 == 0 and self._hidden_dim % 4 == 0)
+    def _has_fused_backward(self, D: int, activation_before: bool = False) -> bool:
+        """The edge MLPs tfgnn_b200_rgcn_bwd (no hidden layer: every aggregation, the activation before or after it; with
+        max aggregation or the activation before it up to hidden_dim 512) and tfgnn_b200_edge_mlp_bwd (one hidden layer, the
+        class defaults of GNN_Edge_MLP and RGIN: sum / mean / sqrt_n with the activation after it, up to hidden_dim 512)
+        differentiate.  `activation_before`: the layer applies its activation before the aggregation (RGIN ignores it)."""
+        n, H = int(self._num_edge_MLP_hidden_layers), self._hidden_dim
+        if D % 4 or H % 4:
+            return False
+        transform_then_aggregate = activation_before or self._aggregation_fn.name == "max"
+        if n == 0:
+            return H <= 512 or not transform_then_aggregate
+        return n == 1 and H <= 512 and not transform_then_aggregate
 
     def call_with_layernorm(self, inputs: MessagePassingInput, gamma: torch.Tensor, beta: torch.Tensor, epsilon: float,
                             prepared: Optional[PreparedBatch] = None) -> torch.Tensor:

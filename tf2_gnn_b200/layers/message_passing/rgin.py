@@ -62,8 +62,8 @@ class RGIN(GNN_Edge_MLP):
                 for i, W in enumerate(aggr):
                     out = dense(out, W, None, self._activation_fn if i == len(aggr) - 1 else relu)
                 return out
-            # two or more hidden layers / max aggregation: the reference's literal op order with per-op backward kernels
-            # (layers/differentiable.py)
+            # two or more hidden layers / one hidden layer with max aggregation: the reference's literal op order with
+            # per-op backward kernels (layers/differentiable.py)
             return edge_mlp_family_forward(
                 self, h, prepared, activation_before=False,
                 aggr_kernels=[v.value for v in self._aggregation_mlp] if self._aggregation_mlp is not None else None)

@@ -1,7 +1,11 @@
 """Measurement of the backward pass (SURVEY.md §8f-1) at bench.py's workloads: forward and backward device time of one
 RGCN, GGNN or GNN-FiLM layer through the autograd hook, CUDA events, inputs resident in HBM.
   python tools/bench_backward.py [--workload cfg2] [--steps 10] [--warmup 3] [--shards N] [--film-literal]
-                                 [--kind rgin|gnn_edge_mlp [--literal]]
+                                 [--kind rgin|gnn_edge_mlp] [--literal]
+                                 [--aggregation sum|mean|sqrt_n|max] [--act-before] [--activation NAME]
+With --aggregation / --act-before / --activation: the layer's hyper-parameters changed accordingly (e.g. the RGCN layer of
+cfg2 with max aggregation, which trains through the transform-then-aggregate backward); --literal then times that
+configuration (RGCN unless --kind) against the literal path on the reduced graph below.
 For GNN-FiLM the line also carries the device memory in use after the steps (the library's pool and torch's allocator keep
 their high-water marks, so this is the peak of the run, inputs included).
 With --film-literal: a reduced FiLM graph on which the literal per-edge path (layers/differentiable.py) fits, 250k nodes /
@@ -43,13 +47,19 @@ def main():
                     help="time this layer kind (class defaults, one hidden layer of width H) on the workload's graph "
                          "instead of the workload's own layer")
     ap.add_argument("--literal", action="store_true",
-                    help="with --kind: fused vs literal training step on a reduced graph the literal path fits")
+                    help="with --kind, --aggregation or --act-before: fused vs literal training step on a reduced graph the "
+                         "literal path fits")
+    ap.add_argument("--aggregation", choices=["sum", "mean", "sqrt_n", "max"],
+                    help="aggregation_function of the timed layer (default: the layer's)")
+    ap.add_argument("--act-before", action="store_true",
+                    help="message_activation_before_aggregation=True for the timed layer")
+    ap.add_argument("--activation", help="message_activation_function of the timed layer (default: the layer's)")
     args = ap.parse_args()
     if args.film_literal:
         return bench_film_literal(args)
     if args.literal:
-        if not args.kind:
-            ap.error("--literal needs --kind")
+        if not args.kind and not config_overrides(args):
+            ap.error("--literal needs --kind, --aggregation or --act-before")
         return bench_edge_mlp_literal(args)
     wl = bench.WORKLOADS[args.workload]
     V, H, L = wl["V"], wl["H"], len(wl["E"])
@@ -59,7 +69,7 @@ def main():
     cls = get_message_passing_class(kind)
     params = cls.get_default_hyperparameters()
     params.update(EDGE_MLP_KINDS[kind] if args.kind else wl.get("params", {}))
-    params.update(hidden_dim=H)
+    params.update(hidden_dim=H, **config_overrides(args))
     layer = cls(params)
     torch.manual_seed(1)
     layer.build(MessagePassingInput((None, H), tuple((None, 2) for _ in range(L))))
@@ -99,13 +109,28 @@ def main():
         rec["literal_saved_activations_GB_from_shapes"] = literal_footprint_gb(M, H, H, params)
     else:
         rec["forward_algorithmic_bytes"] = bench.algorithmic_bytes(kind, V, wl["E"], H, H, params)
-    if kind in ("gnn_film",) + tuple(EDGE_MLP_KINDS):
+    if config_overrides(args):
+        rec["overrides"] = config_overrides(args)
+        rec["note"] = NOTES["transform_aggregate"]
+    if kind in ("gnn_film",) + tuple(EDGE_MLP_KINDS) or config_overrides(args):
         rec["device_memory_used_GB"] = device_used_gb()
     print(json.dumps(rec), flush=True)
 
 
 # --kind: class defaults (one hidden layer in the edge MLPs); RGIN with PPI_RGIN.json's normalisation
 EDGE_MLP_KINDS = {"rgin": {"normalize_by_num_incoming": True}, "gnn_edge_mlp": {}}
+
+
+def config_overrides(args):
+    """Hyper-parameters set by --aggregation / --act-before / --activation."""
+    o = {}
+    if args.aggregation:
+        o["aggregation_function"] = args.aggregation
+    if args.act_before:
+        o["message_activation_before_aggregation"] = True
+    if args.activation:
+        o["message_activation_function"] = args.activation
+    return o
 
 
 def literal_footprint_gb(M, D, H, params):
@@ -128,6 +153,10 @@ NOTES = {
             "(tensor-core GEMM, K = L*H); autograd hook overhead included",
     "gnn_edge_mlp": "as rgin, plus Xt = h_v U^t, the per-column count of active edges in the recompute pass, "
                     "dXt = dA * count, dU^t (TN) and the target rows of grad_h (accumulating GEMM)",
+    "transform_aggregate": "no hidden layer, max aggregation or activation before aggregation: backward = recompute P = h W "
+                           "(node GEMM) and, for max, the maximum and its tie count (one pass of the forward's edge "
+                           "reduce), dZ, dP over the source-keyed CSR (one warp per (type, source)), dW (TN), grad_h "
+                           "(tensor-core GEMM, K = L*H); autograd hook overhead included",
     "gnn_film": "backward = per type: recompute [A_l | T_l] (CSR reduce), dQ_l and dgamma_l (tensor-core GEMMs with the dZ "
                 "multiply in the epilogue), dW_l and dF_l (TN GEMMs, fp32 FFMA), dA_l and the target-side terms "
                 "(tensor-core GEMMs); then one source-keyed CSR reduce for dh; autograd hook overhead included",
@@ -213,17 +242,19 @@ def bench_film_literal(args):
 
 
 def bench_edge_mlp_literal(args):
-    """Fused (tfgnn_b200_edge_mlp_bwd) vs literal (layers/differentiable.py) training step of an RGIN or GNN_Edge_MLP layer
-    with one hidden layer, alternated step by step, on a reduced graph the literal path fits."""
+    """Fused (tfgnn_b200_edge_mlp_bwd / tfgnn_b200_rgcn_bwd) vs literal (layers/differentiable.py) training step of an RGIN
+    or GNN_Edge_MLP layer (class defaults) or of an RGCN layer, with --aggregation / --act-before / --activation applied,
+    alternated step by step, on a reduced graph the literal path fits."""
     from tf2_gnn_b200.layers.differentiable import edge_mlp_family_forward
-    kind = args.kind
+    kind = args.kind or "rgcn"
+    changed = dict(EDGE_MLP_KINDS.get(kind, {}), **config_overrides(args))
     wl = dict(V=250_000, E=[1_000_000] * 4, H=256, kind=kind, graph="er",
               desc=f"{kind} reduced graph: 250k nodes / 4M edges / 4 edge types, D = H = 256 (class defaults, "
-                   f"{EDGE_MLP_KINDS[kind] or 'nothing'} changed)")
+                   f"{changed or 'nothing'} changed)")
     V, H, L = wl["V"], wl["H"], len(wl["E"])
     h_np, adjs_np, _ = bench.make_inputs(wl, seed=0)
     cls = get_message_passing_class(kind)
-    layer = cls(dict(cls.get_default_hyperparameters(), hidden_dim=H, **EDGE_MLP_KINDS[kind]))
+    layer = cls(dict(cls.get_default_hyperparameters(), hidden_dim=H, **changed))
     torch.manual_seed(1)
     layer.build(MessagePassingInput((None, H), tuple((None, 2) for _ in range(L))))
     for v in layer.variables:
