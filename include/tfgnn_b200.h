@@ -276,6 +276,26 @@ TFGNN_API int tfgnn_b200_rgat_fwd(tfgnn_batch_t* batch, const float* h, int32_t 
                         const float* const* attention, int32_t H, int32_t num_heads,
                         int32_t activation, int32_t path, float* out, void* stream);
 
+/* Backward of tfgnn_b200_rgat_fwd (the reference differentiates with tf.GradientTape,
+ * models/graph_task_model.py:338-365) without per-edge tensors: every temporary is node-sized.  batch_t is the SAME adjacency
+ * prepared with TFGNN_PREPARE_TRANSPOSE.  path = the forward's path: P = h W_l and the score halves are recomputed with the
+ * forward's bits.  out = saved forward output, grad_out = dL/dout [V,H]; writes grad_h [V,D] (may be NULL), grad_W[l] [D,H]
+ * and grad_attention[l] [K, 2H/K].
+ * Supported: D % 4 == 0, (H / num_heads) % 4 == 0, H <= 512, activations none/relu/tanh/leaky_relu/elu/selu (derivative
+ * from the output) and gelu (pre-activation recomputed).  Anything else (and TFGNN_PATH_ATOMIC) returns
+ * TFGNN_ERR_UNSUPPORTED.
+ * On a target-range shard (batch from tfgnn_b200_prepare_sharded over targets [lo, hi)), batch_t must be the same
+ * adjacency and range prepared with TFGNN_PREPARE_TRANSPOSE_OWNED.  h is then the full [num_nodes_total, D] table, out and
+ * grad_out have hi-lo rows, and the call writes THIS SHARD'S CONTRIBUTION: grad_h [num_nodes_total, D] (every row),
+ * grad_W[l] and grad_attention[l].  The contributions of all shards sum to the unsharded gradients.  An empty shard, or a
+ * batch without edge types, writes zeros.
+ * No float atomics: hub targets (more than 2048 incoming edges) are cut into fixed chunks whose partials are combined in
+ * chunk order, so every call, and each shard's contribution, is bitwise reproducible for the same inputs. */
+TFGNN_API int tfgnn_b200_rgat_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, const float* h, int32_t D,
+                        const float* const* W, const float* const* attention, int32_t H, int32_t num_heads,
+                        int32_t activation, int32_t path, const float* out, const float* grad_out, float* grad_h,
+                        float* const* grad_W, float* const* grad_attention, void* stream);
+
 /* Node-level dense layer out = act(x W), x [V,K], W [K,N], no bias — the op behind every
  * tf.keras.layers.Dense(use_bias=False) on the path (gnn.py:136-141,165-169) and the building
  * block of the fp32-accurate node-level contractions.  path: 0 auto, 2 SIMT fp32, 3 wgmma 3xTF32. */

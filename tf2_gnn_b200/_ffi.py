@@ -43,7 +43,7 @@ EXPORTED_SYMBOLS = (
     "tfgnn_b200_activation_bwd", "tfgnn_b200_row_scale", "tfgnn_b200_mul_add", "tfgnn_b200_segment_max_bwd",
     "tfgnn_b200_rgcn_fwd_allgather", "tfgnn_b200_softmax_apply", "tfgnn_b200_head_scale", "tfgnn_b200_head_dot",
     "tfgnn_b200_gru_gate_bwd", "tfgnn_b200_rgcn_ln_fwd", "tfgnn_b200_film_bwd",
-    "tfgnn_b200_edge_mlp_bwd",
+    "tfgnn_b200_edge_mlp_bwd", "tfgnn_b200_rgat_bwd",
 )
 
 _PP = POINTER(c_void_p)
@@ -92,6 +92,8 @@ def lib() -> ctypes.CDLL:
                                           c_int32, c_int32, c_void_p, c_void_p, c_void_p, _PP, c_void_p]
     L.tfgnn_b200_rgat_fwd.argtypes = [c_void_p, c_void_p, c_int32, _PP, _PP, c_int32, c_int32, c_int32, c_int32,
                                       c_void_p, c_void_p]
+    L.tfgnn_b200_rgat_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, _PP, _PP, c_int32, c_int32, c_int32, c_int32,
+                                      c_void_p, c_void_p, c_void_p, _PP, _PP, c_void_p]
     L.tfgnn_b200_dense_fwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32,
                                        c_void_p]
     L.tfgnn_b200_gather_rows.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int64, c_int64, c_void_p, c_void_p]

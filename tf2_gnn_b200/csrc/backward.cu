@@ -274,15 +274,6 @@ static int check_backward_pair(const tfgnn_batch* b, const tfgnn_batch* bt) {
   return 0;
 }
 
-// A buffer from the library pool, freed (stream-ordered, after the work queued so far) when it goes out of scope.
-struct PoolBuffer {
-  cudaStream_t st;
-  void* p = nullptr;
-  ~PoolBuffer() { pool_free(p, st); }
-  int alloc(size_t bytes) { return pool_alloc(&p, bytes, st); }
-  float* f() const { return (float*)p; }
-};
-
 static PtrTable one_table(const void* p) {
   PtrTable t{};
   t.p[0] = p;
@@ -1171,6 +1162,92 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
   acc.accumulate = 1;
   return gemm_transposed((const float*)cnt, LH, {us, L, D, H, 1, D, /*stacked=*/true}, (float*)Wp, grad_h + (size_t)lo * D,
                          D, V, D, acc, b, st);
+}
+
+// =====================================================================================================================
+// RGAT backward (rgat.py:91-163 through tfgnn_b200_rgat_fwd; edge-level kernels and their math in rgat.cu).  With
+// P_l = h W_l, the score halves s_src, s_tgt of the forward and dZ = dOut * act':
+//   1. dZ (gelu: the pre-activation from the backward's own target walk, deterministic on hub rows too)
+//   2. P, s_src, s_tgt recomputed by the forward's rgat_tables: the forward's bits
+//   3. target pass: m, den, g = dZ . o per (v, k) and ds_tgt [V, L*K]
+//   4. source pass over the source-keyed CSR: dP [Vs, L*H] (messages and both score halves) and ds_src [Vs, L*K]
+//   5. da_l = [sum_u ds_src P_l[u] | sum_v ds_tgt P_l[v]] per head (fixed row chunks, reduced in chunk order)
+//   6. dW_l = h^T dP_l (TN, fixed 8192-row chunks),  7. grad_h = dP [W_0^T; ..]
+// Every temporary is node-sized; nothing has a per-edge dimension and nothing uses float atomics.  On a shard dP, ds_src and
+// grad_h cover every source (bt is the owned transpose), the target pass and ds_tgt the owned rows.
+// =====================================================================================================================
+extern "C" int tfgnn_b200_rgat_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int32_t D, const float* const* W,
+                                   const float* const* attention, int32_t H, int32_t num_heads, int32_t activation,
+                                   int32_t path, const float* out, const float* grad_out, float* grad_h,
+                                   float* const* grad_W, float* const* grad_attention, void* stream) {
+  // the configuration is judged from the scalar arguments alone, before any batch is read
+  TFGNN_REQUIRE(D > 0 && H > 0 && num_heads > 0, "D, H and num_heads must be positive");
+  TFGNN_REQUIRE(H % num_heads == 0, "hidden_dim must be divisible by num_heads (rgat.py:72)");
+  TFGNN_REQUIRE(valid_act(activation), "unknown activation code");
+  const int K = num_heads, d = H / num_heads;
+  if (D % 4 != 0 || d % 4 != 0) return unsupported("rgat_bwd needs D and hidden_dim / num_heads to be multiples of 4");
+  if (H > 512) return unsupported("rgat_bwd: hidden_dim above 512 is not built");
+  if (path == TFGNN_PATH_ATOMIC) return unsupported("rgat_bwd: TFGNN_PATH_ATOMIC is not available for RGAT");
+  TFGNN_REQUIRE(b != nullptr && bt != nullptr, "batch / transposed batch is NULL");
+  // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
+  const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
+  const int L = b->L;
+  if (int rc = check_backward_pair(b, bt)) return rc;
+  TFGNN_REQUIRE(L == 0 || (W && attention && grad_W && grad_attention), "weight / weight-gradient table is NULL");
+  PtrTable wt{}, at{}, gat{};
+  for (int l = 0; l < L; ++l) {
+    TFGNN_REQUIRE(W[l] && attention[l] && grad_W[l] && grad_attention[l], "a weight pointer is NULL");
+    wt.p[l] = W[l];
+    at.p[l] = attention[l];
+    gat.p[l] = grad_attention[l];
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (V == 0 || L == 0)   // no owned rows (an empty shard) or no edge types: zero contribution
+    return zero_contribution({{grad_W, L, (size_t)D * H}, {grad_attention, L, (size_t)2 * H}}, grad_h, (size_t)Vs * D, st);
+  TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
+  const int LH = L * H, LK = L * K;
+  // 1. dZ = dOut * act'(out)
+  float* dz = nullptr;
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, TFGNN_AGG_SUM, st, &dz, [&](float* z) {
+    const float *P = nullptr, *ss = nullptr, *stt = nullptr;
+    const int r = rgat_tables(b, h, D, wt, at, H, K, path, &P, &ss, &stt, st);
+    return r ? r : launch_rgat_target_pass(b, P, ss, stt, K, d, nullptr, nullptr, nullptr, z, st);
+  });
+  if (rc) return rc;
+  // 2. the forward's tables
+  const float *P = nullptr, *ss = nullptr, *stt = nullptr;
+  rc = rgat_tables(b, h, D, wt, at, H, K, path, &P, &ss, &stt, st);
+  if (rc) return rc;
+  PoolBuffer stat{st}, ds_tgt{st}, dP{st}, ds_src{st};
+  rc = stat.alloc((size_t)V * 3 * K * sizeof(float));
+  if (!rc) rc = ds_tgt.alloc((size_t)V * LK * sizeof(float));
+  if (!rc) rc = dP.alloc((size_t)Vs * LH * sizeof(float));
+  if (!rc) rc = ds_src.alloc((size_t)Vs * LK * sizeof(float));
+  if (rc) return rc;
+  // 3., 4. target pass, source pass
+  rc = launch_rgat_target_pass(b, P, ss, stt, K, d, dz, stat.f(), ds_tgt.f(), nullptr, st);
+  if (rc) return rc;
+  rc = launch_rgat_source_pass(b, bt, P, ss, stt, at, K, d, dz, stat.f(), ds_tgt.f(), dP.f(), ds_src.f(), st);
+  if (rc) return rc;
+  // 5. attention gradients: the source half over all Vs rows, the target half over the owned rows
+  rc = launch_rgat_attention_grad(ds_src.f(), P, Vs, L, K, d, gat, 0, st);
+  if (rc) return rc;
+  rc = launch_rgat_attention_grad(ds_tgt.f(), P + (size_t)lo * LH, V, L, K, d, gat, 1, st);
+  if (rc) return rc;
+  // 6. dW_l = h^T dP_l over all Vs rows
+  void *part = nullptr, *WT = nullptr;
+  rc = batch_scratch(b, 9, tn_partial_floats(Vs, D, H) * sizeof(float), &part);
+  if (rc) return rc;
+  for (int l = 0; l < L; ++l) {
+    rc = weight_grad(h, D, dP.f() + (size_t)l * H, LH, Vs, D, H, (float*)part, one_table(grad_W[l]), 1, D, 0, st);
+    if (rc) return rc;
+  }
+  if (!grad_h) return 0;
+  // 7. grad_h = dP [W_0^T; ..] (K = L*H)
+  rc = batch_scratch(b, 3, (size_t)LH * D * sizeof(float), &WT);
+  if (rc) return rc;
+  return gemm_transposed(dP.f(), LH, {wt, L, D, H, 1, 0, /*stacked=*/true}, (float*)WT, grad_h, D, Vs, D, GemmEpilogue{},
+                         b, st);
 }
 
 // =====================================================================================================================

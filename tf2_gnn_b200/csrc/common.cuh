@@ -190,4 +190,13 @@ int batch_enter(tfgnn_batch* b, cudaStream_t st);
 // after the first batches no call on the per-batch path reaches cudaMalloc / cudaFree or synchronises).
 int pool_alloc(void** p, size_t bytes, cudaStream_t st);
 void pool_free(void* p, cudaStream_t st);
+
+// A buffer from the library pool, freed (stream-ordered, after the work queued so far) when it goes out of scope.
+struct PoolBuffer {
+  cudaStream_t st;
+  void* p = nullptr;
+  ~PoolBuffer() { pool_free(p, st); }
+  int alloc(size_t bytes) { return pool_alloc(&p, bytes, st); }
+  float* f() const { return (float*)p; }
+};
 }  // namespace tfgnn

@@ -398,6 +398,48 @@ __global__ void rgat_aggregate_kernel(const float* __restrict__ P, const float* 
   }
 }
 
+// P_l = h W_l for every one of the Vs nodes (slot 2) and the score halves s_src, s_tgt [Vs, L*K] (slots 13, 14).  The forward
+// and the backward (which recomputes them) both call this, so the backward sees the forward's bits.  Needs L > 0.
+int rgat_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& wt, const PtrTable& at, int H, int K, int path,
+                const float** P_out, const float** s_src_out, const float** s_tgt_out, cudaStream_t st) {
+  const long long Vs = b->V_src;
+  const int L = b->L, d = H / K, LH = L * H;
+  void *P = nullptr, *Wcat = nullptr, *ss = nullptr, *stt = nullptr;
+  int rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &P);
+  if (rc) return rc;
+  rc = batch_scratch(b, 3, (size_t)D * LH * sizeof(float), &Wcat);
+  if (rc) return rc;
+  rc = batch_scratch(b, 13, (size_t)Vs * L * K * sizeof(float), &ss);
+  if (rc) return rc;
+  rc = batch_scratch(b, 14, (size_t)Vs * L * K * sizeof(float), &stt);
+  if (rc) return rc;
+  // P_l = h W_l for every node once (rgat.py:102-109 applies the same Dense to source and target rows)
+  rc = launch_pack_horizontal(wt, L, 0, D, H, H, (float*)Wcat, LH, st);
+  if (rc) return rc;
+  GemmEpilogue none;
+  // Attention score halves in the projection's epilogue when the tensor-core GEMM takes the shape and its column tiles hold
+  // whole heads (TFGNN_B200_RGAT_FUSED_SCORES=0: separate kernel; read per call, the tests compare the two)
+  const char* fs = getenv("TFGNN_B200_RGAT_FUSED_SCORES");
+  const bool tc_path = (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
+  const bool fuse_scores = !(fs && atoi(fs) == 0) && tc_path && gemm_tc_supported(Vs, LH, D, h, D, (const float*)P, LH) &&
+                           gemm_tc_scores_supported(LH, H, d);
+  if (fuse_scores) {
+    none.score_src = (float*)ss; none.score_tgt = (float*)stt; none.score_att = at;
+    none.score_H = H; none.score_K = K; none.score_d = d;
+  }
+  rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
+  if (rc) return rc;
+  if (!fuse_scores) {
+    const long long total = Vs * L * K;
+    rgat_scores_kernel<<<ceil_div(total, 256), 256, 0, st>>>((const float*)P, Vs, L, K, d, at, (float*)ss, (float*)stt);
+    TFGNN_LAUNCH_CHECK();
+  }
+  *P_out = (const float*)P;
+  *s_src_out = (const float*)ss;
+  *s_tgt_out = (const float*)stt;
+  return 0;
+}
+
 }  // namespace tfgnn
 
 extern "C" int tfgnn_b200_rgat_fwd(tfgnn_batch_t* b, const float* h, int32_t D, const float* const* W,
@@ -407,60 +449,30 @@ extern "C" int tfgnn_b200_rgat_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   TFGNN_REQUIRE(D > 0 && H > 0 && num_heads > 0, "D, H and num_heads must be positive");
   TFGNN_REQUIRE(H % num_heads == 0, "hidden_dim must be divisible by num_heads (rgat.py:72)");
   TFGNN_REQUIRE(valid_act(activation), "unknown activation code");
-  const long long V = b->V, Vs = b->V_src;
+  const long long V = b->V;
   const int L = b->L, K = num_heads, d = H / num_heads;
   if (V == 0) return 0;
   TFGNN_REQUIRE(h && out, "h / out is NULL");
   if (path == TFGNN_PATH_ATOMIC) return unsupported("TFGNN_PATH_ATOMIC is not available for RGAT");
   cudaStream_t st = (cudaStream_t)stream;
-  const int LH = L * H;
   PtrTable wt{}, at{};
   for (int l = 0; l < L; ++l) {
     TFGNN_REQUIRE(W && attention && W[l] && attention[l], "a weight pointer is NULL");
     wt.p[l] = W[l];
     at.p[l] = attention[l];
   }
-  void *P = nullptr, *Wcat = nullptr, *ss = nullptr, *stt = nullptr;
+  const float *P = nullptr, *ss = nullptr, *stt = nullptr;
   int rc = batch_enter(b, st);
   if (rc) return rc;
   if (L > 0) {
-    rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &P);
+    rc = rgat_tables(b, h, D, wt, at, H, K, path, &P, &ss, &stt, st);
     if (rc) return rc;
-    rc = batch_scratch(b, 3, (size_t)D * LH * sizeof(float), &Wcat);
-    if (rc) return rc;
-    rc = batch_scratch(b, 13, (size_t)Vs * L * K * sizeof(float), &ss);
-    if (rc) return rc;
-    rc = batch_scratch(b, 14, (size_t)Vs * L * K * sizeof(float), &stt);
-    if (rc) return rc;
-    // P_l = h W_l for every node once (rgat.py:102-109 applies the same Dense to source and target rows)
-    rc = launch_pack_horizontal(wt, L, 0, D, H, H, (float*)Wcat, LH, st);
-    if (rc) return rc;
-    GemmEpilogue none;
-    // Attention score halves in the projection's epilogue when the tensor-core GEMM takes the shape and its column tiles hold
-    // whole heads (TFGNN_B200_RGAT_FUSED_SCORES=0: separate kernel; read per call, the tests compare the two)
-    const char* fs = getenv("TFGNN_B200_RGAT_FUSED_SCORES");
-    const bool tc_path = (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
-    const bool fuse_scores = !(fs && atoi(fs) == 0) && tc_path && gemm_tc_supported(Vs, LH, D, h, D, (const float*)P, LH) &&
-                             gemm_tc_scores_supported(LH, H, d);
-    if (fuse_scores) {
-      none.score_src = (float*)ss; none.score_tgt = (float*)stt; none.score_att = at;
-      none.score_H = H; none.score_K = K; none.score_d = d;
-    }
-    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
-    if (rc) return rc;
-    if (!fuse_scores) {
-      const long long total = Vs * L * K;
-      rgat_scores_kernel<<<ceil_div(total, 256), 256, 0, st>>>((const float*)P, Vs, L, K, d, at, (float*)ss,
-                                                              (float*)stt);
-      TFGNN_LAUNCH_CHECK();
-    }
   }
   const bool vec = (d % 4 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) && L > 0;
-  if (vec) return launch_rgat_aggregate(b, (const float*)P, (const float*)ss, (const float*)stt, K, d, activation, out, st);
+  if (vec) return launch_rgat_aggregate(b, P, ss, stt, K, d, activation, out, st);
   const long long threads = V * H;
   rgat_aggregate_kernel<false><<<ceil_div(threads, 128), 128, 0, st>>>(
-      (const float*)P, (const float*)ss, (const float*)stt, b->row_ptr, b->src_sorted, V, b->tgt_off, L, K, d,
-      activation, out);
+      P, ss, stt, b->row_ptr, b->src_sorted, V, b->tgt_off, L, K, d, activation, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }

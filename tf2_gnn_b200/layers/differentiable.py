@@ -5,10 +5,11 @@ The reference trains EVERY variant by letting tf.GradientTape differentiate its 
 activation).  The fused forward kernels reorder that sequence; RGCN-style layers, GGNN, GNN-FiLM without hidden layers, and
 GNN_Edge_MLP / RGIN (with or without its aggregation MLP) with at most one hidden layer in the edge MLPs have fused backward
 kernels (csrc/backward.cu).  Without a hidden layer in the edge MLPs, max aggregation and activation before aggregation have
-them too (the transform-then-aggregate form, up to hidden_dim 512).  Every other configuration of the Edge-MLP family — two
+them too (the transform-then-aggregate form, up to hidden_dim 512).  RGAT has one (tfgnn_b200_rgat_bwd) when D and the
+per-head width are multiples of 4 and hidden_dim <= 512.  Every other configuration of the Edge-MLP family — two
 or more hidden layers in the edge MLPs, one hidden layer combined with max aggregation or activation before aggregation,
 hidden layers in GNN-FiLM's MLPs, GNN-FiLM with max aggregation or activation before aggregation, D or H not a multiple of
-4 — trains through THIS module: the
+4 — and RGAT outside those shapes train through THIS module: the
 reference's own op order, each op a C-ABI kernel with a C-ABI backward (gather_rows <-> unsorted_segment_sum are each
 other's adjoint).  It materialises [E, D] tensors exactly like the reference does; it is the correctness path for
 training, not the fast path for inference (inference never comes here).

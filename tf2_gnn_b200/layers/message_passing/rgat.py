@@ -12,6 +12,38 @@ from .message_passing import (MessagePassing, MessagePassingInput, Variable, _la
                               register_message_passing_implementation)
 
 
+class _RgatLayerFunction(torch.autograd.Function):
+    """Autograd hook of the RGAT layer: forward = tfgnn_b200_rgat_fwd (so training output equals inference output),
+    backward = tfgnn_b200_rgat_bwd (no per-edge tensors, no float atomics).  weights = the L projection kernels, then the L
+    attention parameters.  The reference gets these gradients from tf.GradientTape (models/graph_task_model.py:338-365)."""
+
+    @staticmethod
+    def forward(ctx, h, prepared, cfg, *weights):
+        L = len(weights) // 2
+        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+        _ffi.check(_ffi.lib().tfgnn_b200_rgat_fwd(
+            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights[:L]), _ffi.ptr_array(weights[L:]),
+            cfg["H"], cfg["K"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+        ctx.prepared, ctx.cfg = prepared, cfg
+        ctx.save_for_backward(h, out, *weights)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        h, out, *weights = ctx.saved_tensors
+        cfg, prepared = ctx.cfg, ctx.prepared
+        L = len(weights) // 2
+        grad_out = grad_out.contiguous()
+        grad_h = torch.empty_like(h) if ctx.needs_input_grad[0] else None
+        grad_w = [torch.empty_like(w) for w in weights]
+        _ffi.check(_ffi.lib().tfgnn_b200_rgat_bwd(
+            prepared.handle, prepared.transposed().handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights[:L]),
+            _ffi.ptr_array(weights[L:]), cfg["H"], cfg["K"], cfg["act"], cfg["path"], out.data_ptr(), grad_out.data_ptr(),
+            grad_h.data_ptr() if grad_h is not None else None, _ffi.ptr_array(grad_w[:L]), _ffi.ptr_array(grad_w[L:]),
+            stream_ptr()))
+        return (grad_h, None, None, *grad_w)
+
+
 @register_message_passing_implementation
 class RGAT(MessagePassing):
     """Relational graph attention (rgat.py:12-51): per type a bias-free Dense W_l [D,H] applied to
@@ -46,13 +78,17 @@ class RGAT(MessagePassing):
              prepared: Optional[PreparedBatch] = None):
         h, prepared = self._device_inputs(inputs, prepared)
         if _needs_grad(h, *[v.value for v in self.variables]):
-            # training: the reference's literal op order with per-op backward kernels (layers/differentiable.py)
+            if self._has_fused_backward(int(h.shape[1])):
+                self._check_shape(prepared)
+                act = self._activation_fn.code if self._activation_fn is not None else _ffi.ACT[None]
+                cfg = dict(H=self._hidden_dim, K=int(self._num_heads), act=act, path=_ffi.PATH[self._path])
+                weights = ([v.value for v in self._edge_type_to_message_computation_layer]
+                           + [v.value for v in self._edge_type_to_attention_parameters])
+                return _RgatLayerFunction.apply(h, prepared, cfg, *weights)
+            # other shapes: the reference's literal op order with per-op backward kernels (layers/differentiable.py)
             from ..differentiable import rgat_forward
             return rgat_forward(self, h, prepared)
-        if prepared.num_edge_types != len(self._edge_type_to_message_computation_layer):
-            raise ValueError("number of adjacency lists differs from the number the layer was built for")
-        if self._hidden_dim % self._num_heads:
-            raise ValueError("hidden_dim must be divisible by num_heads (rgat.py:72)")
+        self._check_shape(prepared)
         out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
         kernels = [v.value for v in self._edge_type_to_message_computation_layer]
         att = [v.value for v in self._edge_type_to_attention_parameters]
@@ -61,6 +97,19 @@ class RGAT(MessagePassing):
             self._hidden_dim, int(self._num_heads), self._activation_fn.code, _ffi.PATH[self._path],
             out.data_ptr(), stream_ptr()))
         return out
+
+    def _check_shape(self, prepared: PreparedBatch) -> None:
+        if prepared.num_edge_types != len(self._edge_type_to_message_computation_layer):
+            raise ValueError("number of adjacency lists differs from the number the layer was built for")
+        if self._hidden_dim % self._num_heads:
+            raise ValueError("hidden_dim must be divisible by num_heads (rgat.py:72)")
+
+    def _has_fused_backward(self, D: int) -> bool:
+        """The shapes tfgnn_b200_rgat_bwd differentiates, on whole batches and target-range shards (the reference's
+        PPI_RGAT.json and bench.py's cfg3 among them): D and the per-head width multiples of 4, hidden_dim <= 512."""
+        H, K = self._hidden_dim, int(self._num_heads)
+        return (K > 0 and H % K == 0 and D % 4 == 0 and (H // K) % 4 == 0 and H <= 512
+                and self._path != "atomic")
 
     def _message_function(self, *args, **kwargs):
         raise NotImplementedError("built-in layers run fused; _message_function is only a plugin hook")

@@ -3,6 +3,7 @@ RGCN, GGNN or GNN-FiLM layer through the autograd hook, CUDA events, inputs resi
   python tools/bench_backward.py [--workload cfg2] [--steps 10] [--warmup 3] [--shards N] [--film-literal]
                                  [--kind rgin|gnn_edge_mlp] [--literal]
                                  [--aggregation sum|mean|sqrt_n|max] [--act-before] [--activation NAME]
+  python tools/bench_backward.py --kind rgat --literal [--steps 5] [--warmup 2]
 With --aggregation / --act-before / --activation: the layer's hyper-parameters changed accordingly (e.g. the RGCN layer of
 cfg2 with max aggregation, which trains through the transform-then-aggregate backward); --literal then times that
 configuration (RGCN unless --kind) against the literal path on the reduced graph below.
@@ -10,6 +11,8 @@ For GNN-FiLM the line also carries the device memory in use after the steps (the
 their high-water marks, so this is the peak of the run, inputs included).
 With --film-literal: a reduced FiLM graph on which the literal per-edge path (layers/differentiable.py) fits, 250k nodes /
 6 x 666,667 edges / D = H = 320, with the fused and the literal training step alternated in one process.
+--workload cfg3 is RGAT (tfgnn_b200_rgat_bwd); with --kind rgat --literal: cfg3's graph and layer shape reduced to 250k
+nodes / 3 x 1M edges, where the literal per-edge path fits, with the fused and the literal step alternated in one process.
 With --kind rgin|gnn_edge_mlp: that layer (class defaults, one hidden layer in the edge MLPs; RGIN normalised as in
 PPI_RGIN.json) on the workload's graph, with D = H = the workload's hidden_dim; the line carries the device memory in use and
 the literal path's saved activations computed from shapes.  Adding --literal runs the fused and the literal path alternated
@@ -43,9 +46,9 @@ def main():
     ap.add_argument("--shards", type=int, default=0, help="time the backward of each of N target-range shards")
     ap.add_argument("--film-literal", action="store_true",
                     help="fused vs literal GNN-FiLM training step on a reduced graph the literal path fits")
-    ap.add_argument("--kind", choices=sorted(EDGE_MLP_KINDS),
+    ap.add_argument("--kind", choices=sorted(EDGE_MLP_KINDS) + ["rgat"],
                     help="time this layer kind (class defaults, one hidden layer of width H) on the workload's graph "
-                         "instead of the workload's own layer")
+                         "instead of the workload's own layer; rgat only with --literal (--workload cfg3 is RGAT)")
     ap.add_argument("--literal", action="store_true",
                     help="with --kind, --aggregation or --act-before: fused vs literal training step on a reduced graph the "
                          "literal path fits")
@@ -57,6 +60,10 @@ def main():
     args = ap.parse_args()
     if args.film_literal:
         return bench_film_literal(args)
+    if args.kind == "rgat":
+        if not args.literal:
+            ap.error("--kind rgat goes with --literal (--workload cfg3 times the RGAT workload)")
+        return bench_rgat_literal(args)
     if args.literal:
         if not args.kind and not config_overrides(args):
             ap.error("--literal needs --kind, --aggregation or --act-before")
@@ -112,7 +119,7 @@ def main():
     if config_overrides(args):
         rec["overrides"] = config_overrides(args)
         rec["note"] = NOTES["transform_aggregate"]
-    if kind in ("gnn_film",) + tuple(EDGE_MLP_KINDS) or config_overrides(args):
+    if kind in ("gnn_film", "rgat") + tuple(EDGE_MLP_KINDS) or config_overrides(args):
         rec["device_memory_used_GB"] = device_used_gb()
     print(json.dumps(rec), flush=True)
 
@@ -160,6 +167,10 @@ NOTES = {
     "gnn_film": "backward = per type: recompute [A_l | T_l] (CSR reduce), dQ_l and dgamma_l (tensor-core GEMMs with the dZ "
                 "multiply in the epilogue), dW_l and dF_l (TN GEMMs, fp32 FFMA), dA_l and the target-side terms "
                 "(tensor-core GEMMs); then one source-keyed CSR reduce for dh; autograd hook overhead included",
+    "rgat": "backward = recompute P = h W and the score halves (the forward's GEMM), target pass (one online-softmax walk "
+            "per target, hubs in chunk-ordered partials), source pass over the source-keyed CSR (dP, ds_src), attention "
+            "gradients (fixed row chunks), dW (TN), grad_h (tensor-core GEMM, K = L*H); no float atomics; autograd hook "
+            "overhead included",
 }
 
 
@@ -234,6 +245,57 @@ def bench_film_literal(args):
                 ms[name][1].append(e1.elapsed_time(e2))
     print(json.dumps({
         "workload": wl["desc"], "kind": "gnn_film", "steps": args.steps, "card": card(),
+        "paths": {k: {"forward_ms": float(np.median(f)), "backward_ms": float(np.median(b)),
+                      "device_memory_used_GB": mem[k]} for k, (f, b) in ms.items()},
+        "note": "alternated step by step in one process; memory = device memory in use after the step with the library's "
+                "pool and torch's allocator cache emptied before it (their high-water mark for that path, inputs included)"}),
+        flush=True)
+
+
+def bench_rgat_literal(args):
+    """Fused (tfgnn_b200_rgat_bwd) vs literal (layers/differentiable.py: rgat_forward) RGAT training step, alternated step
+    by step, on cfg3's graph and layer shape reduced to a size the literal path fits."""
+    from tf2_gnn_b200.layers.differentiable import rgat_forward
+    wl = dict(bench.WORKLOADS["cfg3"], V=250_000, E=[1_000_000] * 3,
+              desc="RGAT reduced cfg3: power-law 250k nodes / 3M edges / 3 edge types, D = H = 128, 4 heads")
+    V, H, L = wl["V"], wl["H"], len(wl["E"])
+    h_np, adjs_np, _ = bench.make_inputs(wl, seed=0)
+    cls = get_message_passing_class("rgat")
+    layer = cls(dict(cls.get_default_hyperparameters(), hidden_dim=H, **wl["params"]))
+    torch.manual_seed(1)
+    layer.build(MessagePassingInput((None, H), tuple((None, 2) for _ in range(L))))
+    for v in layer.variables:
+        v.requires_grad_()
+    dev = torch.device("cuda", 0)
+    h = torch.from_numpy(h_np).to(dev).requires_grad_()
+    adj = tuple(torch.from_numpy(a).to(dev) for a in adjs_np)
+    g = torch.rand((V, H), device=dev) * 2 - 1
+    prepared = PreparedBatch(adj, V)
+    prepared.transposed()
+    paths = {"fused": lambda: layer(MessagePassingInput(h, adj), prepared=prepared),
+             "literal": lambda: rgat_forward(layer, h, prepared)}
+    ms = {k: ([], []) for k in paths}
+    mem = {k: 0.0 for k in paths}
+    for i in range(args.warmup + args.steps):
+        for name, fwd in paths.items():
+            release_memory()
+            e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            h.grad = None
+            for v in layer.variables:
+                v.value.grad = None
+            e0.record()
+            out = fwd()
+            e1.record()
+            out.backward(g)
+            e2.record()
+            torch.cuda.synchronize()
+            mem[name] = max(mem[name], device_used_gb())
+            del out
+            if i >= args.warmup:
+                ms[name][0].append(e0.elapsed_time(e1))
+                ms[name][1].append(e1.elapsed_time(e2))
+    print(json.dumps({
+        "workload": wl["desc"], "kind": "rgat", "steps": args.steps, "card": card(),
         "paths": {k: {"forward_ms": float(np.median(f)), "backward_ms": float(np.median(b)),
                       "device_memory_used_GB": mem[k]} for k, (f, b) in ms.items()},
         "note": "alternated step by step in one process; memory = device memory in use after the step with the library's "
