@@ -14,7 +14,7 @@
  *   - float32 node states / weights, int32 adjacency: [E,2] row-major [src,tgt] pairs
  *     (message_passing.py:102-104,195-196; gnn.py:222-228).
  *   - The caller owns all inputs, weights and the PRE-ALLOCATED output.  The library owns only
- *     the opaque tfgnn_batch_t (CSR + scratch), released by tfgnn_b200_free_batch.
+ *     the opaque tfgnn_batch_t (its CSR), released by tfgnn_b200_free_batch.
  *   - The output of a layer call must not overlap its node-state input (every target gathers arbitrary
  *     source rows); entries that work in place say so.
  *   - All work is enqueued on `stream` (a cudaStream_t passed as void*; NULL = legacy default

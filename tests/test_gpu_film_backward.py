@@ -286,7 +286,8 @@ def trimmed_pool():
     from tf2_gnn_b200 import _ffi
     from tf2_gnn_b200.runtime import clear_prepared_batch_cache
     _need_gpu()
-    # batches of earlier cases (the layer call's prepared-batch cache, reference cycles) hold their grown scratch slots
+    # batches of earlier cases (the layer call's prepared-batch cache, reference cycles) hold their CSR, and the pool keeps
+    # the blocks earlier calls freed
     clear_prepared_batch_cache()
     gc.collect()
     torch.cuda.empty_cache()

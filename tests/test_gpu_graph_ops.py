@@ -742,8 +742,8 @@ def test_segment_max_of_negative_zero():
 
 
 def test_gelu_backward_survives_scratch_regrowth_in_the_nested_forward(monkeypatch):
-    """ADVICE r1 (medium): rgcn_bwd + gelu recomputes the pre-activation through the forward entry point, which on the
-    pipelined path re-grows scratch slot 2; the backward must not keep a pointer into the freed block."""
+    """rgcn_bwd + gelu recomputes the pre-activation through the forward entry point, which on the pipelined path takes
+    and frees its own large chunk buffer; the backward must not hold a pointer into memory that nested call frees."""
     _need_gpu()
     monkeypatch.setenv("TFGNN_B200_PIPE_CHUNK_ROWS", "128")     # forces the pipelined path with a large chunk buffer
     monkeypatch.setenv("TFGNN_B200_FUSED", "0")

@@ -43,20 +43,18 @@ int unsupported(const std::string& msg) {
 bool valid_act(int a) { return a >= TFGNN_ACT_NONE && a <= TFGNN_ACT_SIGMOID; }
 bool valid_agg(int a) { return a >= TFGNN_AGG_SUM && a <= TFGNN_AGG_SQRT_N; }
 
-// Node-level contraction C = epi(A B) with B [K,N] row-major in device memory.  The tensor-core path packs B into slot
-// kPackSlot of `batch`, or without a batch into a pool buffer freed after the GEMM.
-int node_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int N,
-                     int K, const GemmEpilogue& epi, int path, tfgnn_batch* batch, cudaStream_t st) {
-  bool want_tc = (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
+// Node-level contraction C = epi(A B) with B [K,N] row-major in device memory.  The tensor-core path packs B into a pool
+// buffer freed after the GEMM.
+int node_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int N, int K,
+              const GemmEpilogue& epi, int path, cudaStream_t st) {
+  const bool want_tc = (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
   const bool mul_ok = epi.mul == nullptr || (epi.ldm % 4 == 0 && (reinterpret_cast<uintptr_t>(epi.mul) & 15) == 0);
-  if (want_tc && mul_ok && gemm_tc_supported(M, N, K, A, lda, C, ldc)) {   // the packing kernel takes any ldb
-    void* packed = nullptr;
-    const size_t bytes = gemm_tc_packed_bytes(N, K);
-    int rc = batch ? batch_scratch(batch, kPackSlot, bytes, &packed) : pool_alloc(&packed, bytes, st);
-    if (rc) return rc;
-    rc = launch_pack_weights_tc(B, ldb, K, N, (float*)packed, st);
-    if (!rc) rc = launch_gemm_tc(A, lda, (const float*)packed, C, ldc, M, N, K, epi, st);
-    if (!batch) pool_free(packed, st);
+  const bool bias_ok = epi.bias == nullptr || (reinterpret_cast<uintptr_t>(epi.bias) & 15) == 0;   // float4 bias loads
+  if (want_tc && mul_ok && bias_ok && gemm_tc_supported(M, N, K, A, lda, C, ldc)) {   // the packing kernel takes any ldb
+    PoolBuffer packed{st};
+    int rc = packed.alloc(gemm_tc_packed_bytes(N, K));
+    if (!rc) rc = launch_pack_weights_tc(B, ldb, K, N, packed.f(), st);
+    if (!rc) rc = launch_gemm_tc(A, lda, packed.f(), C, ldc, M, N, K, epi, st);
     return rc;
   }
   if (path == TFGNN_PATH_SORTED_TC)
@@ -100,13 +98,14 @@ static int rgcn_pipelined(tfgnn_batch* b, const float* h, int D, const float* Wc
   const int kPipeChunkRows = pipe_chunk_rows();
   int rc = pipeline_init(b);
   if (rc) return rc;
-  void *A = nullptr, *packed = nullptr;
+  // A and the packed weights are allocated on `st` before the fork and freed on `st` by their destructors when this
+  // function returns, after `st` has waited on both join events: the frees are ordered after the last chunk on G and M.
+  // A failed launch inside the loop therefore still leaves through the join.
   const size_t a_chunk_elems = (size_t)kPipeChunkRows * K;
-  rc = batch_scratch(b, 2, a_chunk_elems * tfgnn_batch::kPipeBufs * sizeof(float), &A);
-  if (rc) return rc;
-  rc = batch_scratch(b, kPackSlot, gemm_tc_packed_bytes(H, K), &packed);
-  if (rc) return rc;
-  rc = launch_pack_weights_tc(Wcat, H, K, H, (float*)packed, st);
+  PoolBuffer A{st}, packed{st};
+  rc = A.alloc(a_chunk_elems * tfgnn_batch::kPipeBufs * sizeof(float));
+  if (!rc) rc = packed.alloc(gemm_tc_packed_bytes(H, K));
+  if (!rc) rc = launch_pack_weights_tc(Wcat, H, K, H, packed.f(), st);
   if (rc) return rc;
   cudaStream_t sg = b->pipe_gather, sm = b->pipe_gemm;
   TFGNN_CUDA(cudaEventRecord(b->ev_fork, st));
@@ -117,7 +116,7 @@ static int rgcn_pipelined(tfgnn_batch* b, const float* h, int D, const float* Wc
     const int buf = i % tfgnn_batch::kPipeBufs;
     const int v0 = i * kPipeChunkRows;
     const int vc = (V - v0 < kPipeChunkRows) ? V - v0 : kPipeChunkRows;
-    float* Abuf = (float*)A + (size_t)buf * a_chunk_elems;
+    float* Abuf = A.f() + (size_t)buf * a_chunk_elems;
     if (i >= tfgnn_batch::kPipeBufs) TFGNN_CUDA(cudaStreamWaitEvent(sg, b->ev_m[buf], 0));
     EdgeReduceParams p;
     p.X = h; p.ldx = D; p.x_type_stride = 0;
@@ -130,20 +129,20 @@ static int rgcn_pipelined(tfgnn_batch* b, const float* h, int D, const float* Wc
       return e && atoi(e) > 0 ? atoi(e) : 132 * 3;   // 3 lean CTAs/SM leave registers for the GEMM CTA
     }();
     rc = launch_edge_reduce(p, /*merged=*/false, sg, gather_cap);
-    if (rc) return rc;
+    if (rc) break;
     TFGNN_CUDA(cudaEventRecord(b->ev_g[buf], sg));
     TFGNN_CUDA(cudaStreamWaitEvent(sm, b->ev_g[buf], 0));
     GemmEpilogue epi = epi_in;
     epi.row0 = v0;
-    rc = launch_gemm_tc(Abuf, K, (const float*)packed, out + (size_t)v0 * ldo, ldo, vc, H, K, epi, sm);
-    if (rc) return rc;
+    rc = launch_gemm_tc(Abuf, K, packed.f(), out + (size_t)v0 * ldo, ldo, vc, H, K, epi, sm);
+    if (rc) break;
     TFGNN_CUDA(cudaEventRecord(b->ev_m[buf], sm));
   }
   TFGNN_CUDA(cudaEventRecord(b->ev_join_g, sg));
   TFGNN_CUDA(cudaEventRecord(b->ev_join_m, sm));
   TFGNN_CUDA(cudaStreamWaitEvent(st, b->ev_join_g, 0));
   TFGNN_CUDA(cudaStreamWaitEvent(st, b->ev_join_m, 0));
-  return 0;
+  return rc;
 }
 
 int agg_row_norm(int aggregation) {
@@ -151,34 +150,32 @@ int agg_row_norm(int aggregation) {
 }
 
 // The node-level half of the transform-then-aggregate form (no hidden layer; max aggregation and / or activation before
-// aggregation): P = h [W_0|..|W_{L-1}] over the Vs source rows (slot 2) and, with target-state input, T = h_tgt [W^t_0|..]
-// over the owned rows (slot 4), W_l = W.p[l].  *p becomes the merged edge reduce that forms the layer from them, out / ldo
-// unset:  out[v] = act_final(agg_e act_edge((P_l[u] + T_l[v]) s)).  The backward recomputes both through this function.
+// aggregation): P = h [W_0|..|W_{L-1}] over the Vs source rows and, with target-state input, T = h_tgt [W^t_0|..] over the
+// owned rows, W_l = W.p[l], into the caller's buffers.  *p becomes the merged edge reduce that forms the layer from them,
+// out / ldo unset:  out[v] = act_final(agg_e act_edge((P_l[u] + T_l[v]) s)).  The backward recomputes both through this
+// function.
 int transform_aggregate_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& W, int H, uint32_t flags,
-                               int aggregation, int activation, int path, EdgeReduceParams* p, cudaStream_t st) {
+                               int aggregation, int activation, int path, PoolBuffer& P, PoolBuffer& T,
+                               EdgeReduceParams* p, cudaStream_t st) {
   const int V = (int)b->V, Vs = (int)b->V_src, L = b->L, LH = L * H;
   const bool act_before = flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION;
-  void *P = nullptr, *Tt = nullptr, *Wcat = nullptr;
-  int rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &P);
-  if (rc) return rc;
-  rc = batch_scratch(b, 3, (size_t)D * LH * sizeof(float), &Wcat);
-  if (rc) return rc;
-  rc = launch_pack_horizontal(W, L, 0, D, H, H, (float*)Wcat, LH, st);
+  PoolBuffer Wcat{st};
+  int rc = P.alloc((size_t)Vs * LH * sizeof(float));
+  if (!rc) rc = Wcat.alloc((size_t)D * LH * sizeof(float));
+  if (!rc) rc = launch_pack_horizontal(W, L, 0, D, H, H, Wcat.f(), LH, st);
   if (rc) return rc;
   GemmEpilogue none;
-  rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
+  rc = node_gemm(h, D, Wcat.f(), LH, P.f(), LH, Vs, LH, D, none, path, st);
   if (rc) return rc;
   if (flags & TFGNN_FLAG_USE_TARGET_STATE) {
-    rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Tt);
-    if (rc) return rc;
-    rc = launch_pack_horizontal(W, L, D, D, H, H, (float*)Wcat, LH, st);
-    if (rc) return rc;
-    rc = node_gemm(h + (size_t)b->tgt_off * D, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, st);
+    rc = T.alloc((size_t)V * LH * sizeof(float));
+    if (!rc) rc = launch_pack_horizontal(W, L, D, D, H, H, Wcat.f(), LH, st);
+    if (!rc) rc = node_gemm(h + (size_t)b->tgt_off * D, D, Wcat.f(), LH, T.f(), LH, V, LH, D, none, path, st);
     if (rc) return rc;
   }
   *p = EdgeReduceParams{};
-  p->X = (const float*)P; p->ldx = LH; p->x_type_stride = H;
-  p->T = (const float*)Tt; p->ldt = LH; p->t_type_stride = H;
+  p->X = P.f(); p->ldx = LH; p->x_type_stride = H;
+  p->T = T.f(); p->ldt = LH; p->t_type_stride = H;
   p->row_ptr = b->row_ptr; p->src = b->src_sorted;
   p->V = V; p->L = L; p->C = H;
   p->normalize = (flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING) != 0;
@@ -240,9 +237,6 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
   if (n_hidden == 0 && sum_like && !act_before) {
     // ---- aggregate-then-transform ----
     const int K = L * D * (use_target ? 2 : 1);
-    void *A = nullptr, *Wcat = nullptr;
-    int rc = batch_scratch(b, 3, (size_t)K * H * sizeof(float), &Wcat);
-    if (rc) return rc;
     const bool pipelined = (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_FUSED_TC) && !use_target &&
                            V >= 2 * pipe_chunk_rows() && D % 4 == 0 &&
                            gemm_tc_supported(V, H, K, h, K, out, ldo) &&
@@ -252,13 +246,11 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
       return unsupported("TFGNN_PATH_FUSED_TC needs D % 32 == 0, 16 <= H <= 512 (H % 16 == 0; H > 64: <= 7 edge types), no target-state input");
     static const bool fused_auto = [] { const char* e = getenv("TFGNN_B200_FUSED"); return !e || atoi(e) != 0; }();
     if (fused_ok && (path == TFGNN_PATH_FUSED_TC || (path == TFGNN_PATH_AUTO && fused_auto))) {
-      void *packed = nullptr, *ring = nullptr;
-      rc = batch_scratch(b, kPackSlot, gemm_tc_packed_bytes(H, K), &packed);
-      if (rc) return rc;
-      rc = batch_scratch(b, 15, fused_rgcn_ring_bytes(D, L, H), &ring);
-      if (rc) return rc;
+      PoolBuffer packed{st}, ring{st};
       const int corr = fused_corr_bf16(activation);
-      rc = launch_pack_weights_tc_table(first, L, D, H, corr, (float*)packed, st);   // [W_0;..;W_{L-1}] -> K-major hi / correction
+      int rc = packed.alloc(gemm_tc_packed_bytes(H, K));
+      if (!rc) rc = ring.alloc(fused_rgcn_ring_bytes(D, L, H));
+      if (!rc) rc = launch_pack_weights_tc_table(first, L, D, H, corr, packed.f(), st);   // [W_0;..;W_{L-1}] -> K-major hi / correction
       if (rc) return rc;
       GemmEpilogue epi;
       epi.act = activation;
@@ -267,48 +259,52 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
         epi.ln_gamma = b->ln_gamma; epi.ln_beta = b->ln_beta; epi.ln_eps = b->ln_eps;
         b->ln_gamma = nullptr;         // consumed
       }
-      return launch_fused_rgcn(h, D, b->row_ptr, b->src_sorted, b->M_in, V, L, normalize, (const float*)packed, corr, H,
-                               (float*)ring, out, ldo, epi, st, b->peer_out, b->n_peer_out, b->mc_out);
+      return launch_fused_rgcn(h, D, b->row_ptr, b->src_sorted, b->M_in, V, L, normalize, packed.f(), corr, H, ring.f(),
+                               out, ldo, epi, st, b->peer_out, b->n_peer_out, b->mc_out);
     }
     if (b->n_peer_out > 0)
       return unsupported("rgcn_fwd_allgather: this shard does not take the fused kernel (need D % 32 == 0, 16 <= H <= 512, "
                          "H % 16 == 0, no target-state input)");
+    PoolBuffer Wcat{st};
+    int rc = Wcat.alloc((size_t)K * H * sizeof(float));
+    if (rc) return rc;
     if (pipelined) {
-      rc = launch_pack_vertical(first, L, 0, D, H, H, (float*)Wcat, H, 0, st);
+      rc = launch_pack_vertical(first, L, 0, D, H, H, Wcat.f(), H, 0, st);
       if (rc) return rc;
       GemmEpilogue epi;
       epi.act = activation;
       epi.row_norm = row_norm; epi.row_ptr = b->row_ptr; epi.V = V; epi.L = L;
-      return rgcn_pipelined(b, h, D, (const float*)Wcat, H, normalize, epi, out, ldo, st);
+      return rgcn_pipelined(b, h, D, Wcat.f(), H, normalize, epi, out, ldo, st);
     }
-    rc = batch_scratch(b, 2, (size_t)V * K * sizeof(float), &A);
+    PoolBuffer A{st};
+    rc = A.alloc((size_t)V * K * sizeof(float));
     if (rc) return rc;
     if (path == TFGNN_PATH_ATOMIC) {
       if (sharded) return unsupported("TFGNN_PATH_ATOMIC is not available on a target-range shard");
-      TFGNN_CUDA(cudaMemsetAsync(A, 0, (size_t)V * K * sizeof(float), st));
-      rc = launch_edge_scatter_atomic(b, h, D, D, normalize, (float*)A, K, D, st);
+      TFGNN_CUDA(cudaMemsetAsync(A.p, 0, (size_t)V * K * sizeof(float), st));
+      rc = launch_edge_scatter_atomic(b, h, D, D, normalize, A.f(), K, D, st);
       if (rc) return rc;
     } else {
       EdgeReduceParams p;
       p.X = h; p.ldx = D; p.x_type_stride = 0;
       p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-      p.out = (float*)A; p.ldo = K; p.out_type_stride = D;
+      p.out = A.f(); p.ldo = K; p.out_type_stride = D;
       p.V = V; p.L = L; p.C = D; p.normalize = normalize;
       rc = launch_edge_reduce(p, /*merged=*/false, st);
       if (rc) return rc;
     }
-    rc = launch_pack_vertical(first, L, 0, D, H, H, (float*)Wcat, H, 0, st);
+    rc = launch_pack_vertical(first, L, 0, D, H, H, Wcat.f(), H, 0, st);
     if (rc) return rc;
     if (use_target) {
-      rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, normalize, (float*)A, K, L * D, st);
+      rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, normalize, A.f(), K, L * D, st);
       if (rc) return rc;
-      rc = launch_pack_vertical(first, L, D, D, H, H, (float*)Wcat, H, L * D, st);
+      rc = launch_pack_vertical(first, L, D, D, H, H, Wcat.f(), H, L * D, st);
       if (rc) return rc;
     }
     GemmEpilogue epi;
     epi.act = activation;
     epi.row_norm = row_norm; epi.row_ptr = b->row_ptr; epi.V = V; epi.L = L;
-    return node_gemm((const float*)A, K, (const float*)Wcat, H, out, ldo, V, H, K, epi, path, b, st);
+    return node_gemm(A.f(), K, Wcat.f(), H, out, ldo, V, H, K, epi, path, st);
   }
 
   if (path == TFGNN_PATH_ATOMIC)
@@ -317,7 +313,8 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
   if (n_hidden == 0) {
     // ---- transform-then-aggregate (max aggregation and/or activation before aggregation) ----
     EdgeReduceParams p;
-    int rc = transform_aggregate_tables(b, h, D, first, H, flags, aggregation, activation, path, &p, st);
+    PoolBuffer P{st}, T{st};
+    int rc = transform_aggregate_tables(b, h, D, first, H, flags, aggregation, activation, path, P, T, &p, st);
     if (rc) return rc;
     p.out = out; p.ldo = ldo;
     return launch_edge_reduce(p, /*merged=*/true, st);
@@ -326,42 +323,40 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
   if (n_hidden == 1 && sum_like && !act_before) {
     // ---- hoisted hidden layer: per-edge relu on pre-projected tables, output layer per (v,l) ----
     const int LH = L * H;
-    void *Xs = nullptr, *Xt = nullptr, *Wcat = nullptr, *A = nullptr, *W2 = nullptr;
-    int rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &Xs);
+    PoolBuffer Xs{st}, Xt{st}, A{st}, W2{st};
+    int rc = Xs.alloc((size_t)Vs * LH * sizeof(float));
     if (rc) return rc;
-    rc = batch_scratch(b, 3, (size_t)(D > H ? D : H) * LH * sizeof(float), &Wcat);
-    if (rc) return rc;
-    rc = launch_pack_horizontal(first, L, 0, D, H, H, (float*)Wcat, LH, st);
-    if (rc) return rc;
-    GemmEpilogue none;
-    rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)Xs, LH, Vs, LH, D, none, path, b, st);
-    if (rc) return rc;
-    if (use_target) {
-      rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Xt);
+    {
+      PoolBuffer Wcat{st};
+      rc = Wcat.alloc((size_t)D * LH * sizeof(float));
+      if (!rc) rc = launch_pack_horizontal(first, L, 0, D, H, H, Wcat.f(), LH, st);
       if (rc) return rc;
-      rc = launch_pack_horizontal(first, L, D, D, H, H, (float*)Wcat, LH, st);
+      GemmEpilogue none;
+      rc = node_gemm(h, D, Wcat.f(), LH, Xs.f(), LH, Vs, LH, D, none, path, st);
       if (rc) return rc;
-      rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Xt, LH, V, LH, D, none, path, b, st);
-      if (rc) return rc;
+      if (use_target) {
+        rc = Xt.alloc((size_t)V * LH * sizeof(float));
+        if (!rc) rc = launch_pack_horizontal(first, L, D, D, H, H, Wcat.f(), LH, st);
+        if (!rc) rc = node_gemm(h_tgt, D, Wcat.f(), LH, Xt.f(), LH, V, LH, D, none, path, st);
+        if (rc) return rc;
+      }
     }
-    rc = batch_scratch(b, 5, (size_t)V * LH * sizeof(float), &A);
+    rc = A.alloc((size_t)V * LH * sizeof(float));
     if (rc) return rc;
     EdgeReduceParams p;
-    p.X = (const float*)Xs; p.ldx = LH; p.x_type_stride = H;
-    p.T = (const float*)Xt; p.ldt = LH; p.t_type_stride = H;
+    p.X = Xs.f(); p.ldx = LH; p.x_type_stride = H;
+    p.T = Xt.f(); p.ldt = LH; p.t_type_stride = H;
     p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-    p.out = (float*)A; p.ldo = LH; p.out_type_stride = H;
+    p.out = A.f(); p.ldo = LH; p.out_type_stride = H;
     p.V = V; p.L = L; p.C = H; p.normalize = normalize; p.hidden_relu = 1;
     rc = launch_edge_reduce(p, /*merged=*/false, st);
-    if (rc) return rc;
-    rc = batch_scratch(b, 7, (size_t)LH * H * sizeof(float), &W2);
-    if (rc) return rc;
-    rc = launch_pack_vertical(last, L, 0, H, H, H, (float*)W2, H, 0, st);
+    if (!rc) rc = W2.alloc((size_t)LH * H * sizeof(float));
+    if (!rc) rc = launch_pack_vertical(last, L, 0, H, H, H, W2.f(), H, 0, st);
     if (rc) return rc;
     GemmEpilogue epi;
     epi.act = activation;
     epi.row_norm = row_norm; epi.row_ptr = b->row_ptr; epi.V = V; epi.L = L;
-    return node_gemm((const float*)A, LH, (const float*)W2, H, out, ldo, V, H, LH, epi, path, b, st);
+    return node_gemm(A.f(), LH, W2.f(), H, out, ldo, V, H, LH, epi, path, st);
   }
 
   // edge MLP with >= 2 hidden layers, or hidden layers combined with max-aggregation /
@@ -451,20 +446,7 @@ extern "C" int tfgnn_b200_dense_fwd(const float* x, const float* W, float* out, 
   TFGNN_REQUIRE(valid_act(activation), "unknown activation code");
   if (V == 0) return 0;
   TFGNN_REQUIRE(x && W && out, "NULL pointer");
-  cudaStream_t st = (cudaStream_t)stream;
   GemmEpilogue epi;
   epi.act = activation;
-  const bool want_tc = path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC;
-  if (want_tc && gemm_tc_supported(V, N, K, x, K, out, N)) {
-    void* packed = nullptr;
-    int rc = pool_alloc(&packed, gemm_tc_packed_bytes(N, K), st);
-    if (rc) return rc;
-    rc = launch_pack_weights_tc(W, N, K, N, (float*)packed, st);
-    if (!rc) rc = launch_gemm_tc(x, K, (const float*)packed, out, N, V, N, K, epi, st);
-    pool_free(packed, st);
-    return rc;
-  }
-  if (path == TFGNN_PATH_SORTED_TC)
-    return unsupported("dense_fwd: shape not supported by the tensor-core GEMM (need N%16==0, K%32==0)");
-  return launch_gemm_simt(x, K, W, N, out, N, V, N, K, epi, st);
+  return node_gemm(x, K, W, N, out, N, V, N, K, epi, path, (cudaStream_t)stream);
 }

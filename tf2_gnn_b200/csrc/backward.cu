@@ -314,14 +314,14 @@ struct TransposedWeights {
 // C [M, N] = X WT (epilogue `epi`, node GEMM) after packing WT (pack_transposed_kernel): X [M, H] multiplies every type's
 // block side by side; stacked, X [M, L H] holds one block per type and the product sums over the types.
 static int gemm_transposed(const float* X, int ldx, const TransposedWeights& w, float* WT, float* C, int ldc, long long M,
-                           int N, const GemmEpilogue& epi, tfgnn_batch* b, cudaStream_t st) {
+                           int N, const GemmEpilogue& epi, cudaStream_t st) {
   if (w.stacked) {
     for (int l = 0; l < w.L; ++l) {
       pack_transposed_kernel<<<grid_for((long long)w.D * w.H), 256, 0, st>>>(one_table(w.W.p[l]), 1, w.D, w.H,
                                                                              WT + (size_t)l * w.H * w.D, w.D, 0, w.row0);
       TFGNN_LAUNCH_CHECK();
     }
-    return node_gemm(X, ldx, WT, w.D, C, ldc, M, N, w.L * w.H, epi, TFGNN_PATH_AUTO, b, st);
+    return node_gemm(X, ldx, WT, w.D, C, ldc, M, N, w.L * w.H, epi, TFGNN_PATH_AUTO, st);
   }
   const int LD = w.L * w.D;
   for (int p = 0; p < w.parts; ++p) {
@@ -329,7 +329,7 @@ static int gemm_transposed(const float* X, int ldx, const TransposedWeights& w, 
                                                                           w.row0 + p * w.D);
     TFGNN_LAUNCH_CHECK();
   }
-  return node_gemm(X, ldx, WT, w.parts * LD, C, ldc, M, N, w.H, epi, TFGNN_PATH_AUTO, b, st);
+  return node_gemm(X, ldx, WT, w.parts * LD, C, ldc, M, N, w.H, epi, TFGNN_PATH_AUTO, st);
 }
 
 // n gradient buffers p[0], p[step], p[2 step], .. of `floats` floats each
@@ -360,12 +360,11 @@ static int enter_both(tfgnn_batch* b, tfgnn_batch* bt, cudaStream_t st) {
 }
 
 // The start of a fused layer backward with owned rows and edge types: enters both batches and forms
-// dZ = dOut * act'(out) * rn(v) [V, H] in slot 8 of b.  For gelu, act' needs the pre-activation: `preact(z)` recomputes it
-// (the layer's forward without activation) into a pool buffer that is freed once dZ is formed, so no scratch pointer is held
-// across that nested forward call, which may regrow any slot.
+// dZ = dOut * act'(out) * rn(v) [V, H] in the caller's buffer dz.  For gelu, act' needs the pre-activation: `preact(z)`
+// recomputes it (the layer's forward without activation) into a pool buffer that is freed once dZ is formed.
 template <class Preact>
 static int begin_backward(tfgnn_batch* b, tfgnn_batch* bt, const float* out, const float* grad_out, int H, int activation,
-                          int aggregation, cudaStream_t st, float** dz, Preact preact) {
+                          int aggregation, cudaStream_t st, PoolBuffer& dz, Preact preact) {
   const long long V = b->V;
   int rc = enter_both(b, bt, st);
   if (rc) return rc;
@@ -376,12 +375,10 @@ static int begin_backward(tfgnn_batch* b, tfgnn_batch* bt, const float* out, con
     if (rc) return rc;
     out = z.f();
   }
-  void* d = nullptr;
-  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &d);
+  rc = dz.alloc((size_t)V * H * sizeof(float));
   if (rc) return rc;
-  *dz = (float*)d;
   act_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_out, out, V, H, activation, b->row_ptr, b->L,
-                                                   agg_row_norm(aggregation), *dz);
+                                                   agg_row_norm(aggregation), dz.f());
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -439,10 +436,11 @@ static int transform_aggregate_bwd(tfgnn_batch* b, tfgnn_batch* bt, const float*
   if (rc) return rc;
   // 1. P, T and (max) z, n
   EdgeReduceParams f;
-  rc = transform_aggregate_tables(b, h, D, wt, H, flags, aggregation, activation, TFGNN_PATH_AUTO, &f, st);
+  PoolBuffer P{st}, T{st};
+  rc = transform_aggregate_tables(b, h, D, wt, H, flags, aggregation, activation, TFGNN_PATH_AUTO, P, T, &f, st);
   if (rc) return rc;
   const int final_act = f.final_act;
-  PoolBuffer zn{st}, dP{st}, dT{st};
+  PoolBuffer zn{st}, dz{st}, dP{st}, dT{st};
   if (use_max) {
     rc = zn.alloc((size_t)2 * V * H * sizeof(float));   // z, then n
     if (rc) return rc;
@@ -452,49 +450,51 @@ static int transform_aggregate_bwd(tfgnn_batch* b, tfgnn_batch* bt, const float*
     if (rc) return rc;
   }
   const float* z = use_max ? zn.f() : nullptr;
-  void *dz = nullptr, *part = nullptr, *WT = nullptr;
-  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &dz);
-  if (rc) return rc;
-  rc = batch_scratch(b, 9, tn_partial_floats(Vs, D, H) * sizeof(float), &part);   // Vs >= V
-  if (rc) return rc;
-  rc = batch_scratch(b, 3, (size_t)LH * D * sizeof(float), &WT);
+  rc = dz.alloc((size_t)V * H * sizeof(float));
   if (rc) return rc;
   // 2. dZ (act_final' from the saved output, or for gelu from z)
   act_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_out, final_act == TFGNN_ACT_GELU ? z : out, V, H, final_act,
-                                                   b->row_ptr, L, f.row_norm, (float*)dz,
+                                                   b->row_ptr, L, f.row_norm, dz.f(),
                                                    use_max ? z + (size_t)V * H : nullptr);
   TFGNN_LAUNCH_CHECK();
   // 3. dP over the source-keyed CSR, dT over the forward's
   rc = dP.alloc((size_t)Vs * LH * sizeof(float));
   if (rc) return rc;
-  rc = launch_edge_grad(f, z, (const float*)dz, bt->row_ptr, bt->src_sorted, (int)Vs, dP.f(), st);
+  rc = launch_edge_grad(f, z, dz.f(), bt->row_ptr, bt->src_sorted, (int)Vs, dP.f(), st);
   if (rc) return rc;
   if (use_target) {
     rc = dT.alloc((size_t)V * LH * sizeof(float));
     if (rc) return rc;
-    rc = launch_edge_grad(f, z, (const float*)dz, nullptr, nullptr, 0, dT.f(), st);
+    rc = launch_edge_grad(f, z, dz.f(), nullptr, nullptr, 0, dT.f(), st);
     if (rc) return rc;
   }
   // 4. dW_l over all Vs rows, dW^t_l (rows [D, 2D) of W_l) over the owned rows
   const float* h_tgt = h + (size_t)lo * D;
-  for (int l = 0; l < L; ++l) {
-    const PtrTable gw = one_table(grad_W[l]);
-    rc = weight_grad(h, D, dP.f() + (size_t)l * H, LH, Vs, D, H, (float*)part, gw, 1, D, 0, st);
+  {
+    PoolBuffer part{st};
+    rc = part.alloc(tn_partial_floats(Vs, D, H) * sizeof(float));   // Vs >= V
     if (rc) return rc;
-    if (use_target) {
-      rc = weight_grad(h_tgt, D, dT.f() + (size_t)l * H, LH, V, D, H, (float*)part, gw, 1, D, D, st);
+    for (int l = 0; l < L; ++l) {
+      const PtrTable gw = one_table(grad_W[l]);
+      rc = weight_grad(h, D, dP.f() + (size_t)l * H, LH, Vs, D, H, part.f(), gw, 1, D, 0, st);
       if (rc) return rc;
+      if (use_target) {
+        rc = weight_grad(h_tgt, D, dT.f() + (size_t)l * H, LH, V, D, H, part.f(), gw, 1, D, D, st);
+        if (rc) return rc;
+      }
     }
   }
   if (!grad_h) return 0;
   // 5. grad_h = dP [W_0^T; ..] (K = L*H), then the owned rows += dT [W^t_0^T; ..]
-  rc = gemm_transposed(dP.f(), LH, {wt, L, D, H, 1, 0, /*stacked=*/true}, (float*)WT, grad_h, D, Vs, D, GemmEpilogue{},
-                       b, st);
+  PoolBuffer WT{st};
+  rc = WT.alloc((size_t)LH * D * sizeof(float));
+  if (!rc) rc = gemm_transposed(dP.f(), LH, {wt, L, D, H, 1, 0, /*stacked=*/true}, WT.f(), grad_h, D, Vs, D,
+                                GemmEpilogue{}, st);
   if (rc || !use_target) return rc;
   GemmEpilogue acc;
   acc.accumulate = 1;
-  return gemm_transposed(dT.f(), LH, {wt, L, D, H, 1, D, /*stacked=*/true}, (float*)WT, grad_h + (size_t)lo * D, D, V, D,
-                         acc, b, st);
+  return gemm_transposed(dT.f(), LH, {wt, L, D, H, 1, D, /*stacked=*/true}, WT.f(), grad_h + (size_t)lo * D, D, V, D,
+                         acc, st);
 }
 
 }  // namespace tfgnn
@@ -535,17 +535,13 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   if (transform_aggregate)
     return transform_aggregate_bwd(b, bt, h, D, wt, grad_W, H, flags, aggregation, activation, out, grad_out, grad_h, st);
   // 1. dZ = dOut * act'(out) * rn(v)
-  float* dz = nullptr;
-  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, &dz, [&](float* z) {
+  PoolBuffer dz{st};
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, dz, [&](float* z) {
     return edge_mlp_core(b, h, D, W, 0, H, flags, aggregation, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, z, H, st);
   });
   if (rc) return rc;
-  void *A = nullptr, *WT = nullptr, *part = nullptr;
-  rc = batch_scratch(b, 2, (size_t)V * K * sizeof(float), &A);     // A (forward operand), then dA
-  if (rc) return rc;
-  rc = batch_scratch(b, 3, (size_t)K * H * sizeof(float), &WT);
-  if (rc) return rc;
-  rc = batch_scratch(b, 9, tn_partial_floats(V, K, H) * sizeof(float), &part);
+  PoolBuffer A{st};   // A (forward operand), then dA
+  rc = A.alloc((size_t)V * K * sizeof(float));
   if (rc) return rc;
 
   // 2. A_l (recomputed, normalised) and dW = A^T dZ
@@ -553,29 +549,37 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     EdgeReduceParams p;
     p.X = h; p.ldx = D; p.x_type_stride = 0;
     p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-    p.out = (float*)A; p.ldo = K; p.out_type_stride = D;
+    p.out = A.f(); p.ldo = K; p.out_type_stride = D;
     p.V = (int)V; p.L = L; p.C = D; p.normalize = normalize;
     rc = launch_edge_reduce(p, /*merged=*/false, st);
     if (rc) return rc;
   }
   if (use_target) {
-    rc = launch_target_term(h_tgt, D, b->row_ptr, (int)V, L, D, normalize, (float*)A, K, LD, st);
+    rc = launch_target_term(h_tgt, D, b->row_ptr, (int)V, L, D, normalize, A.f(), K, LD, st);
     if (rc) return rc;
   }
-  rc = weight_grad((const float*)A, K, dz, H, V, K, H, (float*)part, gwt, L, D, 0, st);
-  if (rc || !grad_h) return rc;
+  {
+    PoolBuffer part{st};
+    rc = part.alloc(tn_partial_floats(V, K, H) * sizeof(float));
+    if (!rc) rc = weight_grad(A.f(), K, dz.f(), H, V, K, H, part.f(), gwt, L, D, 0, st);
+    if (rc || !grad_h) return rc;
+  }
   // 3. dA = dZ Wcat^T (overwrites A), scaled per (v,l)
-  rc = gemm_transposed(dz, H, {wt, L, D, H, use_target ? 2 : 1}, (float*)WT, (float*)A, K, V, K, GemmEpilogue{}, b, st);
-  if (rc) return rc;
+  {
+    PoolBuffer WT{st};
+    rc = WT.alloc((size_t)K * H * sizeof(float));
+    if (!rc) rc = gemm_transposed(dz.f(), H, {wt, L, D, H, use_target ? 2 : 1}, WT.f(), A.f(), K, V, K, GemmEpilogue{}, st);
+    if (rc) return rc;
+  }
   if (normalize) {
-    scale_by_type_kernel<<<grid_for(V * LD), 256, 0, st>>>((float*)A, K, V, L, D, b->row_ptr);
+    scale_by_type_kernel<<<grid_for(V * LD), 256, 0, st>>>(A.f(), K, V, L, D, b->row_ptr);
     TFGNN_LAUNCH_CHECK();
   }
   // 4. dh[u] = sum over the edges LEAVING u
-  rc = reduce_over_sources(bt, (const float*)A, K, D, Vs, grad_h, st);
+  rc = reduce_over_sources(bt, A.f(), K, D, Vs, grad_h, st);
   if (rc) return rc;
   if (use_target) {   // 5. the target half: grad_h[lo + v] += sum_l coeff(v,l) * dT_l[v]
-    target_term_bwd_kernel<<<grid_for(V * D), 256, 0, st>>>((const float*)A + LD, K, b->row_ptr, V, L, D, normalize,
+    target_term_bwd_kernel<<<grid_for(V * D), 256, 0, st>>>(A.f() + LD, K, b->row_ptr, V, L, D, normalize,
                                                             grad_h + (size_t)lo * D);
     TFGNN_LAUNCH_CHECK();
   }
@@ -618,67 +622,61 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
   const float* h_tgt = h + (size_t)lo * D;
   const int chunks = tn_chunks(V);
-  void *agg = nullptr, *gx = nullptr, *gh = nullptr, *dagg = nullptr, *wT = nullptr, *part = nullptr, *dhd = nullptr,
-       *tmp = nullptr;
   int rc = enter_both(b, bt, st);
   if (rc) return rc;
-  rc = batch_scratch(b, 11, (size_t)V * H * sizeof(float), &agg);
+  PoolBuffer dagg{st}, dhd{st}, tmp{st};
+  rc = dagg.alloc((size_t)V * H * sizeof(float));
+  if (!rc) rc = dhd.alloc((size_t)V * H * sizeof(float));
+  if (!rc) rc = tmp.alloc((size_t)V * H * sizeof(float));
   if (rc) return rc;
-  rc = batch_scratch(b, 12, (size_t)V * N3 * sizeof(float), &gx);
-  if (rc) return rc;
-  rc = batch_scratch(b, 13, (size_t)V * N3 * sizeof(float), &gh);
-  if (rc) return rc;
-  rc = batch_scratch(b, 14, (size_t)V * H * sizeof(float), &dagg);
-  if (rc) return rc;
-  rc = batch_scratch(b, 7, (size_t)N3 * H * sizeof(float), &wT);
-  if (rc) return rc;
-  rc = batch_scratch(b, 10, (tn_partial_floats(V, H, N3) + (size_t)chunks * N3) * sizeof(float), &part);
-  if (rc) return rc;
-  rc = batch_scratch(b, 4, (size_t)V * H * sizeof(float), &dhd);
-  if (rc) return rc;
-  rc = batch_scratch(b, 5, (size_t)V * H * sizeof(float), &tmp);
-  if (rc) return rc;
-  // 1. forward quantities: agg (no message activation, ggnn.py:68-83), gx, gh
-  rc = edge_mlp_core(b, h, D, W, 0, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION, aggregation, TFGNN_ACT_NONE,
-                     TFGNN_PATH_AUTO, (float*)agg, H, st);
-  if (rc) return rc;
-  GemmEpilogue e0, e1;
-  e0.bias = gru_bias;
-  e1.bias = gru_bias + N3;
-  rc = node_gemm((const float*)agg, H, gru_kernel, N3, (float*)gx, N3, V, N3, H, e0, TFGNN_PATH_AUTO, b, st);
-  if (rc) return rc;
-  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, N3, (float*)gh, N3, V, N3, H, e1, TFGNN_PATH_AUTO, b, st);
-  if (rc) return rc;
-  // 2. gates, in place
-  gru_gate_bwd_kernel<<<grid_for(V * H), 256, 0, st>>>((const float*)gx, (const float*)gh, h_tgt, D, grad_out, V, H,
-                                                       (float*)gx, (float*)gh, (float*)dhd);
-  TFGNN_LAUNCH_CHECK();
-  // 3. bias gradients: rows 0 / 1 of gru_bias belong to gx / gh
-  float* cpart = (float*)part + tn_partial_floats(V, H, N3);
-  rc = column_sums((const float*)gx, V, N3, grad_gru_bias, cpart, st);
-  if (rc) return rc;
-  rc = column_sums((const float*)gh, V, N3, grad_gru_bias + N3, cpart, st);
-  if (rc) return rc;
-  // 4. dK = agg^T dgx, dU = h^T dgh
-  rc = weight_grad((const float*)agg, H, (const float*)gx, N3, V, H, N3, (float*)part, one_table(grad_gru_kernel), 1, H, 0,
-                   st);
-  if (rc) return rc;
-  rc = weight_grad(h_tgt, D, (const float*)gh, N3, V, H, N3, (float*)part, one_table(grad_gru_recurrent_kernel), 1, H, 0,
-                   st);
-  if (rc) return rc;
-  // 5. dagg = dgx K^T, dh_rec = dgh U^T
-  rc = gemm_transposed((const float*)gx, N3, {one_table(gru_kernel), 1, H, N3}, (float*)wT, (float*)dagg, H, V, H,
-                       GemmEpilogue{}, b, st);
-  if (rc) return rc;
-  rc = gemm_transposed((const float*)gh, N3, {one_table(gru_recurrent_kernel), 1, H, N3}, (float*)wT, (float*)tmp, H, V,
-                       H, GemmEpilogue{}, b, st);
-  if (rc) return rc;
+  {
+    // the forward quantities and the GRU's own gradients are freed before the message backward below
+    PoolBuffer agg{st}, gx{st}, gh{st}, wT{st}, part{st};
+    rc = agg.alloc((size_t)V * H * sizeof(float));
+    if (!rc) rc = gx.alloc((size_t)V * N3 * sizeof(float));
+    if (!rc) rc = gh.alloc((size_t)V * N3 * sizeof(float));
+    if (!rc) rc = wT.alloc((size_t)N3 * H * sizeof(float));
+    if (!rc) rc = part.alloc((tn_partial_floats(V, H, N3) + (size_t)chunks * N3) * sizeof(float));
+    if (rc) return rc;
+    // 1. forward quantities: agg (no message activation, ggnn.py:68-83), gx, gh
+    rc = edge_mlp_core(b, h, D, W, 0, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION, aggregation, TFGNN_ACT_NONE,
+                       TFGNN_PATH_AUTO, agg.f(), H, st);
+    if (rc) return rc;
+    GemmEpilogue e0, e1;
+    e0.bias = gru_bias;
+    e1.bias = gru_bias + N3;
+    rc = node_gemm(agg.f(), H, gru_kernel, N3, gx.f(), N3, V, N3, H, e0, TFGNN_PATH_AUTO, st);
+    if (rc) return rc;
+    rc = node_gemm(h_tgt, D, gru_recurrent_kernel, N3, gh.f(), N3, V, N3, H, e1, TFGNN_PATH_AUTO, st);
+    if (rc) return rc;
+    // 2. gates, in place
+    gru_gate_bwd_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), gh.f(), h_tgt, D, grad_out, V, H, gx.f(), gh.f(),
+                                                         dhd.f());
+    TFGNN_LAUNCH_CHECK();
+    // 3. bias gradients: rows 0 / 1 of gru_bias belong to gx / gh
+    float* cpart = part.f() + tn_partial_floats(V, H, N3);
+    rc = column_sums(gx.f(), V, N3, grad_gru_bias, cpart, st);
+    if (rc) return rc;
+    rc = column_sums(gh.f(), V, N3, grad_gru_bias + N3, cpart, st);
+    if (rc) return rc;
+    // 4. dK = agg^T dgx, dU = h^T dgh
+    rc = weight_grad(agg.f(), H, gx.f(), N3, V, H, N3, part.f(), one_table(grad_gru_kernel), 1, H, 0, st);
+    if (rc) return rc;
+    rc = weight_grad(h_tgt, D, gh.f(), N3, V, H, N3, part.f(), one_table(grad_gru_recurrent_kernel), 1, H, 0, st);
+    if (rc) return rc;
+    // 5. dagg = dgx K^T, dh_rec = dgh U^T
+    rc = gemm_transposed(gx.f(), N3, {one_table(gru_kernel), 1, H, N3}, wT.f(), dagg.f(), H, V, H, GemmEpilogue{}, st);
+    if (rc) return rc;
+    rc = gemm_transposed(gh.f(), N3, {one_table(gru_recurrent_kernel), 1, H, N3}, wT.f(), tmp.f(), H, V, H,
+                         GemmEpilogue{}, st);
+    if (rc) return rc;
+  }
   // 6. messages: dagg -> grad_h (through the edges) and grad_W
   rc = tfgnn_b200_rgcn_bwd(b, bt, h, D, W, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION, aggregation, TFGNN_ACT_NONE,
-                           (const float*)dagg, (const float*)dagg, grad_h, grad_W, stream);
+                           dagg.f(), dagg.f(), grad_h, grad_W, stream);
   if (rc) return rc;
   // 7. grad_h[lo + v] += dh_direct + dh_rec
-  add3_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dhd, (const float*)tmp, V * H);
+  add3_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_h + (size_t)lo * D, dhd.f(), tmp.f(), V * H);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -705,7 +703,7 @@ extern "C" int tfgnn_b200_gru_gate_bwd(const float* gx, const float* gh, const f
 //   dW_l = [A_l | T_l]^T dQ_l,   dF_l = h_v^T [dgamma_l | dbeta_l]          (TN, fixed 8192-row chunks)
 //   dA_l = s dQ_l W^s_l^T       -> grad_h[u] through the source-keyed CSR (all types merged, no atomics)
 //   grad_h[v] += [dgamma_l | dbeta_l] F_l^T (+ c s dQ_l W^t_l^T)            (owned rows)
-// Every per-type temporary is [V, D], [V, H] or [V, 2H]; only dA holds all types ([V, L*D], the forward's slot-2 table).
+// Every per-type temporary is [V, D], [V, H] or [V, 2H]; only dA holds all types ([V, L*D]).
 // =====================================================================================================================
 namespace tfgnn {
 
@@ -760,35 +758,29 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
   const int LD = L * D;
   // 1. dZ = dOut * act'(out) * rn(v)
-  float* dz = nullptr;
-  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, &dz, [&](float* z) {
+  PoolBuffer dz{st};
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, dz, [&](float* z) {
     return tfgnn_b200_film_fwd(b, h, D, mlp_weights, 0, film_weights, H, flags, aggregation, TFGNN_ACT_NONE,
                                TFGNN_PATH_AUTO, z, stream);
   });
   if (rc) return rc;
-  void *AT = nullptr, *dQ = nullptr, *dGB = nullptr, *part = nullptr;
-  void *dA = nullptr, *dHt = nullptr, *WT = nullptr, *FT = nullptr;
-  rc = batch_scratch(b, 4, (size_t)V * KT * sizeof(float), &AT);   // [A_l | T_l], later dT_l
+  PoolBuffer AT{st}, dQ{st}, dGB{st}, part{st};
+  rc = AT.alloc((size_t)V * KT * sizeof(float));                                       // [A_l | T_l], later dT_l
+  if (!rc) rc = dQ.alloc((size_t)V * H * sizeof(float));
+  if (!rc) rc = dGB.alloc((size_t)V * 2 * H * sizeof(float));                          // [dgamma_l | dbeta_l]
+  if (!rc) rc = part.alloc(tn_partial_floats(V, D, 2 * H) * sizeof(float));   // KT * H <= D * 2H
   if (rc) return rc;
-  rc = batch_scratch(b, 5, (size_t)V * H * sizeof(float), &dQ);
-  if (rc) return rc;
-  rc = batch_scratch(b, 11, (size_t)V * 2 * H * sizeof(float), &dGB);   // [dgamma_l | dbeta_l]
-  if (rc) return rc;
-  rc = batch_scratch(b, 9, tn_partial_floats(V, D, 2 * H) * sizeof(float), &part);   // KT * H <= D * 2H
-  if (rc) return rc;
+  PoolBuffer dA{st}, dHt{st}, WT{st}, FT{st};
   if (grad_h) {
-    rc = batch_scratch(b, 2, (size_t)V * LD * sizeof(float), &dA);
-    if (rc) return rc;
-    rc = batch_scratch(b, 13, (size_t)V * D * sizeof(float), &dHt);   // target-side terms of grad_h, summed over types
-    if (rc) return rc;
-    rc = batch_scratch(b, 7, (size_t)H * KT * sizeof(float), &WT);
-    if (rc) return rc;
-    rc = batch_scratch(b, 3, (size_t)2 * H * D * sizeof(float), &FT);
+    rc = dA.alloc((size_t)V * LD * sizeof(float));
+    if (!rc) rc = dHt.alloc((size_t)V * D * sizeof(float));   // target-side terms of grad_h, summed over types
+    if (!rc) rc = WT.alloc((size_t)H * KT * sizeof(float));
+    if (!rc) rc = FT.alloc((size_t)2 * H * D * sizeof(float));
     if (rc) return rc;
   }
 
   GemmEpilogue none, by_dz;
-  by_dz.mul = dz;
+  by_dz.mul = dz.f();
   by_dz.ldm = H;
   for (int l = 0; l < L; ++l) {
     const int* rp = b->row_ptr + (size_t)l * V;   // the V segments of type l
@@ -799,55 +791,53 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
       EdgeReduceParams p;
       p.X = h; p.ldx = D; p.x_type_stride = 0;
       p.row_ptr = rp; p.src = b->src_sorted;
-      p.out = (float*)AT; p.ldo = KT; p.out_type_stride = 0;
+      p.out = AT.f(); p.ldo = KT; p.out_type_stride = 0;
       p.V = (int)V; p.L = 1; p.C = D; p.normalize = normalize;
       rc = launch_edge_reduce(p, /*merged=*/false, st);
       if (rc) return rc;
       if (use_target) {
-        rc = launch_target_term(h_tgt, D, rp, (int)V, 1, D, normalize, (float*)AT, KT, D, st);
+        rc = launch_target_term(h_tgt, D, rp, (int)V, 1, D, normalize, AT.f(), KT, D, st);
         if (rc) return rc;
       }
     }
     // 3. dQ_l = dZ * (h_v Fgamma_l);  dgamma_l = dZ * ([A_l | T_l] W_l);  dbeta_l = c dZ
-    rc = node_gemm(h_tgt, D, Fl, 2 * H, (float*)dQ, H, V, H, D, by_dz, TFGNN_PATH_AUTO, b, st);
+    rc = node_gemm(h_tgt, D, Fl, 2 * H, dQ.f(), H, V, H, D, by_dz, TFGNN_PATH_AUTO, st);
     if (rc) return rc;
-    rc = node_gemm((const float*)AT, KT, Wl, H, (float*)dGB, 2 * H, V, H, KT, by_dz, TFGNN_PATH_AUTO, b, st);
+    rc = node_gemm(AT.f(), KT, Wl, H, dGB.f(), 2 * H, V, H, KT, by_dz, TFGNN_PATH_AUTO, st);
     if (rc) return rc;
-    film_beta_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(dz, rp, V, H, (float*)dGB);
+    film_beta_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(dz.f(), rp, V, H, dGB.f());
     TFGNN_LAUNCH_CHECK();
     // 4. dW_l = [A_l | T_l]^T dQ_l,  dF_l = h_v^T [dgamma_l | dbeta_l]
-    rc = weight_grad((const float*)AT, KT, (const float*)dQ, H, V, KT, H, (float*)part, one_table(grad_W[l]), 1, KT, 0, st);
+    rc = weight_grad(AT.f(), KT, dQ.f(), H, V, KT, H, part.f(), one_table(grad_W[l]), 1, KT, 0, st);
     if (rc) return rc;
-    rc = weight_grad(h_tgt, D, (const float*)dGB, 2 * H, V, D, 2 * H, (float*)part, one_table(grad_film[l]), 1, D, 0, st);
+    rc = weight_grad(h_tgt, D, dGB.f(), 2 * H, V, D, 2 * H, part.f(), one_table(grad_film[l]), 1, D, 0, st);
     if (rc) return rc;
     if (!grad_h) continue;
     // 5. dA_l = dQ_l W^s_l^T into columns [l*D, (l+1)*D) of dA (scaled by s after the loop)
-    rc = gemm_transposed((const float*)dQ, H, {one_table(Wl), 1, KT, H}, (float*)WT, (float*)dA + (size_t)l * D, LD, V, D,
-                         none, b, st);
+    rc = gemm_transposed(dQ.f(), H, {one_table(Wl), 1, KT, H}, WT.f(), dA.f() + (size_t)l * D, LD, V, D, none, st);
     if (rc) return rc;
     // 6. target side: dHt (+)= [dgamma_l | dbeta_l] F_l^T (+ coeff(v,l) dQ_l W^t_l^T)
     GemmEpilogue sum_types;
     sum_types.accumulate = l > 0;
-    rc = gemm_transposed((const float*)dGB, 2 * H, {one_table(Fl), 1, D, 2 * H}, (float*)FT, (float*)dHt, D, V, D,
-                         sum_types, b, st);
+    rc = gemm_transposed(dGB.f(), 2 * H, {one_table(Fl), 1, D, 2 * H}, FT.f(), dHt.f(), D, V, D, sum_types, st);
     if (rc) return rc;
     if (use_target) {   // dT_l overwrites [A_l | T_l] (read for the last time by the dW_l pass above); W^t_l^T is packed
-      rc = node_gemm((const float*)dQ, H, (const float*)WT + D, KT, (float*)AT, KT, V, D, H, none, TFGNN_PATH_AUTO, b, st);
+      rc = node_gemm(dQ.f(), H, WT.f() + D, KT, AT.f(), KT, V, D, H, none, TFGNN_PATH_AUTO, st);
       if (rc) return rc;
-      target_term_bwd_kernel<<<grid_for(V * D), 256, 0, st>>>((const float*)AT, KT, rp, V, 1, D, normalize, (float*)dHt);
+      target_term_bwd_kernel<<<grid_for(V * D), 256, 0, st>>>(AT.f(), KT, rp, V, 1, D, normalize, dHt.f());
       TFGNN_LAUNCH_CHECK();
     }
   }
   if (!grad_h) return 0;
   if (normalize) {
-    scale_by_type_kernel<<<grid_for(V * LD), 256, 0, st>>>((float*)dA, LD, V, L, D, b->row_ptr);
+    scale_by_type_kernel<<<grid_for(V * LD), 256, 0, st>>>(dA.f(), LD, V, L, D, b->row_ptr);
     TFGNN_LAUNCH_CHECK();
   }
   // 7. grad_h[u] = sum over the edges LEAVING u
-  rc = reduce_over_sources(bt, (const float*)dA, LD, D, Vs, grad_h, st);
+  rc = reduce_over_sources(bt, dA.f(), LD, D, Vs, grad_h, st);
   if (rc) return rc;
   // 8. grad_h[lo + v] += target-side terms
-  add_kernel<<<grid_for(V * D), 256, 0, st>>>(grad_h + (size_t)lo * D, (const float*)dHt, V * D);
+  add_kernel<<<grid_for(V * D), 256, 0, st>>>(grad_h + (size_t)lo * D, dHt.f(), V * D);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -1072,96 +1062,86 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
   const int LH = L * H;
   // 1. dZ = dOut * act'(out) * rn(v)
-  float* dz = nullptr;
-  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, &dz, [&](float* z) {
+  PoolBuffer dz{st};
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, dz, [&](float* z) {
     return edge_mlp_core(b, h, D, mlp_weights, 1, H, flags, aggregation, TFGNN_ACT_NONE, TFGNN_PATH_AUTO, z, H, st);
   });
   if (rc) return rc;
-  void *Xs = nullptr, *Xt = nullptr, *A = nullptr, *cnt = nullptr, *dXs = nullptr, *Wp = nullptr, *W2T = nullptr,
-       *part = nullptr;
-  rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &Xs);   // the forward's slots for Xs, Xt, A, Wcat, W2
-  if (rc) return rc;
-  rc = batch_scratch(b, 5, (size_t)V * LH * sizeof(float), &A);      // A, then dA
-  if (rc) return rc;
-  rc = batch_scratch(b, 3, (size_t)(D > H ? D : H) * LH * sizeof(float), &Wp);   // [D, LH] packs, then [LH, D]
-  if (rc) return rc;
-  rc = batch_scratch(b, 7, (size_t)LH * H * sizeof(float), &W2T);
-  if (rc) return rc;
-  rc = batch_scratch(b, 13, (size_t)Vs * LH * sizeof(float), &dXs);
-  if (rc) return rc;
-  if (use_target) {
-    rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Xt);
-    if (rc) return rc;
-    rc = batch_scratch(b, 11, (size_t)V * LH * sizeof(float), &cnt);   // cnt, then dXt
-    if (rc) return rc;
-  }
-  {
+  PoolBuffer Xs{st}, Xt{st}, A{st}, cnt{st}, dXs{st}, Wp{st}, part{st};
+  rc = Xs.alloc((size_t)Vs * LH * sizeof(float));
+  if (!rc) rc = A.alloc((size_t)V * LH * sizeof(float));                              // A, then dA
+  if (!rc) rc = Wp.alloc((size_t)(D > H ? D : H) * LH * sizeof(float));               // [D, LH] packs, then [LH, D]
+  if (!rc) rc = dXs.alloc((size_t)Vs * LH * sizeof(float));
+  if (!rc && use_target) rc = Xt.alloc((size_t)V * LH * sizeof(float));
+  if (!rc && use_target) rc = cnt.alloc((size_t)V * LH * sizeof(float));              // cnt, then dXt
+  if (!rc) {
     const size_t a = tn_partial_floats(V, LH, H), c = tn_partial_floats(Vs, D, H);
-    rc = batch_scratch(b, 9, (a > c ? a : c) * sizeof(float), &part);
-    if (rc) return rc;
+    rc = part.alloc((a > c ? a : c) * sizeof(float));
   }
+  if (rc) return rc;
 
   // 2. Xs, Xt and A_l (+ cnt_l) recomputed with the forward's GEMMs and summation order
   GemmEpilogue none;
-  rc = launch_pack_horizontal(us, L, 0, D, H, H, (float*)Wp, LH, st);
+  rc = launch_pack_horizontal(us, L, 0, D, H, H, Wp.f(), LH, st);
   if (rc) return rc;
-  rc = node_gemm(h, D, (const float*)Wp, LH, (float*)Xs, LH, Vs, LH, D, none, TFGNN_PATH_AUTO, b, st);
+  rc = node_gemm(h, D, Wp.f(), LH, Xs.f(), LH, Vs, LH, D, none, TFGNN_PATH_AUTO, st);
   if (rc) return rc;
   if (use_target) {
-    rc = launch_pack_horizontal(us, L, D, D, H, H, (float*)Wp, LH, st);
+    rc = launch_pack_horizontal(us, L, D, D, H, H, Wp.f(), LH, st);
     if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Wp, LH, (float*)Xt, LH, V, LH, D, none, TFGNN_PATH_AUTO, b, st);
+    rc = node_gemm(h_tgt, D, Wp.f(), LH, Xt.f(), LH, V, LH, D, none, TFGNN_PATH_AUTO, st);
     if (rc) return rc;
-    rc = launch_hidden_relu_count((const float*)Xs, (const float*)Xt, b->row_ptr, b->src_sorted, (int)V, L, H, normalize,
-                                  (float*)A, (float*)cnt, st);
+    rc = launch_hidden_relu_count(Xs.f(), Xt.f(), b->row_ptr, b->src_sorted, (int)V, L, H, normalize, A.f(), cnt.f(), st);
     if (rc) return rc;
   } else {
     EdgeReduceParams p;
-    p.X = (const float*)Xs; p.ldx = LH; p.x_type_stride = H;
+    p.X = Xs.f(); p.ldx = LH; p.x_type_stride = H;
     p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-    p.out = (float*)A; p.ldo = LH; p.out_type_stride = H;
+    p.out = A.f(); p.ldo = LH; p.out_type_stride = H;
     p.V = (int)V; p.L = L; p.C = H; p.normalize = normalize; p.hidden_relu = 1;
     rc = launch_edge_reduce(p, /*merged=*/false, st);
     if (rc) return rc;
   }
   // 3. dW2_l = A_l^T dZ
-  rc = weight_grad((const float*)A, LH, dz, H, V, LH, H, (float*)part, gw2, L, H, 0, st);
+  rc = weight_grad(A.f(), LH, dz.f(), H, V, LH, H, part.f(), gw2, L, H, 0, st);
   if (rc) return rc;
   // 4. dA = dZ [W2_0; ..]^T (overwrites A), dA_l[v] *= s_{v,l}
-  rc = gemm_transposed(dz, H, {w2, L, H, H}, (float*)W2T, (float*)A, LH, V, LH, none, b, st);
-  if (rc) return rc;
+  {
+    PoolBuffer W2T{st};
+    rc = W2T.alloc((size_t)LH * H * sizeof(float));
+    if (!rc) rc = gemm_transposed(dz.f(), H, {w2, L, H, H}, W2T.f(), A.f(), LH, V, LH, none, st);
+    if (rc) return rc;
+  }
   if (normalize) {
-    scale_by_type_kernel<<<grid_for(V * LH), 256, 0, st>>>((float*)A, LH, V, L, H, b->row_ptr);
+    scale_by_type_kernel<<<grid_for(V * LH), 256, 0, st>>>(A.f(), LH, V, L, H, b->row_ptr);
     TFGNN_LAUNCH_CHECK();
   }
   // 5. dXs over the source-keyed CSR (on a shard: its owned transpose, every global source, local target ids);
   //    dXt = dA * cnt in place of cnt
-  rc = launch_hidden_relu_src_bwd((const float*)Xs, (const float*)Xt, (const float*)A, bt->row_ptr, bt->src_sorted,
-                                  (int)Vs, L, H, (float*)dXs, st);
+  rc = launch_hidden_relu_src_bwd(Xs.f(), Xt.f(), A.f(), bt->row_ptr, bt->src_sorted, (int)Vs, L, H, dXs.f(), st);
   if (rc) return rc;
   if (use_target) {
-    mul_inplace_kernel<<<grid_for(V * LH), 256, 0, st>>>((float*)cnt, (const float*)A, V * LH);
+    mul_inplace_kernel<<<grid_for(V * LH), 256, 0, st>>>(cnt.f(), A.f(), V * LH);
     TFGNN_LAUNCH_CHECK();
   }
   // 6. dU^s_l = h^T dXs_l over all Vs rows, dU^t_l = h_v^T dXt_l over the owned rows (rows [D, 2D) of U_l)
   for (int l = 0; l < L; ++l) {
     const PtrTable gu = one_table(grad_weights[2 * l]);
-    rc = weight_grad(h, D, (const float*)dXs + (size_t)l * H, LH, Vs, D, H, (float*)part, gu, 1, D, 0, st);
+    rc = weight_grad(h, D, dXs.f() + (size_t)l * H, LH, Vs, D, H, part.f(), gu, 1, D, 0, st);
     if (rc) return rc;
     if (use_target) {
-      rc = weight_grad(h_tgt, D, (const float*)cnt + (size_t)l * H, LH, V, D, H, (float*)part, gu, 1, D, D, st);
+      rc = weight_grad(h_tgt, D, cnt.f() + (size_t)l * H, LH, V, D, H, part.f(), gu, 1, D, D, st);
       if (rc) return rc;
     }
   }
   if (!grad_h) return 0;
   // 7. grad_h = dXs [U^s_0^T; ..] (K = L*H), then the owned rows += dXt [U^t_0^T; ..]
-  rc = gemm_transposed((const float*)dXs, LH, {us, L, D, H, 1, 0, /*stacked=*/true}, (float*)Wp, grad_h, D, Vs, D, none,
-                       b, st);
+  rc = gemm_transposed(dXs.f(), LH, {us, L, D, H, 1, 0, /*stacked=*/true}, Wp.f(), grad_h, D, Vs, D, none, st);
   if (rc || !use_target) return rc;
   GemmEpilogue acc;
   acc.accumulate = 1;
-  return gemm_transposed((const float*)cnt, LH, {us, L, D, H, 1, D, /*stacked=*/true}, (float*)Wp, grad_h + (size_t)lo * D,
-                         D, V, D, acc, b, st);
+  return gemm_transposed(cnt.f(), LH, {us, L, D, H, 1, D, /*stacked=*/true}, Wp.f(), grad_h + (size_t)lo * D, D, V, D, acc,
+                         st);
 }
 
 // =====================================================================================================================
@@ -1207,16 +1187,16 @@ extern "C" int tfgnn_b200_rgat_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
   const int LH = L * H, LK = L * K;
   // 1. dZ = dOut * act'(out)
-  float* dz = nullptr;
-  int rc = begin_backward(b, bt, out, grad_out, H, activation, TFGNN_AGG_SUM, st, &dz, [&](float* z) {
-    const float *P = nullptr, *ss = nullptr, *stt = nullptr;
-    const int r = rgat_tables(b, h, D, wt, at, H, K, path, &P, &ss, &stt, st);
-    return r ? r : launch_rgat_target_pass(b, P, ss, stt, K, d, nullptr, nullptr, nullptr, z, st);
+  PoolBuffer dz{st};
+  int rc = begin_backward(b, bt, out, grad_out, H, activation, TFGNN_AGG_SUM, st, dz, [&](float* z) {
+    PoolBuffer P{st}, ss{st}, stt{st};
+    const int r = rgat_tables(b, h, D, wt, at, H, K, path, P, ss, stt, st);
+    return r ? r : launch_rgat_target_pass(b, P.f(), ss.f(), stt.f(), K, d, nullptr, nullptr, nullptr, z, st);
   });
   if (rc) return rc;
   // 2. the forward's tables
-  const float *P = nullptr, *ss = nullptr, *stt = nullptr;
-  rc = rgat_tables(b, h, D, wt, at, H, K, path, &P, &ss, &stt, st);
+  PoolBuffer P{st}, ss{st}, stt{st};
+  rc = rgat_tables(b, h, D, wt, at, H, K, path, P, ss, stt, st);
   if (rc) return rc;
   PoolBuffer stat{st}, ds_tgt{st}, dP{st}, ds_src{st};
   rc = stat.alloc((size_t)V * 3 * K * sizeof(float));
@@ -1225,29 +1205,30 @@ extern "C" int tfgnn_b200_rgat_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   if (!rc) rc = ds_src.alloc((size_t)Vs * LK * sizeof(float));
   if (rc) return rc;
   // 3., 4. target pass, source pass
-  rc = launch_rgat_target_pass(b, P, ss, stt, K, d, dz, stat.f(), ds_tgt.f(), nullptr, st);
+  rc = launch_rgat_target_pass(b, P.f(), ss.f(), stt.f(), K, d, dz.f(), stat.f(), ds_tgt.f(), nullptr, st);
   if (rc) return rc;
-  rc = launch_rgat_source_pass(b, bt, P, ss, stt, at, K, d, dz, stat.f(), ds_tgt.f(), dP.f(), ds_src.f(), st);
+  rc = launch_rgat_source_pass(b, bt, P.f(), ss.f(), stt.f(), at, K, d, dz.f(), stat.f(), ds_tgt.f(), dP.f(), ds_src.f(),
+                               st);
   if (rc) return rc;
   // 5. attention gradients: the source half over all Vs rows, the target half over the owned rows
-  rc = launch_rgat_attention_grad(ds_src.f(), P, Vs, L, K, d, gat, 0, st);
+  rc = launch_rgat_attention_grad(ds_src.f(), P.f(), Vs, L, K, d, gat, 0, st);
   if (rc) return rc;
-  rc = launch_rgat_attention_grad(ds_tgt.f(), P + (size_t)lo * LH, V, L, K, d, gat, 1, st);
+  rc = launch_rgat_attention_grad(ds_tgt.f(), P.f() + (size_t)lo * LH, V, L, K, d, gat, 1, st);
   if (rc) return rc;
   // 6. dW_l = h^T dP_l over all Vs rows
-  void *part = nullptr, *WT = nullptr;
-  rc = batch_scratch(b, 9, tn_partial_floats(Vs, D, H) * sizeof(float), &part);
-  if (rc) return rc;
-  for (int l = 0; l < L; ++l) {
-    rc = weight_grad(h, D, dP.f() + (size_t)l * H, LH, Vs, D, H, (float*)part, one_table(grad_W[l]), 1, D, 0, st);
+  {
+    PoolBuffer part{st};
+    rc = part.alloc(tn_partial_floats(Vs, D, H) * sizeof(float));
+    for (int l = 0; l < L && !rc; ++l)
+      rc = weight_grad(h, D, dP.f() + (size_t)l * H, LH, Vs, D, H, part.f(), one_table(grad_W[l]), 1, D, 0, st);
     if (rc) return rc;
   }
   if (!grad_h) return 0;
   // 7. grad_h = dP [W_0^T; ..] (K = L*H)
-  rc = batch_scratch(b, 3, (size_t)LH * D * sizeof(float), &WT);
-  if (rc) return rc;
-  return gemm_transposed(dP.f(), LH, {wt, L, D, H, 1, 0, /*stacked=*/true}, (float*)WT, grad_h, D, Vs, D, GemmEpilogue{},
-                         b, st);
+  PoolBuffer WT{st};
+  rc = WT.alloc((size_t)LH * D * sizeof(float));
+  return rc ? rc : gemm_transposed(dP.f(), LH, {wt, L, D, H, 1, 0, /*stacked=*/true}, WT.f(), grad_h, D, Vs, D,
+                                   GemmEpilogue{}, st);
 }
 
 // =====================================================================================================================
@@ -1389,7 +1370,7 @@ extern "C" int tfgnn_b200_dense_bwd(const float* x, const float* W, const float*
   PoolBuffer wT{st};
   rc = wT.alloc((size_t)N * K * sizeof(float));
   if (rc) return rc;
-  return gemm_transposed(dz.f(), N, {one_table(W), 1, K, N}, wT.f(), grad_x, K, V, K, GemmEpilogue{}, nullptr, st);
+  return gemm_transposed(dz.f(), N, {one_table(W), 1, K, N}, wT.f(), grad_x, K, V, K, GemmEpilogue{}, st);
 }
 
 extern "C" int tfgnn_b200_layer_norm_bwd(const float* x, const float* gamma, const float* grad_out, int64_t V, int32_t H,

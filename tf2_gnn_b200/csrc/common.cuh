@@ -155,9 +155,6 @@ struct tfgnn_batch {
   // caller-owned adjacency (kept for the TFGNN_PATH_ATOMIC evidence path only)
   const int32_t* adj[TFGNN_MAX_EDGE_TYPES] = {};
   long long E[TFGNN_MAX_EDGE_TYPES] = {};
-  // grow-only scratch owned by the batch (stream-ordered allocations from the library's private pool, mempool.cu)
-  void* scratch[16] = {};
-  size_t scratch_bytes[16] = {};
   // the stream the batch was last used on: allocations / frees of its buffers are ordered on it.  A batch may move
   // between streams from one call to the next (batch_enter orders the new stream after the old one), but it must
   // not be used from two streams or two host threads at the same time.
@@ -182,8 +179,6 @@ struct tfgnn_batch {
 };
 
 namespace tfgnn {
-// Returns a device scratch buffer of at least `bytes` in slot `slot` of the batch (valid on b->cur_stream).
-int batch_scratch(tfgnn_batch* b, int slot, size_t bytes, void** out);
 // Every entry point that takes a batch calls this first: binds the batch to `st` for this call.
 int batch_enter(tfgnn_batch* b, cudaStream_t st);
 // Stream-ordered device memory from the library's PRIVATE cudaMemPool (release threshold = keep everything:
@@ -191,10 +186,16 @@ int batch_enter(tfgnn_batch* b, cudaStream_t st);
 int pool_alloc(void** p, size_t bytes, cudaStream_t st);
 void pool_free(void* p, cudaStream_t st);
 
-// A buffer from the library pool, freed (stream-ordered, after the work queued so far) when it goes out of scope.
+// A buffer from the library pool, freed (stream-ordered, after the work queued so far) when it goes out of scope.  Every
+// temporary of a layer call is one, owned by the narrowest scope that covers its uses: a nested call cannot free or
+// regrow a buffer its caller still holds.  Move-only: it owns its pointer.
 struct PoolBuffer {
   cudaStream_t st;
   void* p = nullptr;
+  explicit PoolBuffer(cudaStream_t s) : st(s) {}
+  PoolBuffer(PoolBuffer&& o) noexcept : st(o.st), p(o.p) { o.p = nullptr; }
+  PoolBuffer(const PoolBuffer&) = delete;
+  PoolBuffer& operator=(const PoolBuffer&) = delete;
   ~PoolBuffer() { pool_free(p, st); }
   int alloc(size_t bytes) { return pool_alloc(&p, bytes, st); }
   float* f() const { return (float*)p; }

@@ -132,12 +132,13 @@ extern "C" int tfgnn_b200_unsorted_segment_reduce(const float* data, const int32
   const bool need_counts = aggregation == TFGNN_AGG_MEAN || aggregation == TFGNN_AGG_SQRT_N;
   fill_kernel<<<grid_for(num_segments * H), 256, 0, st>>>(out, num_segments * H, use_max ? kLowestFloat : 0.f);
   TFGNN_LAUNCH_CHECK();
-  int* counts = nullptr;
+  PoolBuffer count_buf{st};
   if (need_counts) {
-    int rc = pool_alloc((void**)&counts, (size_t)num_segments * sizeof(int), st);
+    int rc = count_buf.alloc((size_t)num_segments * sizeof(int));
     if (rc) return rc;
-    TFGNN_CUDA(cudaMemsetAsync(counts, 0, (size_t)num_segments * sizeof(int), st));
+    TFGNN_CUDA(cudaMemsetAsync(count_buf.p, 0, (size_t)num_segments * sizeof(int), st));
   }
+  int* counts = (int*)count_buf.p;
   if (M > 0) {
     TFGNN_REQUIRE(data && segment_ids, "NULL pointer");
     segment_scatter_kernel<<<grid_for(M * H), 256, 0, st>>>(data, segment_ids, ids_stride, M, H, num_segments,
@@ -148,7 +149,6 @@ extern "C" int tfgnn_b200_unsorted_segment_reduce(const float* data, const int32
     segment_norm_kernel<<<grid_for(num_segments * H), 256, 0, st>>>(out, counts, num_segments, H,
                                                                    aggregation == TFGNN_AGG_MEAN ? 1 : 2);
     TFGNN_LAUNCH_CHECK();
-    pool_free(counts, st);
   }
   return 0;
 }
@@ -295,17 +295,16 @@ extern "C" int tfgnn_b200_segment_max_bwd(const float* data, const int32_t* segm
   if (M == 0) return 0;
   TFGNN_REQUIRE(data && segment_ids && segment_out && segment_grad && grad_data, "NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  void* ties = nullptr;
-  int rc = pool_alloc(&ties, (size_t)num_segments * H * sizeof(float), st);
+  PoolBuffer ties{st};
+  int rc = ties.alloc((size_t)num_segments * H * sizeof(float));
   if (rc) return rc;
-  TFGNN_CUDA(cudaMemsetAsync(ties, 0, (size_t)num_segments * H * sizeof(float), st));
+  TFGNN_CUDA(cudaMemsetAsync(ties.p, 0, (size_t)num_segments * H * sizeof(float), st));
   segment_max_ties_kernel<<<grid_for(M * H), 256, 0, st>>>(data, segment_ids, ids_stride, segment_out, M, H, num_segments,
-                                                          (float*)ties);
+                                                          ties.f());
   TFGNN_LAUNCH_CHECK();
   segment_max_bwd_kernel<<<grid_for(M * H), 256, 0, st>>>(data, segment_ids, ids_stride, segment_out, segment_grad,
-                                                         (const float*)ties, M, H, num_segments, grad_data);
+                                                         ties.f(), M, H, num_segments, grad_data);
   TFGNN_LAUNCH_CHECK();
-  pool_free(ties, st);
   return 0;
 }
 

@@ -113,9 +113,10 @@ extern "C" int tfgnn_b200_graph_offsets(const int32_t* node_to_graph_map, int64_
   TFGNN_REQUIRE(graph_ptr != nullptr, "graph_ptr is NULL");
   TFGNN_REQUIRE(num_nodes == 0 || node_to_graph_map != nullptr, "node_to_graph_map is NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  int* bad = nullptr;
-  int rc = pool_alloc((void**)&bad, sizeof(int), st);
+  PoolBuffer bad_buf{st};
+  int rc = bad_buf.alloc(sizeof(int));
   if (rc) return rc;
+  int* bad = (int*)bad_buf.p;
   TFGNN_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
   graph_offsets_kernel<<<grid_for(num_nodes + 1), 256, 0, st>>>(node_to_graph_map, num_nodes, num_graphs, graph_ptr, bad);
   TFGNN_LAUNCH_CHECK();
@@ -124,7 +125,6 @@ extern "C" int tfgnn_b200_graph_offsets(const int32_t* node_to_graph_map, int64_
     TFGNN_CUDA(cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
     TFGNN_CUDA(cudaStreamSynchronize(st));
   }
-  pool_free(bad, st);
   if (host_bad) {
     set_error(TFGNN_ERR_INVALID_ARGUMENT,
               "node_to_graph_map must be non-decreasing with values in [0, num_graphs) (graph_dataset.py:211-217)");
@@ -187,22 +187,8 @@ extern "C" int tfgnn_b200_dense_bias_fwd(const float* x, const float* W, const f
   TFGNN_REQUIRE(valid_act(activation), "unknown activation code");
   if (V == 0) return 0;
   TFGNN_REQUIRE(x && W && out, "NULL pointer");
-  cudaStream_t st = (cudaStream_t)stream;
   GemmEpilogue epi;
   epi.act = activation;
   epi.bias = bias;
-  const bool want_tc = path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC;
-  const bool bias_ok = bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15) == 0;   // float4 bias loads
-  if (want_tc && bias_ok && gemm_tc_supported(V, N, K, x, K, out, N)) {
-    void* packed = nullptr;
-    int rc = pool_alloc(&packed, gemm_tc_packed_bytes(N, K), st);
-    if (rc) return rc;
-    rc = launch_pack_weights_tc(W, N, K, N, (float*)packed, st);
-    if (!rc) rc = launch_gemm_tc(x, K, (const float*)packed, out, N, V, N, K, epi, st);
-    pool_free(packed, st);
-    return rc;
-  }
-  if (path == TFGNN_PATH_SORTED_TC)
-    return unsupported("dense_bias_fwd: shape not supported by the tensor-core GEMM (need N%16==0, K%32==0)");
-  return launch_gemm_simt(x, K, W, N, out, N, V, N, K, epi, st);
+  return node_gemm(x, K, W, N, out, N, V, N, K, epi, path, (cudaStream_t)stream);
 }

@@ -8,13 +8,12 @@ int unsupported(const std::string& msg);
 bool valid_act(int a);
 bool valid_agg(int a);
 int agg_row_norm(int aggregation);
-// the batch scratch slot that holds a GEMM's tensor-core-packed weights for the duration of that GEMM
-constexpr int kPackSlot = 6;
 int node_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int N, int K,
-              const GemmEpilogue& epi, int path, tfgnn_batch* batch, cudaStream_t st);
-// P (slot 2), T (slot 4) and the merged edge reduce of the transform-then-aggregate form (api.cu)
+              const GemmEpilogue& epi, int path, cudaStream_t st);
+// P, T (into the caller's buffers) and the merged edge reduce of the transform-then-aggregate form (api.cu)
 int transform_aggregate_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& W, int H, uint32_t flags,
-                               int aggregation, int activation, int path, EdgeReduceParams* p, cudaStream_t st);
+                               int aggregation, int activation, int path, PoolBuffer& P, PoolBuffer& T,
+                               EdgeReduceParams* p, cudaStream_t st);
 int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                   uint32_t flags, int aggregation, int activation, int path, float* out, int ldo, cudaStream_t st);
 // literal per-edge path (literal.cu); FB = optional FiLM table [V, L*2H] (gamma | beta per type)
@@ -24,9 +23,9 @@ int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* 
 // RGAT edge-level aggregation (rgat.cu): warp per target + chunked hub path; needs (H/K) % 4 == 0
 int launch_rgat_aggregate(tfgnn_batch* b, const float* P, const float* s_src, const float* s_tgt, int K, int d,
                           int activation, float* out, cudaStream_t st);
-// RGAT projection P (slot 2) and score halves s_src, s_tgt (slots 13, 14) of the forward (variants.cu); L > 0
+// RGAT projection P and score halves s_src, s_tgt of the forward, into the caller's buffers (variants.cu); L > 0
 int rgat_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& wt, const PtrTable& at, int H, int K, int path,
-                const float** P, const float** s_src, const float** s_tgt, cudaStream_t st);
+                PoolBuffer& P, PoolBuffer& s_src, PoolBuffer& s_tgt, cudaStream_t st);
 // Edge-level steps of the RGAT backward (rgat.cu), no float atomics; d % 4 == 0, H <= 512.
 //   target pass, dz given: stat [V, 3K] = (m, den, g) per head, ds_tgt [V, L*K];  dz NULL: the pre-activation pre [V, H]
 //   source pass over bt's source-keyed CSR: dP [Vs, L*H], ds_src [Vs, L*K]

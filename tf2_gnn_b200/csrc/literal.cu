@@ -121,37 +121,36 @@ int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* 
   long long maxE = 1;
   for (int l = 0; l < L; ++l) maxE = b->E[l] > maxE ? b->E[l] : maxE;
   const int wide = D_in > H ? D_in : H;
-  void *X0 = nullptr, *X1 = nullptr, *tgt_of = nullptr;
   int rc = batch_enter(b, st);
   if (rc) return rc;
-  rc = batch_scratch(b, 2, (size_t)maxE * wide * sizeof(float), &X0);
+  PoolBuffer X0{st}, X1{st}, tgt_buf{st};
+  rc = X0.alloc((size_t)maxE * wide * sizeof(float));
+  if (!rc) rc = X1.alloc((size_t)maxE * wide * sizeof(float));
+  if (!rc) rc = tgt_buf.alloc((size_t)maxE * sizeof(int));
   if (rc) return rc;
-  rc = batch_scratch(b, 5, (size_t)maxE * wide * sizeof(float), &X1);
-  if (rc) return rc;
-  rc = batch_scratch(b, 4, (size_t)maxE * sizeof(int), &tgt_of);
-  if (rc) return rc;
+  const int* tgt_of = (const int*)tgt_buf.p;
   fill2d_kernel<<<grid_for(V * H), 256, 0, st>>>(out, V, H, ldo, use_max ? kLowestFloat : 0.f);
   TFGNN_LAUNCH_CHECK();
   for (int l = 0; l < L; ++l) {
     const long long E = b->E[l];
     if (E == 0) continue;
-    expand_targets_kernel<<<grid_for(V), 256, 0, st>>>(b->row_ptr, V, l, (int*)tgt_of);
+    expand_targets_kernel<<<grid_for(V), 256, 0, st>>>(b->row_ptr, V, l, (int*)tgt_buf.p);
     TFGNN_LAUNCH_CHECK();
-    gather_concat_kernel<<<grid_for(E * 32), 256, 0, st>>>(h, h_tgt, D, b->row_ptr, b->src_sorted, V, l,
-                                                         (const int*)tgt_of, use_target, (float*)X0, D_in);
+    gather_concat_kernel<<<grid_for(E * 32), 256, 0, st>>>(h, h_tgt, D, b->row_ptr, b->src_sorted, V, l, tgt_of,
+                                                         use_target, X0.f(), D_in);
     TFGNN_LAUNCH_CHECK();
-    float* cur = (float*)X0;
-    float* nxt = (float*)X1;
+    float* cur = X0.f();
+    float* nxt = X1.f();
     int k_in = D_in;
     for (int i = 0; i < n_layers; ++i) {
       GemmEpilogue epi;
       epi.act = i < n_hidden ? TFGNN_ACT_RELU : TFGNN_ACT_NONE;   // dpu_utils MLP: ReLU hidden, linear output
-      rc = node_gemm(cur, k_in, mlp_weights[l * n_layers + i], H, nxt, H, E, H, k_in, epi, path, b, st);
+      rc = node_gemm(cur, k_in, mlp_weights[l * n_layers + i], H, nxt, H, E, H, k_in, epi, path, st);
       if (rc) return rc;
       float* t = cur; cur = nxt; nxt = t;
       k_in = H;
     }
-    edge_post_kernel<<<grid_for(E * H), 256, 0, st>>>(cur, H, b->row_ptr, V, l, (const int*)tgt_of, normalize, FB, ldf,
+    edge_post_kernel<<<grid_for(E * H), 256, 0, st>>>(cur, H, b->row_ptr, V, l, tgt_of, normalize, FB, ldf,
                                                      act_before ? activation : TFGNN_ACT_NONE);
     TFGNN_LAUNCH_CHECK();
     segment_reduce_sorted_kernel<<<grid_for(V * H), 256, 0, st>>>(cur, H, b->row_ptr, V, l, use_max, out, ldo);

@@ -1,4 +1,4 @@
-// Stream-ordered device memory for everything the library owns (CSR, scratch, operand packing): a PRIVATE
+// Stream-ordered device memory for everything the library owns (CSR, per-call temporaries, operand packing): a PRIVATE
 // cudaMemPool per device with its release threshold at the maximum, so freed blocks stay cached in the pool.
 // After warm-up the per-batch path (tfgnn_b200_prepare -> layer calls -> tfgnn_b200_free_batch) performs no
 // cudaMalloc / cudaFree and never synchronises the device: round 1 paid 26 ms per PPI-sized batch for those
@@ -74,19 +74,6 @@ int batch_enter(tfgnn_batch* b, cudaStream_t st) {
   }
   b->cur_stream = st;
   b->used = true;
-  return 0;
-}
-
-int batch_scratch(tfgnn_batch* b, int slot, size_t bytes, void** out) {
-  if (b->scratch_bytes[slot] < bytes) {
-    if (b->scratch[slot]) pool_free(b->scratch[slot], b->cur_stream);
-    b->scratch[slot] = nullptr;
-    b->scratch_bytes[slot] = 0;
-    int rc = pool_alloc(&b->scratch[slot], bytes, b->cur_stream);
-    if (rc) return rc;
-    b->scratch_bytes[slot] = bytes;
-  }
-  *out = b->scratch[slot];
   return 0;
 }
 

@@ -333,41 +333,44 @@ static int prepare_impl(const int32_t* const* adj, const int64_t* num_edges, int
     g_launch_count.fetch_add(1);
     TRY_CUDA(cudaGetLastError());
   }
-  {
-    // scan + cursor scratch
-    const int nb = ceil_div(S + 1, kScanTile);
-    void* bs = nullptr;
-    TRY(batch_scratch(b, 0, (size_t)nb * sizeof(int), &bs));
-    TRY(exclusive_scan_inplace(b->row_ptr, S + 1, (int*)bs, st));
-  }
-  if (M > 0 && V > 0) {
-    void* cursor = nullptr;
-    TRY(batch_scratch(b, 1, (size_t)(S + 1) * sizeof(int), &cursor));
-    TRY_CUDA(cudaMemcpyAsync(cursor, b->row_ptr, (size_t)S * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  // scan of the counts, then the sources in segment order.  The block sums, the fill cursor and the hub list belong to this
+  // call alone: they are freed on `st` when the lambda returns, before fail() can free the batch.
+  auto scan_and_fill = [&]() -> int {
+    PoolBuffer bs{st};
+    int r = bs.alloc((size_t)ceil_div(S + 1, kScanTile) * sizeof(int));
+    if (!r) r = exclusive_scan_inplace(b->row_ptr, S + 1, (int*)bs.p, st);
+    if (r || M == 0 || V == 0) return r;
+    PoolBuffer cursor{st};
+    r = cursor.alloc((size_t)(S + 1) * sizeof(int));
+    if (r) return r;
+    TFGNN_CUDA(cudaMemcpyAsync(cursor.p, b->row_ptr, (size_t)S * sizeof(int), cudaMemcpyDeviceToDevice, st));
     int bx = ceil_div(maxE, 256);
     if (bx > 132 * 16) bx = 132 * 16;
     dim3 grid(bx, L);
     fill_sources_kernel<<<grid, 256, 0, st>>>(pt, ct, (int)V, (int)V_total, (int)tgt_begin, (int)V_own, kind,
-                                              (int*)cursor, b->src_sorted);
+                                              (int*)cursor.p, b->src_sorted);
     g_launch_count.fetch_add(1);
-    TRY_CUDA(cudaGetLastError());
+    TFGNN_CUDA(cudaGetLastError());
     long long warps_needed = S;
     int blocks = ceil_div(warps_needed * 32, 256);
     if (blocks > 132 * 32) blocks = 132 * 32;
     // a segment longer than 256 edges is a "hub"; there are at most M/257 of them
     const long long max_long = M / 257 + 1;
-    void* long_buf = nullptr;
-    TRY(batch_scratch(b, 7, (size_t)max_long * sizeof(long long) + 16, &long_buf));
-    int* long_count = reinterpret_cast<int*>(long_buf);
-    long long* long_list = reinterpret_cast<long long*>(reinterpret_cast<char*>(long_buf) + 16);
-    TRY_CUDA(cudaMemsetAsync(long_count, 0, sizeof(int), st));
+    PoolBuffer long_buf{st};
+    r = long_buf.alloc((size_t)max_long * sizeof(long long) + 16);
+    if (r) return r;
+    int* long_count = reinterpret_cast<int*>(long_buf.p);
+    long long* long_list = reinterpret_cast<long long*>(reinterpret_cast<char*>(long_buf.p) + 16);
+    TFGNN_CUDA(cudaMemsetAsync(long_count, 0, sizeof(int), st));
     sort_segments_kernel<<<blocks, 256, 0, st>>>(b->row_ptr, S, b->src_sorted, long_list, long_count);
     g_launch_count.fetch_add(1);
-    TRY_CUDA(cudaGetLastError());
+    TFGNN_CUDA(cudaGetLastError());
     sort_long_segments_kernel<<<132 * 2, 512, 0, st>>>(b->row_ptr, long_list, long_count, b->src_sorted);
     g_launch_count.fetch_add(1);
-    TRY_CUDA(cudaGetLastError());
-  }
+    TFGNN_CUDA(cudaGetLastError());
+    return 0;
+  };
+  TRY(scan_and_fill());
   if (prepare_flags & TFGNN_PREPARE_VALIDATE) {
     int bad = 0;
     TRY_CUDA(cudaMemcpyAsync(&bad, b->invalid_count, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -402,7 +405,6 @@ extern "C" int tfgnn_b200_free_batch(tfgnn_batch_t* b) {
   pool_free(b->row_ptr, b->cur_stream);
   pool_free(b->src_sorted, b->cur_stream);
   pool_free(b->invalid_count, b->cur_stream);
-  for (int i = 0; i < 16; ++i) pool_free(b->scratch[i], b->cur_stream);
   if (b->ev_switch) cudaEventDestroy(b->ev_switch);
   if (b->pipe_ready) {
     cudaStreamDestroy(b->pipe_gather);

@@ -210,16 +210,14 @@ int launch_rgat_aggregate(tfgnn_batch* b, const float* P, const float* s_src, co
   p.P = P; p.s_src = s_src; p.s_tgt = s_tgt; p.row_ptr = b->row_ptr; p.src = b->src_sorted;
   p.V = b->V; p.tgt_off = b->tgt_off; p.L = b->L; p.K = K; p.d = d; p.H = K * d; p.act = activation; p.out = out;
   const long long max_items = b->M_in / kHubChunk + b->M_in / kHubThreshold + 2;
-  void *hm = nullptr, *hd = nullptr, *items = nullptr;
-  int rc = batch_scratch(b, 8, (size_t)p.V * K * sizeof(float), &hm);
+  PoolBuffer hm{st}, hd{st}, items{st};
+  int rc = hm.alloc((size_t)p.V * K * sizeof(float));
+  if (!rc) rc = hd.alloc((size_t)p.V * K * sizeof(float));
+  if (!rc) rc = items.alloc((size_t)max_items * sizeof(int2) + 16);
   if (rc) return rc;
-  rc = batch_scratch(b, 9, (size_t)p.V * K * sizeof(float), &hd);
-  if (rc) return rc;
-  rc = batch_scratch(b, 10, (size_t)max_items * sizeof(int2) + 16, &items);
-  if (rc) return rc;
-  p.hub_max = (float*)hm; p.hub_den = (float*)hd;
-  p.item_count = (int*)items;
-  p.items = reinterpret_cast<int2*>(reinterpret_cast<char*>(items) + 16);
+  p.hub_max = hm.f(); p.hub_den = hd.f();
+  p.item_count = (int*)items.p;
+  p.items = reinterpret_cast<int2*>(reinterpret_cast<char*>(items.p) + 16);
   TFGNN_CUDA(cudaMemsetAsync(p.item_count, 0, sizeof(int), st));
   const int col_blocks = (p.H / 4 + 31) / 32;
   int scan_blocks = ceil_div(p.V, 256);

@@ -38,14 +38,14 @@ extern "C" int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   if (V == 0) return 0;
   TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  void *agg = nullptr, *gx = nullptr, *gh = nullptr;
   int rc = batch_enter(b, st);
   if (rc) return rc;
-  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &agg);
+  PoolBuffer agg{st};
+  rc = agg.alloc((size_t)V * H * sizeof(float));
   if (rc) return rc;
   // ggnn.py:68-89: aggregation of the messages, no activation (act_before is ignored too).
   rc = edge_mlp_core(b, h, D, mlp_weights, num_hidden_layers, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION,
-                     aggregation, TFGNN_ACT_NONE, path, (float*)agg, H, st);
+                     aggregation, TFGNN_ACT_NONE, path, agg.f(), H, st);
   if (rc) return rc;
   {
     // The GRU update as ONE tensor-core contraction over [agg | h] with the gate math in its epilogue: no [V,3H] tables.
@@ -57,27 +57,27 @@ extern "C" int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     // the contraction reads whole rows of h for every 32-unit column tile while earlier tiles' epilogues already store new
     // states: an in-place update (out overlapping h; the gate kernel below tolerates it) must not take this form
     const bool in_place = out < h + (size_t)b->V_src * D && h < out + (size_t)V * H;
-    if (want && !in_place && gemm_tc_gru_supported(V, H, (const float*)agg, H, h_tgt0, D, out, H)) {
-      void* packed = nullptr;
-      rc = batch_scratch(b, kPackSlot, gemm_tc_gru_packed_bytes(H), &packed);
+    if (want && !in_place && gemm_tc_gru_supported(V, H, agg.f(), H, h_tgt0, D, out, H)) {
+      PoolBuffer packed{st};
+      rc = packed.alloc(gemm_tc_gru_packed_bytes(H));
       if (rc) return rc;
-      return launch_gemm_tc_gru((const float*)agg, H, h_tgt0, D, gru_kernel, gru_recurrent_kernel, gru_bias, (float*)packed,
-                                out, H, V, H, st);
+      return launch_gemm_tc_gru(agg.f(), H, h_tgt0, D, gru_kernel, gru_recurrent_kernel, gru_bias, packed.f(), out, H, V,
+                                H, st);
     }
   }
-  rc = batch_scratch(b, 9, (size_t)V * 3 * H * sizeof(float), &gx);
-  if (rc) return rc;
-  rc = batch_scratch(b, 10, (size_t)V * 3 * H * sizeof(float), &gh);
+  PoolBuffer gx{st}, gh{st};
+  rc = gx.alloc((size_t)V * 3 * H * sizeof(float));
+  if (!rc) rc = gh.alloc((size_t)V * 3 * H * sizeof(float));
   if (rc) return rc;
   GemmEpilogue ex, eh;
   ex.bias = gru_bias;
   eh.bias = gru_bias + 3 * H;
-  rc = node_gemm((const float*)agg, H, gru_kernel, 3 * H, (float*)gx, 3 * H, V, 3 * H, H, ex, path, b, st);
+  rc = node_gemm(agg.f(), H, gru_kernel, 3 * H, gx.f(), 3 * H, V, 3 * H, H, ex, path, st);
   if (rc) return rc;
   const float* h_tgt = h + (size_t)b->tgt_off * D;
-  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, 3 * H, (float*)gh, 3 * H, V, 3 * H, H, eh, path, b, st);
+  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, 3 * H, gh.f(), 3 * H, V, 3 * H, H, eh, path, st);
   if (rc) return rc;
-  gru_gate_kernel<<<grid_for(V * H), 256, 0, st>>>((const float*)gx, nullptr, (const float*)gh, h_tgt, D, V, H, out);
+  gru_gate_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), nullptr, gh.f(), h_tgt, D, V, H, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
@@ -108,25 +108,23 @@ extern "C" int tfgnn_b200_rgin_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
                          st);
   TFGNN_REQUIRE(aggr_weights != nullptr, "aggr_weights is NULL");
   if (V == 0) return 0;
-  void *t0 = nullptr, *t1 = nullptr;
   int rc = batch_enter(b, st);
   if (rc) return rc;
-  rc = batch_scratch(b, 8, (size_t)V * H * sizeof(float), &t0);
+  PoolBuffer t0{st}, t1{st};
+  rc = t0.alloc((size_t)V * H * sizeof(float));
+  if (!rc) rc = t1.alloc((size_t)V * H * sizeof(float));
+  if (!rc) rc = edge_mlp_core(b, h, D, mlp_weights, num_hidden_layers, H, flags, aggregation, TFGNN_ACT_NONE, path, t0.f(),
+                              H, st);
   if (rc) return rc;
-  rc = batch_scratch(b, 9, (size_t)V * H * sizeof(float), &t1);
-  if (rc) return rc;
-  rc = edge_mlp_core(b, h, D, mlp_weights, num_hidden_layers, H, flags, aggregation, TFGNN_ACT_NONE, path,
-                     (float*)t0, H, st);
-  if (rc) return rc;
-  float* cur = (float*)t0;
-  float* nxt = (float*)t1;
+  float* cur = t0.f();
+  float* nxt = t1.f();
   for (int i = 0; i < num_aggr_layers; ++i) {
     TFGNN_REQUIRE(aggr_weights[i] != nullptr, "an aggregation MLP weight pointer is NULL");
     const bool last = i == num_aggr_layers - 1;
     GemmEpilogue epi;
     epi.act = last ? activation : TFGNN_ACT_RELU;
     float* dst = last ? out : nxt;
-    rc = node_gemm(cur, H, aggr_weights[i], H, dst, H, V, H, H, epi, path, b, st);
+    rc = node_gemm(cur, H, aggr_weights[i], H, dst, H, V, H, H, epi, path, st);
     if (rc) return rc;
     float* t = cur; cur = nxt; nxt = t;
     if (!last) cur = dst;
@@ -162,7 +160,6 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   }
   const int Vs = (int)b->V_src;
   const float* h_tgt = h + (size_t)b->tgt_off * D;
-  void *P = nullptr, *Tt = nullptr, *Wcat = nullptr, *FB = nullptr, *Fcat = nullptr;
   GemmEpilogue none;
   int rc = batch_enter(b, st);
   if (rc) return rc;
@@ -185,53 +182,54 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     // the OWNED rows are ever multiplied (the transform-then-aggregate form projects all num_nodes_total sources on
     // every rank: 123 GB per rank at BASELINE config 5).
     const int K = L * D;
-    void *A = nullptr, *T = nullptr, *Fb = nullptr;
-    rc = batch_scratch(b, 2, (size_t)V * K * sizeof(float), &A);
-    if (rc) return rc;
-    rc = batch_scratch(b, 4, (size_t)V * K * sizeof(float), &T);
-    if (rc) return rc;
-    rc = batch_scratch(b, 3, (size_t)K * H * sizeof(float), &Fb);
+    PoolBuffer A{st}, T{st};
+    rc = A.alloc((size_t)V * K * sizeof(float));
+    if (!rc) rc = T.alloc((size_t)V * K * sizeof(float));
     if (rc) return rc;
     {
       EdgeReduceParams p;
       p.X = h; p.ldx = D; p.x_type_stride = 0;
       p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-      p.out = (float*)A; p.ldo = K; p.out_type_stride = D;
+      p.out = A.f(); p.ldo = K; p.out_type_stride = D;
       p.V = V; p.L = L; p.C = D; p.normalize = normalize;
       rc = launch_edge_reduce(p, /*merged=*/false, st);
       if (rc) return rc;
     }
     // beta part: out = [c_0 h_v | .. | c_{L-1} h_v] [Fbeta_0; ..; Fbeta_{L-1}]   (one K = L*D contraction, not finalised)
-    rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, /*normalize=*/0, (float*)T, K, 0, st);
+    rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, /*normalize=*/0, T.f(), K, 0, st);
     if (rc) return rc;
-    PtrTable fbeta{};
-    for (int l = 0; l < L; ++l) fbeta.p[l] = reinterpret_cast<const float*>(film.p[l]) + H;
-    rc = launch_pack_vertical(fbeta, L, 0, D, H, 2 * H, (float*)Fb, H, 0, st);
-    if (rc) return rc;
-    GemmEpilogue raw;
-    raw.finalize = 0;
-    rc = node_gemm((const float*)T, K, (const float*)Fb, H, out, H, V, H, K, raw, path, b, st);
-    if (rc) return rc;
+    {
+      PoolBuffer Fb{st};
+      PtrTable fbeta{};
+      for (int l = 0; l < L; ++l) fbeta.p[l] = reinterpret_cast<const float*>(film.p[l]) + H;
+      rc = Fb.alloc((size_t)K * H * sizeof(float));
+      if (!rc) rc = launch_pack_vertical(fbeta, L, 0, D, H, 2 * H, Fb.f(), H, 0, st);
+      if (rc) return rc;
+      GemmEpilogue raw;
+      raw.finalize = 0;
+      rc = node_gemm(T.f(), K, Fb.f(), H, out, H, V, H, K, raw, path, st);
+      if (rc) return rc;
+    }
     if (use_target && normalize) {   // coeff(v,l) h_v with the normalised coefficient (the beta operand used the raw count)
-      rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, 1, (float*)T, K, 0, st);
+      rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, 1, T.f(), K, 0, st);
       if (rc) return rc;
     }
     // gamma for all types in ONE wide contraction: Gall [V, L*H] = h_v [Fgamma_0 | .. | Fgamma_{L-1}] (128-column tiles:
     // the k-block rate of the GEMM pipeline is latency-bound, so work per k-block ~ tile width; 6 GEMMs of N = 320 ran in
     // 80-column tiles at 4.7 ms each, the wide one takes about half of their sum)
     const int LHw = L * H;
-    void *Gall = nullptr, *Fg = nullptr;
-    rc = batch_scratch(b, 11, (size_t)V * LHw * sizeof(float), &Gall);
-    if (rc) return rc;
-    rc = batch_scratch(b, 12, (size_t)D * LHw * sizeof(float), &Fg);
-    if (rc) return rc;
-    rc = launch_pack_horizontal(film, L, 0, D, H, 2 * H, (float*)Fg, LHw, st);   // first H columns of every F_l [D, 2H]
-    if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Fg, LHw, (float*)Gall, LHw, V, LHw, D, none, path, b, st);
-    if (rc) return rc;
+    PoolBuffer Gall{st};
+    {
+      PoolBuffer Fg{st};
+      rc = Gall.alloc((size_t)V * LHw * sizeof(float));
+      if (!rc) rc = Fg.alloc((size_t)D * LHw * sizeof(float));
+      if (!rc) rc = launch_pack_horizontal(film, L, 0, D, H, 2 * H, Fg.f(), LHw, st);   // first H columns of every F_l [D, 2H]
+      if (!rc) rc = node_gemm(h_tgt, D, Fg.f(), LHw, Gall.f(), LHw, V, LHw, D, none, path, st);
+      if (rc) return rc;
+    }
     for (int l = 0; l < L; ++l) {
       GemmEpilogue chain;
-      chain.mul = (const float*)Gall + (size_t)l * H; chain.ldm = LHw;
+      chain.mul = Gall.f() + (size_t)l * H; chain.ldm = LHw;
       chain.accumulate = 1;
       chain.finalize = 0;
       const bool last_src = !use_target && l == L - 1;
@@ -240,8 +238,8 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
         chain.act = activation;
         chain.row_norm = agg_row_norm(aggregation); chain.row_ptr = b->row_ptr; chain.V = V; chain.L = L;
       }
-      rc = node_gemm((const float*)A + (size_t)l * D, K, reinterpret_cast<const float*>(first.p[l]), H, out, H, V, H, D,
-                     chain, path, b, st);
+      rc = node_gemm(A.f() + (size_t)l * D, K, reinterpret_cast<const float*>(first.p[l]), H, out, H, V, H, D, chain,
+                     path, st);
       if (rc) return rc;
       if (use_target) {
         if (l == L - 1) {
@@ -249,52 +247,50 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
           chain.act = activation;
           chain.row_norm = agg_row_norm(aggregation); chain.row_ptr = b->row_ptr; chain.V = V; chain.L = L;
         }
-        rc = node_gemm((const float*)T + (size_t)l * D, K, reinterpret_cast<const float*>(first.p[l]) + (size_t)D * H, H,
-                       out, H, V, H, D, chain, path, b, st);
+        rc = node_gemm(T.f() + (size_t)l * D, K, reinterpret_cast<const float*>(first.p[l]) + (size_t)D * H, H, out, H, V,
+                       H, D, chain, path, st);
         if (rc) return rc;
       }
     }
     return 0;
   }
-  rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &P);
-  if (rc) return rc;
-  rc = batch_scratch(b, 3, (size_t)D * LH * sizeof(float), &Wcat);
-  if (rc) return rc;
-  rc = batch_scratch(b, 11, (size_t)V * 2 * LH * sizeof(float), &FB);
-  if (rc) return rc;
-  rc = batch_scratch(b, 12, (size_t)D * 2 * LH * sizeof(float), &Fcat);
-  if (rc) return rc;
+  // FiLM parameters [gamma_l | beta_l] = h F_l depend on (target, type) only (gnn_film.py:99-103)
+  PoolBuffer FB{st};
+  auto film_parameters = [&]() {
+    PoolBuffer Fcat{st};
+    int r = FB.alloc((size_t)V * 2 * LH * sizeof(float));
+    if (!r) r = Fcat.alloc((size_t)D * 2 * LH * sizeof(float));
+    if (!r) r = launch_pack_horizontal(film, L, 0, D, 2 * H, 2 * H, Fcat.f(), 2 * LH, st);
+    return r ? r : node_gemm(h_tgt, D, Fcat.f(), 2 * LH, FB.f(), 2 * LH, V, 2 * LH, D, none, path, st);
+  };
   if (num_hidden_layers > 0) {
     // hidden layers in the edge MLP: FiLM parameters at node level, messages on the literal per-edge path
-    rc = launch_pack_horizontal(film, L, 0, D, 2 * H, 2 * H, (float*)Fcat, 2 * LH, st);
-    if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Fcat, 2 * LH, (float*)FB, 2 * LH, V, 2 * LH, D, none, path, b, st);
-    if (rc) return rc;
-    return edge_mlp_literal(b, h, D, mlp_weights, num_hidden_layers, H, flags, aggregation, activation,
-                            (const float*)FB, 2 * LH, path, out, H, st);
+    rc = film_parameters();
+    return rc ? rc : edge_mlp_literal(b, h, D, mlp_weights, num_hidden_layers, H, flags, aggregation, activation, FB.f(),
+                                      2 * LH, path, out, H, st);
   }
   // projected source messages P_l = h W^s_l  (gnn_edge_mlp.py:100 hoisted to node level)
-  rc = launch_pack_horizontal(first, L, 0, D, H, H, (float*)Wcat, LH, st);
-  if (rc) return rc;
-  rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
-  if (rc) return rc;
-  if (use_target) {
-    rc = batch_scratch(b, 4, (size_t)V * LH * sizeof(float), &Tt);
+  PoolBuffer P{st}, Tt{st};
+  {
+    PoolBuffer Wcat{st};
+    rc = P.alloc((size_t)Vs * LH * sizeof(float));
+    if (!rc) rc = Wcat.alloc((size_t)D * LH * sizeof(float));
+    if (!rc) rc = launch_pack_horizontal(first, L, 0, D, H, H, Wcat.f(), LH, st);
+    if (!rc) rc = node_gemm(h, D, Wcat.f(), LH, P.f(), LH, Vs, LH, D, none, path, st);
     if (rc) return rc;
-    rc = launch_pack_horizontal(first, L, D, D, H, H, (float*)Wcat, LH, st);
-    if (rc) return rc;
-    rc = node_gemm(h_tgt, D, (const float*)Wcat, LH, (float*)Tt, LH, V, LH, D, none, path, b, st);
-    if (rc) return rc;
+    if (use_target) {
+      rc = Tt.alloc((size_t)V * LH * sizeof(float));
+      if (!rc) rc = launch_pack_horizontal(first, L, D, D, H, H, Wcat.f(), LH, st);
+      if (!rc) rc = node_gemm(h_tgt, D, Wcat.f(), LH, Tt.f(), LH, V, LH, D, none, path, st);
+      if (rc) return rc;
+    }
   }
-  // FiLM parameters [gamma_l | beta_l] = h F_l depend on (target, type) only (gnn_film.py:99-103)
-  rc = launch_pack_horizontal(film, L, 0, D, 2 * H, 2 * H, (float*)Fcat, 2 * LH, st);
-  if (rc) return rc;
-  rc = node_gemm(h_tgt, D, (const float*)Fcat, 2 * LH, (float*)FB, 2 * LH, V, 2 * LH, D, none, path, b, st);
+  rc = film_parameters();
   if (rc) return rc;
   EdgeReduceParams p;
-  p.X = (const float*)P; p.ldx = LH; p.x_type_stride = H;
-  p.T = (const float*)Tt; p.ldt = LH; p.t_type_stride = H;
-  p.G = (const float*)FB; p.ldg = 2 * LH; p.g_type_stride = 2 * H; p.beta_off = H;
+  p.X = P.f(); p.ldx = LH; p.x_type_stride = H;
+  p.T = Tt.f(); p.ldt = LH; p.t_type_stride = H;
+  p.G = FB.f(); p.ldg = 2 * LH; p.g_type_stride = 2 * H; p.beta_off = H;
   p.row_ptr = b->row_ptr; p.src = b->src_sorted;
   p.out = out; p.ldo = H; p.V = V; p.L = L; p.C = H;
   p.normalize = normalize;
@@ -398,45 +394,38 @@ __global__ void rgat_aggregate_kernel(const float* __restrict__ P, const float* 
   }
 }
 
-// P_l = h W_l for every one of the Vs nodes (slot 2) and the score halves s_src, s_tgt [Vs, L*K] (slots 13, 14).  The forward
-// and the backward (which recomputes them) both call this, so the backward sees the forward's bits.  Needs L > 0.
+// P_l = h W_l for every one of the Vs nodes and the score halves s_src, s_tgt [Vs, L*K], into the caller's buffers.  The
+// forward and the backward (which recomputes them) both call this, so the backward sees the forward's bits.  Needs L > 0.
 int rgat_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& wt, const PtrTable& at, int H, int K, int path,
-                const float** P_out, const float** s_src_out, const float** s_tgt_out, cudaStream_t st) {
+                PoolBuffer& P, PoolBuffer& ss, PoolBuffer& stt, cudaStream_t st) {
   const long long Vs = b->V_src;
   const int L = b->L, d = H / K, LH = L * H;
-  void *P = nullptr, *Wcat = nullptr, *ss = nullptr, *stt = nullptr;
-  int rc = batch_scratch(b, 2, (size_t)Vs * LH * sizeof(float), &P);
-  if (rc) return rc;
-  rc = batch_scratch(b, 3, (size_t)D * LH * sizeof(float), &Wcat);
-  if (rc) return rc;
-  rc = batch_scratch(b, 13, (size_t)Vs * L * K * sizeof(float), &ss);
-  if (rc) return rc;
-  rc = batch_scratch(b, 14, (size_t)Vs * L * K * sizeof(float), &stt);
-  if (rc) return rc;
+  PoolBuffer Wcat{st};
+  int rc = P.alloc((size_t)Vs * LH * sizeof(float));
+  if (!rc) rc = Wcat.alloc((size_t)D * LH * sizeof(float));
+  if (!rc) rc = ss.alloc((size_t)Vs * L * K * sizeof(float));
+  if (!rc) rc = stt.alloc((size_t)Vs * L * K * sizeof(float));
   // P_l = h W_l for every node once (rgat.py:102-109 applies the same Dense to source and target rows)
-  rc = launch_pack_horizontal(wt, L, 0, D, H, H, (float*)Wcat, LH, st);
+  if (!rc) rc = launch_pack_horizontal(wt, L, 0, D, H, H, Wcat.f(), LH, st);
   if (rc) return rc;
   GemmEpilogue none;
   // Attention score halves in the projection's epilogue when the tensor-core GEMM takes the shape and its column tiles hold
   // whole heads (TFGNN_B200_RGAT_FUSED_SCORES=0: separate kernel; read per call, the tests compare the two)
   const char* fs = getenv("TFGNN_B200_RGAT_FUSED_SCORES");
   const bool tc_path = (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
-  const bool fuse_scores = !(fs && atoi(fs) == 0) && tc_path && gemm_tc_supported(Vs, LH, D, h, D, (const float*)P, LH) &&
+  const bool fuse_scores = !(fs && atoi(fs) == 0) && tc_path && gemm_tc_supported(Vs, LH, D, h, D, P.f(), LH) &&
                            gemm_tc_scores_supported(LH, H, d);
   if (fuse_scores) {
-    none.score_src = (float*)ss; none.score_tgt = (float*)stt; none.score_att = at;
+    none.score_src = ss.f(); none.score_tgt = stt.f(); none.score_att = at;
     none.score_H = H; none.score_K = K; none.score_d = d;
   }
-  rc = node_gemm(h, D, (const float*)Wcat, LH, (float*)P, LH, Vs, LH, D, none, path, b, st);
+  rc = node_gemm(h, D, Wcat.f(), LH, P.f(), LH, Vs, LH, D, none, path, st);
   if (rc) return rc;
   if (!fuse_scores) {
     const long long total = Vs * L * K;
-    rgat_scores_kernel<<<ceil_div(total, 256), 256, 0, st>>>((const float*)P, Vs, L, K, d, at, (float*)ss, (float*)stt);
+    rgat_scores_kernel<<<ceil_div(total, 256), 256, 0, st>>>(P.f(), Vs, L, K, d, at, ss.f(), stt.f());
     TFGNN_LAUNCH_CHECK();
   }
-  *P_out = (const float*)P;
-  *s_src_out = (const float*)ss;
-  *s_tgt_out = (const float*)stt;
   return 0;
 }
 
@@ -461,18 +450,18 @@ extern "C" int tfgnn_b200_rgat_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     wt.p[l] = W[l];
     at.p[l] = attention[l];
   }
-  const float *P = nullptr, *ss = nullptr, *stt = nullptr;
   int rc = batch_enter(b, st);
   if (rc) return rc;
+  PoolBuffer P{st}, ss{st}, stt{st};
   if (L > 0) {
-    rc = rgat_tables(b, h, D, wt, at, H, K, path, &P, &ss, &stt, st);
+    rc = rgat_tables(b, h, D, wt, at, H, K, path, P, ss, stt, st);
     if (rc) return rc;
   }
   const bool vec = (d % 4 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) && L > 0;
-  if (vec) return launch_rgat_aggregate(b, P, ss, stt, K, d, activation, out, st);
+  if (vec) return launch_rgat_aggregate(b, P.f(), ss.f(), stt.f(), K, d, activation, out, st);
   const long long threads = V * H;
   rgat_aggregate_kernel<false><<<ceil_div(threads, 128), 128, 0, st>>>(
-      P, ss, stt, b->row_ptr, b->src_sorted, V, b->tgt_off, L, K, d, activation, out);
+      P.f(), ss.f(), stt.f(), b->row_ptr, b->src_sorted, V, b->tgt_off, L, K, d, activation, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }
