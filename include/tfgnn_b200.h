@@ -407,6 +407,40 @@ TFGNN_API int tfgnn_b200_clamp(float* x, int64_t n, float lower, float upper, in
 TFGNN_API int tfgnn_b200_dense_bias_fwd(const float* x, const float* W, const float* bias, float* out, int64_t V, int32_t K,
                                         int32_t N, int32_t activation, int32_t path, void* stream);
 
+/* Backward of the readout and the exchange combines on the same row ranges.  No float atomics: every result is a function
+ * of its inputs alone (bitwise equal run to run, independent of the launch geometry).
+ *   segment_sum_rows       out[g,:] = sum of data[v,:] over graph_ptr[g] <= v < graph_ptr[g+1] (zeros for an empty graph): the
+ *                          adjoint of table[node_to_graph_map].  Rows are reduced in row order inside fixed 64-row chunks
+ *                          and a graph's chunk sums are added in a fixed order, so few long graphs and many short ones
+ *                          both fill the device
+ *   readout_bwd            backward of weighted_segment_sum through the weighting (tfgnn_readout_mode_t) and the clamp.
+ *                          node_reprs [V,GD] is the transformation result BEFORE the clamp, weights [V,K] the forward's
+ *                          softmax / sigmoid output (NULL for none / average), out [G,GD] the forward result (softmax only).
+ *                          With g = node_to_graph_map[v], R = clamp(node_reprs), d = GD/K:
+ *                            grad_reprs[v,kd+c] = w[v,k] grad_out[g,kd+c]  (none: w = 1, average: 1/max(n_g,1)); zero where the
+ *                              clamp cut: tf.maximum / tf.minimum pass the gradient where x >= lower resp. x <= upper
+ *                            dw[v,k] = sum_c grad_out[g,kd+c] R[v,kd+c]
+ *                            grad_scores[v,k] = dw w (1 - w)  (sigmoid)  |  w (dw - sum_c grad_out[g,kd+c] out[g,kd+c])  (softmax)
+ *   gru_gate_bwd_indexed   gru_gate_bwd for gx [G,3H] picked up through node_to_graph_map: grad_gh [V,3H], grad_h_direct
+ *                          [V,H] and grad_gx summed per graph to [G,3H] */
+typedef enum {
+  TFGNN_READOUT_SOFTMAX = 0,
+  TFGNN_READOUT_SIGMOID = 1,
+  TFGNN_READOUT_NONE = 2,
+  TFGNN_READOUT_AVERAGE = 3
+} tfgnn_readout_mode_t;
+TFGNN_API int tfgnn_b200_segment_sum_rows(const float* data, const int32_t* node_to_graph_map, const int32_t* graph_ptr,
+                                          int64_t num_rows, int32_t num_graphs, int32_t C, float* out, void* stream);
+TFGNN_API int tfgnn_b200_readout_bwd(const float* node_reprs, const float* weights, const int32_t* node_to_graph_map,
+                                     const int32_t* graph_ptr, const float* out, const float* grad_out, int64_t num_nodes,
+                                     int32_t num_graphs, int32_t repr_dim, int32_t num_heads, int32_t mode, float lower,
+                                     float upper, int32_t has_lower, int32_t has_upper, float* grad_reprs,
+                                     float* grad_scores, void* stream);
+TFGNN_API int tfgnn_b200_gru_gate_bwd_indexed(const float* gx, const int32_t* node_to_graph_map, const int32_t* graph_ptr,
+                                              const float* gh, const float* h, const float* grad_out, int64_t num_rows,
+                                              int32_t num_graphs, int32_t H, float* grad_gx, float* grad_gh,
+                                              float* grad_h_direct, void* stream);
+
 /* ---- On-device batch builder (SURVEY.md section 8f-2) ------------------------------------------------------
  * Bit-exact int32 bookkeeping of the data layer, so that a training loop never leaves the device between the
  * packed dataset and the layer call.

@@ -22,6 +22,7 @@ AGG = {"sum": 0, "mean": 1, "max": 2, "sqrt_n": 3}
 ACT = {None: 0, "relu": 1, "tanh": 2, "leaky_relu": 3, "elu": 4, "selu": 5, "gelu": 6}
 ACT_SIGMOID = 7  # library-internal (readout weights); deliberately NOT in the name table: the reference raises on "sigmoid"
 FLAG_NORMALIZE, FLAG_ACT_BEFORE_AGG, FLAG_USE_TARGET = 1, 2, 4
+READOUT_MODE = {"softmax": 0, "sigmoid": 1, "none": 2, "average": 3}
 PATH = {"auto": 0, "atomic": 1, "sorted": 2, "sorted_tc": 3, "fused_tc": 4}
 PREPARE_VALIDATE = 1
 PREPARE_TRANSPOSE = 2
@@ -44,6 +45,7 @@ EXPORTED_SYMBOLS = (
     "tfgnn_b200_rgcn_fwd_allgather", "tfgnn_b200_softmax_apply", "tfgnn_b200_head_scale", "tfgnn_b200_head_dot",
     "tfgnn_b200_gru_gate_bwd", "tfgnn_b200_rgcn_ln_fwd", "tfgnn_b200_film_bwd",
     "tfgnn_b200_edge_mlp_bwd", "tfgnn_b200_rgat_bwd",
+    "tfgnn_b200_segment_sum_rows", "tfgnn_b200_readout_bwd", "tfgnn_b200_gru_gate_bwd_indexed",
 )
 
 _PP = POINTER(c_void_p)
@@ -144,6 +146,12 @@ def lib() -> ctypes.CDLL:
                                           c_void_p, c_void_p]
     L.tfgnn_b200_rgcn_ln_fwd.argtypes = [c_void_p, c_void_p, c_int32, _PP, c_int32, c_uint32, c_int32, c_int32, c_int32,
                                          c_void_p, c_void_p, c_float, c_void_p, c_void_p]
+    L.tfgnn_b200_segment_sum_rows.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p]
+    L.tfgnn_b200_readout_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
+                                         c_int32, c_int32, c_int32, c_float, c_float, c_int32, c_int32, c_void_p, c_void_p,
+                                         c_void_p]
+    L.tfgnn_b200_gru_gate_bwd_indexed.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+                                                  c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]
     L.tfgnn_b200_set_l2_persist_mb.argtypes = [c_int32]
     L.tfgnn_b200_release_device_state.argtypes = []
     for name in EXPORTED_SYMBOLS:

@@ -206,16 +206,17 @@ __global__ void reduce_partials_kernel(const float* __restrict__ Cpart, int chun
 // ---- GGNN: Keras GRUCell (reset_after=True) backward, ggnn.py:84-87 -------------------------------------------------
 // forward: z = sig(gx_z+gh_z), r = sig(gx_r+gh_r), hh = tanh(gx_h + r*gh_h), h' = z*h + (1-z)*hh.
 // dgx = dL/dgx, dgh = dL/dgh, dh_direct = dL/dh' * z (the path of h through the convex combination).  dgx / dgh may be
-// gx / gh (GGNN's backward works in place): each thread reads its six pre-activations before it writes.
-__global__ void gru_gate_bwd_kernel(const float* gx, const float* gh, const float* __restrict__ h, int ldh,
-                                    const float* __restrict__ grad_out, long long V, int H, float* dgx, float* dgh,
-                                    float* __restrict__ dh_direct) {
+// gx / gh (GGNN's backward works in place): each thread reads its six pre-activations before it writes.  gx_index
+// (optional) picks row gx_index[v] of gx as gru_gate_kernel does; dgx is per node either way.
+__global__ void gru_gate_bwd_kernel(const float* gx, const int* __restrict__ gx_index, const float* gh,
+                                    const float* __restrict__ h, int ldh, const float* __restrict__ grad_out, long long V,
+                                    int H, float* dgx, float* dgh, float* __restrict__ dh_direct) {
   const long long total = V * H;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const long long v = i / H;
     const int c = (int)(i - v * H);
-    const float* x = gx + v * 3 * H;
+    const float* x = gx + (gx_index ? (long long)__ldg(gx_index + v) : v) * 3 * H;
     const float* y = gh + v * 3 * H;
     const float ghh = y[2 * H + c];
     const float hv = h[v * ldh + c];
@@ -650,7 +651,7 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     rc = node_gemm(h_tgt, D, gru_recurrent_kernel, N3, gh.f(), N3, V, N3, H, e1, TFGNN_PATH_AUTO, st);
     if (rc) return rc;
     // 2. gates, in place
-    gru_gate_bwd_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), gh.f(), h_tgt, D, grad_out, V, H, gx.f(), gh.f(),
+    gru_gate_bwd_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), nullptr, gh.f(), h_tgt, D, grad_out, V, H, gx.f(), gh.f(),
                                                          dhd.f());
     TFGNN_LAUNCH_CHECK();
     // 3. bias gradients: rows 0 / 1 of gru_bias belong to gx / gh
@@ -687,10 +688,33 @@ extern "C" int tfgnn_b200_gru_gate_bwd(const float* gx, const float* gh, const f
   TFGNN_REQUIRE(num_rows >= 0 && H > 0, "bad gru_gate_bwd sizes");
   if (num_rows == 0) return 0;
   TFGNN_REQUIRE(gx && gh && h && grad_out && grad_gx && grad_gh && grad_h_direct, "NULL pointer");
-  gru_gate_bwd_kernel<<<grid_for(num_rows * H), 256, 0, (cudaStream_t)stream>>>(gx, gh, h, H, grad_out, num_rows, H,
-                                                                               grad_gx, grad_gh, grad_h_direct);
+  gru_gate_bwd_kernel<<<grid_for(num_rows * H), 256, 0, (cudaStream_t)stream>>>(gx, nullptr, gh, h, H, grad_out, num_rows,
+                                                                               H, grad_gx, grad_gh, grad_h_direct);
   TFGNN_LAUNCH_CHECK();
   return 0;
+}
+
+// The GRU exchange's backward: gx = graph_repr K + b0 has one row per GRAPH, so grad_gx is the per-node gate gradient summed
+// over each graph's rows (tfgnn_b200_segment_sum_rows): the input-side GEMMs of the cell stay G-row GEMMs in the backward too.
+extern "C" int tfgnn_b200_gru_gate_bwd_indexed(const float* gx, const int32_t* node_to_graph_map, const int32_t* graph_ptr,
+                                               const float* gh, const float* h, const float* grad_out, int64_t num_rows,
+                                               int32_t num_graphs, int32_t H, float* grad_gx, float* grad_gh,
+                                               float* grad_h_direct, void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && num_rows < (1ll << 31) && num_graphs >= 0 && H > 0, "bad gru_gate_bwd_indexed sizes");
+  if (num_graphs == 0) return 0;
+  TFGNN_REQUIRE(graph_ptr && grad_gx, "NULL pointer");
+  TFGNN_REQUIRE(num_rows == 0 || (gx && node_to_graph_map && gh && h && grad_out && grad_gh && grad_h_direct),
+                "NULL pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  PoolBuffer dgx{st};
+  if (num_rows) {
+    int rc = dgx.alloc((size_t)num_rows * 3 * H * sizeof(float));
+    if (rc) return rc;
+    gru_gate_bwd_kernel<<<grid_for(num_rows * H), 256, 0, st>>>(gx, node_to_graph_map, gh, h, H, grad_out, num_rows, H,
+                                                               dgx.f(), grad_gh, grad_h_direct);
+    TFGNN_LAUNCH_CHECK();
+  }
+  return tfgnn_b200_segment_sum_rows(dgx.f(), node_to_graph_map, graph_ptr, num_rows, num_graphs, 3 * H, grad_gx, stream);
 }
 
 // =====================================================================================================================

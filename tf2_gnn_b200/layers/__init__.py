@@ -5,4 +5,4 @@ from .gnn import GNN, GNNInput
 from .graph_global_exchange import (GraphGlobalExchange, GraphGlobalExchangeInput, GraphGlobalGRUExchange,
                                     GraphGlobalMeanExchange, GraphGlobalMLPExchange)
 from .nodes_to_graph_representation import (NodesToGraphRepresentation, NodesToGraphRepresentationInput,
-                                            WeightedSumGraphRepresentation)
+                                            WASGraphRepresentation, WeightedSumGraphRepresentation)

@@ -15,7 +15,7 @@ import torch
 
 from ..runtime import to_device_f32
 from ..utils.param_helpers import get_activation_function
-from . import node_ops
+from . import graph_autograd, node_ops
 from .message_passing.message_passing import Variable, glorot_uniform
 from .nodes_to_graph_representation import (NodesToGraphRepresentationInput, WeightedSumGraphRepresentation, _MLP)
 
@@ -62,42 +62,35 @@ class GraphGlobalExchange:
         return self.call(inputs, training=training)
 
     def _prepare(self, inputs: GraphGlobalExchangeInput, training: bool):
-        """graph_global_exchange.py:83-103: per-graph representations [G, H] + the node -> graph index."""
+        """graph_global_exchange.py:83-103: the node states, the per-graph representations [G, H], node_to_graph_map and
+        graph_ptr.  With the exchange's own dropout active the representations come back per NODE ([V, H]) and the map is
+        None: tf.nn.dropout acts on the per-node copies (:98-101), the mask differs per node."""
         x = to_device_f32(inputs.node_embeddings)
         n2g = inputs.node_to_graph_map
         if not isinstance(n2g, torch.Tensor):
             n2g = torch.as_tensor(n2g)
         n2g = n2g.to(device=x.device, dtype=torch.int32).contiguous()
         num_graphs = int(inputs.num_graphs)
-        if node_ops._needs_grad(x, *[v.value for v in self.variables]):
-            # training: the reference's op order with per-op backward kernels; per-node copies are materialised
-            from .differentiable import per_node_graph_representations
-            return x, per_node_graph_representations(self, x, n2g, num_graphs, training), None
+        graph_ptr = node_ops.graph_offsets(n2g, num_graphs)
         self._node_to_graph_representation_layer.dropout_state = self.dropout_state
         graph_reprs = self._node_to_graph_representation_layer.call(
-            NodesToGraphRepresentationInput(x, n2g, num_graphs), training=training)
+            NodesToGraphRepresentationInput(x, n2g, num_graphs), training=training, graph_ptr=graph_ptr)
         if training and self._dropout_rate > 0.0:
-            # tf.nn.dropout on the per-NODE copies of the graph representation (:98-101): the mask differs per node, so the
-            # gathered table is materialised for this (training-only) case
-            ids = n2g.to(torch.int64)
-            per_node = torch.empty((x.shape[0], self._hidden_dim), dtype=torch.float32, device=x.device)
-            from .. import _ffi
-            from ..runtime import stream_ptr
-            _ffi.check(_ffi.lib().tfgnn_b200_gather_rows(graph_reprs.data_ptr(), num_graphs, self._hidden_dim, n2g.data_ptr(),
-                                                         1, int(x.shape[0]), per_node.data_ptr(), stream_ptr()))
-            del ids
-            return x, node_ops.dropout(per_node, self._dropout_rate, self.dropout_state), None
-        return x, graph_reprs, n2g
+            per_node = graph_autograd.gather_graph_rows(graph_reprs, n2g, graph_ptr)
+            return x, node_ops.dropout(per_node, self._dropout_rate, self.dropout_state), None, graph_ptr
+        return x, graph_reprs, n2g, graph_ptr
 
 
 class GraphGlobalMeanExchange(GraphGlobalExchange):
     """(x + g[node_to_graph_map]) / 2 (graph_global_exchange.py:106-124)."""
 
     def call(self, inputs: GraphGlobalExchangeInput, training: bool = False):
-        x, g, index = self._prepare(inputs, training)
+        x, g, index, graph_ptr = self._prepare(inputs, training)
         if node_ops._needs_grad(x, g):
-            from .differentiable import _AddFunction
-            return _AddFunction.apply(x, g, 0.5, 0.5)
+            if index is None:
+                from .differentiable import _AddFunction
+                return _AddFunction.apply(x, g, 0.5, 0.5)
+            return graph_autograd.gathered_add(x, g, index, graph_ptr, scale=0.5)
         return node_ops.gathered_add(x, g, index, scale=0.5)
 
 
@@ -120,10 +113,13 @@ class GraphGlobalGRUExchange(GraphGlobalExchange):
     trainable_variables = variables
 
     def call(self, inputs: GraphGlobalExchangeInput, training: bool = False):
-        x, g, index = self._prepare(inputs, training)
+        x, g, index, graph_ptr = self._prepare(inputs, training)
         if node_ops._needs_grad(x, g, self._gru_kernel.value, self._gru_recurrent_kernel.value, self._gru_bias.value):
-            from .differentiable import gru_cell
-            return gru_cell(g, x, self._gru_kernel.value, self._gru_recurrent_kernel.value, self._gru_bias.value)
+            if index is None:
+                from .differentiable import gru_cell
+                return gru_cell(g, x, self._gru_kernel.value, self._gru_recurrent_kernel.value, self._gru_bias.value)
+            return graph_autograd.gru_cell(g, index, graph_ptr, x, self._gru_kernel.value, self._gru_recurrent_kernel.value,
+                                           self._gru_bias.value)
         return node_ops.gru_cell(g, index, x, self._gru_kernel.value, self._gru_recurrent_kernel.value,
                                  self._gru_bias.value)
 
@@ -145,15 +141,21 @@ class GraphGlobalMLPExchange(GraphGlobalExchange):
     trainable_variables = variables
 
     def call(self, inputs: GraphGlobalExchangeInput, training: bool = False):
-        x, g, index = self._prepare(inputs, training)
+        x, g, index, graph_ptr = self._prepare(inputs, training)
         H = self._hidden_dim
         W1, W2 = self._mlp.kernels[0].value, self._mlp.kernels[1].value
-        if node_ops._needs_grad(x, g, W1, W2):
+        needs_grad = node_ops._needs_grad(x, g, W1, W2)
+        if needs_grad and index is None:
             # tf.concat([per_node_graph_representations, node_embeddings], -1) -> MLP (graph_global_exchange.py:176-181)
             return self._mlp(torch.cat([g, x], dim=-1), training, self.dropout_state)
         # first layer split by rows: [g || x] W1 = g W1[:H] + x W1[H:]; the graph half once per graph (or per node when the
-        # training-time dropout already materialised per-node copies: index is None then)
+        # training-time dropout already materialised per-node copies: index is None then).  The slices of W1 are views: under
+        # autograd the two halves' gradients land in the one variable.
+        relu = get_activation_function("relu")
         gp = node_ops.dense(g, W1[:H])
         xp = node_ops.dense(x, W1[H:])
-        hidden = node_ops.gathered_add(xp, gp, index, scale=1.0, activation=get_activation_function("relu"))
+        if needs_grad:
+            hidden = graph_autograd.gathered_add(xp, gp, index, graph_ptr, scale=1.0, activation=relu)
+        else:
+            hidden = node_ops.gathered_add(xp, gp, index, scale=1.0, activation=relu)
         return node_ops.dense(hidden, W2)

@@ -13,7 +13,7 @@ import torch
 
 from ..runtime import to_device_f32
 from ..utils.param_helpers import get_activation_function
-from . import node_ops
+from . import differentiable, graph_autograd, node_ops
 from .message_passing.message_passing import Variable, glorot_uniform
 
 
@@ -125,19 +125,71 @@ class WeightedSumGraphRepresentation(NodesToGraphRepresentation):
         num_graphs = int(inputs.num_graphs)
         if graph_ptr is None:
             graph_ptr = node_ops.graph_offsets(n2g, num_graphs)
-        weights = None
-        if self._weighting_fun not in ("none", "average"):                       # (1) weights per node / head
+        scores = None
+        if self._weighting_fun not in ("none", "average"):                       # (1) scores per node / head
             scores = self._scoring_mlp(x, training, self.dropout_state)           # [V, H]
-            if self._weighting_fun == "sigmoid":
-                weights = _sigmoid(scores)
-            else:
-                weights = node_ops.segment_softmax(scores, graph_ptr)
         reprs = self._transformation_mlp(x, training, self.dropout_state)         # (2) representations
-        if self._transformation_mlp_activation_fun is not None:
-            reprs = self._transformation_mlp_activation_fun(reprs)
-        node_ops.clamp_(reprs, self._transformation_mlp_result_lower_bound, self._transformation_mlp_result_upper_bound)
+        reprs = differentiable.activation(reprs, self._transformation_mlp_activation_fun)
+        lower, upper = self._transformation_mlp_result_lower_bound, self._transformation_mlp_result_upper_bound
+        if node_ops._needs_grad(scores, reprs):
+            # same forward kernels as below; backward on the graphs' row ranges (graph_autograd.py)
+            return graph_autograd.readout(scores, reprs, n2g, graph_ptr, self._num_heads, self._weighting_fun, lower, upper)
+        weights = None
+        if self._weighting_fun == "sigmoid":
+            weights = _sigmoid(scores)
+        elif self._weighting_fun == "softmax":
+            weights = node_ops.segment_softmax(scores, graph_ptr)
+        node_ops.clamp_(reprs, lower, upper)
         return node_ops.weighted_segment_sum(reprs, weights, graph_ptr, self._num_heads,      # (3) aggregate by graph
                                              mean=self._weighting_fun == "average")
+
+
+class WASGraphRepresentation(NodesToGraphRepresentation):
+    """_W_eighted _A_verage and _S_um graph representation (nodes_to_graph_representation.py:232-314): a softmax- and a
+    sigmoid-weighted WeightedSumGraphRepresentation, concatenated and projected without bias; same constructor arguments
+    and defaults."""
+
+    def __init__(self, graph_representation_size: int = 128, num_heads: int = 8, pooling_mlp_layers: List[int] = [128, 128],
+                 pooling_mlp_activation_fun: str = "elu", pooling_mlp_use_biases: bool = True,
+                 pooling_mlp_dropout_rate: float = 0.0, **kwargs):
+        super().__init__(graph_representation_size, **kwargs)
+
+        def pooling(weighting_fun: str) -> WeightedSumGraphRepresentation:
+            return WeightedSumGraphRepresentation(
+                graph_representation_size=graph_representation_size, num_heads=num_heads, weighting_fun=weighting_fun,
+                scoring_mlp_layers=pooling_mlp_layers, scoring_mlp_dropout_rate=pooling_mlp_dropout_rate,
+                scoring_mlp_use_biases=pooling_mlp_use_biases, scoring_mlp_activation_fun=pooling_mlp_activation_fun,
+                transformation_mlp_layers=pooling_mlp_layers, transformation_mlp_dropout_rate=pooling_mlp_dropout_rate,
+                transformation_mlp_use_biases=pooling_mlp_use_biases,
+                transformation_mlp_activation_fun=pooling_mlp_activation_fun)
+
+        self._weighted_avg_graph_repr_layer = pooling("softmax")
+        self._weighted_sum_graph_repr_layer = pooling("sigmoid")
+        self._out_projection: Optional[Variable] = None
+        self.dropout_state = None
+
+    def build(self, input_shapes: NodesToGraphRepresentationInput, name: str = "WASGraphRepresentation"):
+        self._weighted_avg_graph_repr_layer.build(
+            input_shapes, name=f"{name}/WeightedAvgGraphRepresentation/WeightedSumGraphRepresentation")
+        self._weighted_sum_graph_repr_layer.build(
+            input_shapes, name=f"{name}/WeightedSumGraphRepresentation/WeightedSumGraphRepresentation")
+        size = self._graph_representation_size
+        self._out_projection = Variable(f"{name}/dense/kernel:0", glorot_uniform((2 * size, size)))
+        self.built = True
+
+    @property
+    def variables(self) -> List[Variable]:
+        return (self._weighted_avg_graph_repr_layer.variables + self._weighted_sum_graph_repr_layer.variables
+                + [self._out_projection])
+
+    trainable_variables = variables
+
+    def call(self, inputs: NodesToGraphRepresentationInput, training: bool = False):
+        self._weighted_avg_graph_repr_layer.dropout_state = self.dropout_state
+        self._weighted_sum_graph_repr_layer.dropout_state = self.dropout_state
+        avg_graph_repr = self._weighted_avg_graph_repr_layer.call(inputs, training=training)
+        sum_graph_repr = self._weighted_sum_graph_repr_layer.call(inputs, training=training)
+        return node_ops.dense(torch.cat([avg_graph_repr, sum_graph_repr], dim=-1), self._out_projection.value)
 
 
 def _sigmoid(x: torch.Tensor) -> torch.Tensor:
