@@ -271,7 +271,8 @@ TFGNN_API int tfgnn_b200_film_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, 
                         void* stream);
 
 /* RGAT (rgat.py:91-163): per-type projection W_l [D,H], attention a_l [K, 2H/K]; softmax over all
- * incoming edges of all types jointly, per head; activation after. */
+ * incoming edges of all types jointly, per head; activation after.  The result is run-to-run reproducible (no float
+ * atomics, hub targets included). */
 TFGNN_API int tfgnn_b200_rgat_fwd(tfgnn_batch_t* batch, const float* h, int32_t D, const float* const* W,
                         const float* const* attention, int32_t H, int32_t num_heads,
                         int32_t activation, int32_t path, float* out, void* stream);

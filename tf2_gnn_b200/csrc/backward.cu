@@ -1171,7 +1171,7 @@ extern "C" int tfgnn_b200_edge_mlp_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, cons
 // =====================================================================================================================
 // RGAT backward (rgat.py:91-163 through tfgnn_b200_rgat_fwd; edge-level kernels and their math in rgat.cu).  With
 // P_l = h W_l, the score halves s_src, s_tgt of the forward and dZ = dOut * act':
-//   1. dZ (gelu: the pre-activation from the backward's own target walk, deterministic on hub rows too)
+//   1. dZ (gelu: the pre-activation from the forward's target walk with activation none)
 //   2. P, s_src, s_tgt recomputed by the forward's rgat_tables: the forward's bits
 //   3. target pass: m, den, g = dZ . o per (v, k) and ds_tgt [V, L*K]
 //   4. source pass over the source-keyed CSR: dP [Vs, L*H] (messages and both score halves) and ds_src [Vs, L*K]
@@ -1215,7 +1215,7 @@ extern "C" int tfgnn_b200_rgat_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   int rc = begin_backward(b, bt, out, grad_out, H, activation, TFGNN_AGG_SUM, st, dz, [&](float* z) {
     PoolBuffer P{st}, ss{st}, stt{st};
     const int r = rgat_tables(b, h, D, wt, at, H, K, path, P, ss, stt, st);
-    return r ? r : launch_rgat_target_pass(b, P.f(), ss.f(), stt.f(), K, d, nullptr, nullptr, nullptr, z, st);
+    return r ? r : launch_rgat_aggregate(b, P.f(), ss.f(), stt.f(), K, d, TFGNN_ACT_NONE, z, st);
   });
   if (rc) return rc;
   // 2. the forward's tables
@@ -1229,7 +1229,7 @@ extern "C" int tfgnn_b200_rgat_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   if (!rc) rc = ds_src.alloc((size_t)Vs * LK * sizeof(float));
   if (rc) return rc;
   // 3., 4. target pass, source pass
-  rc = launch_rgat_target_pass(b, P.f(), ss.f(), stt.f(), K, d, dz.f(), stat.f(), ds_tgt.f(), nullptr, st);
+  rc = launch_rgat_target_pass(b, P.f(), ss.f(), stt.f(), K, d, dz.f(), stat.f(), ds_tgt.f(), st);
   if (rc) return rc;
   rc = launch_rgat_source_pass(b, bt, P.f(), ss.f(), stt.f(), at, K, d, dz.f(), stat.f(), ds_tgt.f(), dP.f(), ds_src.f(),
                                st);

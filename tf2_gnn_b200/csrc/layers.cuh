@@ -20,18 +20,18 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
 int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                      uint32_t flags, int aggregation, int activation, const float* FB, int ldf, int path, float* out,
                      int ldo, cudaStream_t st);
-// RGAT edge-level aggregation (rgat.cu): warp per target + chunked hub path; needs (H/K) % 4 == 0
+// RGAT edge-level aggregation (rgat.cu): the target walk in output mode, out = act(o) [V, H]; needs (H/K) % 4 == 0
 int launch_rgat_aggregate(tfgnn_batch* b, const float* P, const float* s_src, const float* s_tgt, int K, int d,
                           int activation, float* out, cudaStream_t st);
 // RGAT projection P and score halves s_src, s_tgt of the forward, into the caller's buffers (variants.cu); L > 0
 int rgat_tables(tfgnn_batch* b, const float* h, int D, const PtrTable& wt, const PtrTable& at, int H, int K, int path,
                 PoolBuffer& P, PoolBuffer& s_src, PoolBuffer& s_tgt, cudaStream_t st);
 // Edge-level steps of the RGAT backward (rgat.cu), no float atomics; d % 4 == 0, H <= 512.
-//   target pass, dz given: stat [V, 3K] = (m, den, g) per head, ds_tgt [V, L*K];  dz NULL: the pre-activation pre [V, H]
+//   target pass (the target walk in statistics mode): stat [V, 3K] = (m, den, g) per head, ds_tgt [V, L*K]
 //   source pass over bt's source-keyed CSR: dP [Vs, L*H], ds_src [Vs, L*K]
 //   attention gradient: rows of ds [rows, L*K] and P (ldP = L*H) -> half `half` (0: source, 1: target) of every grad_att[l]
 int launch_rgat_target_pass(tfgnn_batch* b, const float* P, const float* s_src, const float* s_tgt, int K, int d,
-                            const float* dz, float* stat, float* ds_tgt, float* pre, cudaStream_t st);
+                            const float* dz, float* stat, float* ds_tgt, cudaStream_t st);
 int launch_rgat_source_pass(const tfgnn_batch* b, const tfgnn_batch* bt, const float* P, const float* s_src,
                             const float* s_tgt, const PtrTable& att, int K, int d, const float* dz, const float* stat,
                             const float* ds_tgt, float* dP, float* ds_src, cudaStream_t st);

@@ -4,261 +4,38 @@
 // Node-level part (variants.cu): P_l = h W_l for every node once, and the per-edge score is split by linearity
 // of the einsum (rgat.py:115-121) into node-level halves s_src[u,l,k] + s_tgt[v,l,k].
 //
-// Edge-level part (this file), HBM-bound: per edge 4 B index + 4*K B of source scores (twice) + 4*H B of P row.
-//   * regular targets (in-degree <= kHubThreshold): one WARP per target, lanes over float4 column groups,
-//     two passes over the CSR segments (running max, then exp-sum + weighted accumulate): coalesced 4*H-byte
-//     row reads, no atomics, deterministic.
-//   * hub targets (power-law graphs: up to 1e5+ incoming edges): the joint edge list is cut into chunks of
-//     kHubChunk edges, one warp per chunk; chunk results are combined with float atomics (max, then sum)
-//     and normalised in a final pass.  Without this a single warp would walk a hub serially for ~50 ms.
+// Edge-level part (this file), HBM-bound: per edge 4 B index + 4*K B of source scores + 4*H B of P row.  The forward and the
+// backward's statistics share ONE target walk (rgat_warp_kernel):
+//   * regular targets (in-degree <= kHubThreshold): one warp per target, lanes over float4 column groups, one pass over
+//     the CSR segments with a running maximum ("online softmax"): when the maximum grows, the sums so far are rescaled by
+//     exp(m_old - m_new), so every edge's score and P row are read once.
+//   * hub targets (power-law graphs: up to 1e5+ incoming edges): the joint edge list is cut into chunks of kHubChunk edges,
+//     one warp per chunk; each chunk writes its partial and the partials are combined in chunk order
+//     (rgat_hub_combine_kernel).  Without this a single warp would walk a hub serially for ~50 ms.
+// No float atomics: every result is bitwise reproducible.
+//
+// Backward (tfgnn_b200_rgat_bwd, backward.cu).  For an edge e = (u -> v) of type l and head k: x_e = s_src[u,l,k] +
+// s_tgt[v,l,k], sigma_e = leaky(x_e), alpha_e = exp(sigma_e - m[v,k]) / den[v,k], and with dZ = dOut * act':
+//   da_e = dZ[v]_k . P_l[u]_k,   g[v,k] = sum_e alpha_e da_e,   dx_e = alpha_e (da_e - g[v,k]) leaky'(x_e)
+//   ds_tgt[v,l,k] = sum over the edges of type l into v of dx_e                      (target walk, statistics mode)
+//   ds_src[u,l,k] = sum over the edges of type l leaving u of dx_e,
+//   dP_l[u]_k = sum over those edges of alpha_e dZ[v]_k + ds_src[u,l,k] a_l[k,:d] + ds_tgt[u,l,k] a_l[k,d:]   (source pass)
+// In statistics mode the walk keeps den = sum w_e, G = sum w_e da_e and, for the type being walked, A1 = sum w_e leaky'(x_e)
+// da_e and A2 = sum w_e leaky'(x_e), all rescaled by exp(m_old - m_new) when the maximum grows.  At the end of each type A1,
+// A2 and the maximum they refer to are flushed to memory; after the walk they are brought to the final maximum: g = G / den,
+// ds_tgt = (A1 - g A2) / den.  A hub chunk's partial is (m_c, den_c, G_c, A1_c, A2_c).  A head's dot product (d columns =
+// d/4 float4 groups) is summed inside the warp by rgat_head_sum.
 #include "layers.cuh"
 
 namespace tfgnn {
 
 constexpr int kHubThreshold = 2048;
 constexpr int kHubChunk = 1024;
+constexpr int kRgatRowChunk = 8192;   // rows per partial of the attention gradient
 
 __device__ __forceinline__ float rgat_leaky(float x) { return x > 0.f ? x : kLeakyReluAlpha * x; }
 
-__device__ __forceinline__ void rgat_atomic_max(float* addr, float val) {
-  if (__float_as_int(val) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(val));   // sign bit: -0.0f goes to the atomicMin branch
-  else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(val));
-}
-
-struct RgatParams {
-  const float* P;       // [Vs, L*H]
-  const float* s_src;   // [Vs, L*K]
-  const float* s_tgt;   // [Vs, L*K]
-  const int* row_ptr;
-  const int* src;
-  long long V, tgt_off;
-  int L, K, d, H, act;
-  float* out;           // [V, H]
-  // hub machinery
-  float* hub_max;       // [V, K]
-  float* hub_den;       // [V, K]
-  int2* items;          // (target, chunk)
-  int* item_count;
-};
-
-// One pass over the edges [e_lo, e_hi) of segment (l, v) for this lane's column group (head k):
-//   PASS 0: m = max(m, score)      PASS 1: w = exp(score - m); den += w; acc += w * P_l[src, c..c+3]
-//   PASS 2 (regular targets): ONE pass with a running maximum ("online softmax"): when the maximum grows, the sums so
-//   far are rescaled by exp(m_old - m_new).  Every edge's score and P row are read once instead of twice (round 1 walked
-//   each target's edges twice: 13 ms of the 22 ms cfg3 layer).
-template <int PASS>
-__device__ __forceinline__ void rgat_walk(const RgatParams& p, int l, int e_lo, int e_hi, float st, int k, int c,
-                                          int lane, bool col_ok, float& m, float& den, float4& acc) {
-  const long long LK = (long long)p.L * p.K, LH = (long long)p.L * p.H;
-  for (int base = e_lo; base < e_hi; base += 32) {
-    const int n = min(32, e_hi - base);
-    const int my_src = lane < n ? __ldg(p.src + base + lane) : 0;
-    for (int j0 = 0; j0 < n; j0 += 4) {
-      float sc[4];
-      float4 x[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const long long s = __shfl_sync(0xffffffffu, my_src, (j0 + u) & 31);
-        const bool ok = (j0 + u < n) && col_ok;
-        sc[u] = ok ? __ldg(p.s_src + s * LK + l * p.K + k) : 0.f;
-        if (PASS >= 1) x[u] = ok ? ldg_f4(p.P + s * LH + (long long)l * p.H + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        if (j0 + u < n) {
-          const float score = rgat_leaky(sc[u] + st);
-          if (PASS == 0) {
-            m = fmaxf(m, score);
-          } else if (PASS == 2) {
-            // one expf per edge: either the maximum grows (weight of this edge is exp(0) = 1, the sums so far are rescaled;
-            // the very first edge has m = -FLT_MAX: rescale = 0) or it stays (no rescale)
-            if (score > m) {
-              const float rescale = expf(m - score);
-              m = score;
-              den = fmaf(den, rescale, 1.0f);
-              acc.x = fmaf(acc.x, rescale, x[u].x); acc.y = fmaf(acc.y, rescale, x[u].y);
-              acc.z = fmaf(acc.z, rescale, x[u].z); acc.w = fmaf(acc.w, rescale, x[u].w);
-            } else {
-              const float w = expf(score - m);
-              den += w;
-              acc.x = fmaf(w, x[u].x, acc.x); acc.y = fmaf(w, x[u].y, acc.y);
-              acc.z = fmaf(w, x[u].z, acc.z); acc.w = fmaf(w, x[u].w, acc.w);
-            }
-          } else {
-            const float w = expf(score - m);
-            den += w;
-            acc.x = fmaf(w, x[u].x, acc.x); acc.y = fmaf(w, x[u].y, acc.y);
-            acc.z = fmaf(w, x[u].z, acc.z); acc.w = fmaf(w, x[u].w, acc.w);
-          }
-        }
-      }
-    }
-  }
-}
-
-// Regular targets: one warp per (target, 32-column-group block).  NVW = number of 128-column blocks (H <= 128*NVW
-// handled by blockIdx.y).  Hubs are skipped here.
-__global__ void __launch_bounds__(256) rgat_warp_kernel(const RgatParams p) {
-  const int lane = threadIdx.x & 31;
-  const long long v = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (v >= p.V) return;
-  const int c = (blockIdx.y * 32 + lane) * 4;
-  const bool col_ok = c < p.H;
-  const int k = col_ok ? c / p.d : 0;
-  int deg = 0;
-  for (int l = 0; l < p.L; ++l) {
-    const long long seg = (long long)l * p.V + v;
-    deg += __ldg(p.row_ptr + seg + 1) - __ldg(p.row_ptr + seg);
-  }
-  if (deg > kHubThreshold) return;   // handled by the hub kernels
-  const long long LK = (long long)p.L * p.K;
-  float m = kLowestFloat, den = 0.f;
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int l = 0; l < p.L; ++l) {
-    const long long seg = (long long)l * p.V + v;
-    const float st = __ldg(p.s_tgt + (v + p.tgt_off) * LK + l * p.K + k);
-    rgat_walk<2>(p, l, __ldg(p.row_ptr + seg), __ldg(p.row_ptr + seg + 1), st, k, c, lane, col_ok, m, den, acc);
-  }
-  if (col_ok) {
-    const float inv = den > 0.f ? 1.0f / den : 0.f;
-    float o[4] = {acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv};
-    apply_act_vec<4>(o, p.act);
-    *reinterpret_cast<float4*>(p.out + v * p.H + c) = make_float4(o[0], o[1], o[2], o[3]);
-  }
-}
-
-// Hub discovery: one thread per target; a hub gets ceil(deg / kHubChunk) work items and its accumulators reset.
-__global__ void rgat_hub_scan_kernel(const RgatParams p) {
-  for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < p.V;
-       v += (long long)gridDim.x * blockDim.x) {
-    int deg = 0;
-    for (int l = 0; l < p.L; ++l) {
-      const long long seg = (long long)l * p.V + v;
-      deg += p.row_ptr[seg + 1] - p.row_ptr[seg];
-    }
-    if (deg <= kHubThreshold) continue;
-    const int nchunks = (deg + kHubChunk - 1) / kHubChunk;
-    const int base = atomicAdd(p.item_count, nchunks);
-    for (int c = 0; c < nchunks; ++c) p.items[base + c] = make_int2((int)v, c);
-    for (int k = 0; k < p.K; ++k) {
-      p.hub_max[v * p.K + k] = kLowestFloat;
-      p.hub_den[v * p.K + k] = 0.f;
-    }
-    for (int c = 0; c < p.H; ++c) p.out[v * p.H + c] = 0.f;
-  }
-}
-
-// Hub chunk pass: warp per (item, 128-column block).  PASS 0: chunk max -> atomic max.  PASS 1: chunk exp-sum and
-// weighted sum against the final max -> atomic adds into hub_den and out (un-normalised).
-template <int PASS>
-__global__ void __launch_bounds__(256) rgat_hub_chunk_kernel(const RgatParams p) {
-  const int lane = threadIdx.x & 31;
-  const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-  const int count = *p.item_count;
-  const int c = (blockIdx.y * 32 + lane) * 4;
-  const bool col_ok = c < p.H;
-  const int k = col_ok ? c / p.d : 0;
-  const long long LK = (long long)p.L * p.K;
-  for (long long it = warp; it < count; it += nwarps) {
-    const int2 item = p.items[it];
-    const long long v = item.x;
-    const int r_lo = item.y * kHubChunk, r_hi = r_lo + kHubChunk;   // rank range in the joint edge list of v
-    float m = PASS == 0 ? kLowestFloat : (col_ok ? p.hub_max[v * p.K + k] : 0.f);
-    float den = 0.f;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    int rank0 = 0;
-    for (int l = 0; l < p.L; ++l) {
-      const long long seg = (long long)l * p.V + v;
-      const int beg = __ldg(p.row_ptr + seg), end = __ldg(p.row_ptr + seg + 1);
-      const int lo = max(r_lo - rank0, 0), hi = min(r_hi - rank0, end - beg);
-      if (lo < hi) {
-        const float st = __ldg(p.s_tgt + (v + p.tgt_off) * LK + l * p.K + k);
-        rgat_walk<PASS>(p, l, beg + lo, beg + hi, st, k, c, lane, col_ok, m, den, acc);
-      }
-      rank0 += end - beg;
-    }
-    if (!col_ok) continue;
-    if (PASS == 0) {
-      if ((c % p.d) == 0) rgat_atomic_max(p.hub_max + v * p.K + k, m);
-    } else {
-      if ((c % p.d) == 0) atomicAdd(p.hub_den + v * p.K + k, den);
-      float* o = p.out + v * p.H + c;
-      atomicAdd(o, acc.x); atomicAdd(o + 1, acc.y); atomicAdd(o + 2, acc.z); atomicAdd(o + 3, acc.w);
-    }
-  }
-}
-
-__global__ void rgat_hub_finalize_kernel(const RgatParams p) {
-  const int count = *p.item_count;
-  for (int it = blockIdx.x; it < count; it += gridDim.x) {
-    const int2 item = p.items[it];
-    if (item.y != 0) continue;           // once per hub
-    const long long v = item.x;
-    for (int c = threadIdx.x; c < p.H; c += blockDim.x) {
-      const float den = p.hub_den[v * p.K + c / p.d];
-      float o[1] = {den > 0.f ? p.out[v * p.H + c] / den : 0.f};
-      apply_act_vec<1>(o, p.act);
-      p.out[v * p.H + c] = o[0];
-    }
-  }
-}
-
-int launch_rgat_aggregate(tfgnn_batch* b, const float* P, const float* s_src, const float* s_tgt, int K, int d,
-                          int activation, float* out, cudaStream_t st) {
-  RgatParams p{};
-  p.P = P; p.s_src = s_src; p.s_tgt = s_tgt; p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-  p.V = b->V; p.tgt_off = b->tgt_off; p.L = b->L; p.K = K; p.d = d; p.H = K * d; p.act = activation; p.out = out;
-  const long long max_items = b->M_in / kHubChunk + b->M_in / kHubThreshold + 2;
-  PoolBuffer hm{st}, hd{st}, items{st};
-  int rc = hm.alloc((size_t)p.V * K * sizeof(float));
-  if (!rc) rc = hd.alloc((size_t)p.V * K * sizeof(float));
-  if (!rc) rc = items.alloc((size_t)max_items * sizeof(int2) + 16);
-  if (rc) return rc;
-  p.hub_max = hm.f(); p.hub_den = hd.f();
-  p.item_count = (int*)items.p;
-  p.items = reinterpret_cast<int2*>(reinterpret_cast<char*>(items.p) + 16);
-  TFGNN_CUDA(cudaMemsetAsync(p.item_count, 0, sizeof(int), st));
-  const int col_blocks = (p.H / 4 + 31) / 32;
-  int scan_blocks = ceil_div(p.V, 256);
-  if (scan_blocks > 132 * 16) scan_blocks = 132 * 16;
-  rgat_hub_scan_kernel<<<scan_blocks, 256, 0, st>>>(p);
-  TFGNN_LAUNCH_CHECK();
-  {
-    dim3 grid((unsigned)ceil_div(p.V * 32, 256), col_blocks);
-    rgat_warp_kernel<<<grid, 256, 0, st>>>(p);
-    TFGNN_LAUNCH_CHECK();
-  }
-  {
-    dim3 grid(132 * 4, col_blocks);
-    rgat_hub_chunk_kernel<0><<<grid, 256, 0, st>>>(p);
-    TFGNN_LAUNCH_CHECK();
-    rgat_hub_chunk_kernel<1><<<grid, 256, 0, st>>>(p);
-    TFGNN_LAUNCH_CHECK();
-    rgat_hub_finalize_kernel<<<132, 128, 0, st>>>(p);
-    TFGNN_LAUNCH_CHECK();
-  }
-  return 0;
-}
-
-// ---- Backward (tfgnn_b200_rgat_bwd, backward.cu) -----------------------------------------------------------------------
-// For an edge e = (u -> v) of type l and head k: x_e = s_src[u,l,k] + s_tgt[v,l,k], sigma_e = leaky(x_e),
-// alpha_e = exp(sigma_e - m[v,k]) / den[v,k], and with dZ = dOut * act':
-//   da_e = dZ[v]_k . P_l[u]_k,   g[v,k] = sum_e alpha_e da_e,   dx_e = alpha_e (da_e - g[v,k]) leaky'(x_e)
-//   ds_tgt[v,l,k] = sum over the edges of type l into v of dx_e                      (target pass)
-//   ds_src[u,l,k] = sum over the edges of type l leaving u of dx_e,
-//   dP_l[u]_k = sum over those edges of alpha_e dZ[v]_k + ds_src[u,l,k] a_l[k,:d] + ds_tgt[u,l,k] a_l[k,d:]   (source pass)
-// The target pass is ONE walk over a target's edges with the forward's running maximum (rgat_warp_kernel): it keeps
-// den = sum w_e, G = sum w_e da_e and, for the type being walked, A1 = sum w_e leaky'(x_e) da_e and A2 = sum w_e leaky'(x_e),
-// all rescaled by exp(m_old - m_new) when the maximum grows.  At the end of each type A1, A2 and the maximum they refer to
-// are flushed to memory; after the walk they are brought to the final maximum: g = G / den, ds_tgt = (A1 - g A2) / den.
-// A hub (more than kHubThreshold incoming edges) is cut into kHubChunk-edge chunks, one warp per chunk; each chunk writes
-// its partial (m_c, den_c, G_c, A1_c, A2_c) and the partials are combined in chunk order.  No float atomics: every result
-// is bitwise reproducible.  A head's dot product (d columns = d/4 float4 groups) is summed inside the warp by rgat_head_sum.
-
-constexpr int kRgatRowChunk = 8192;   // rows per partial of the attention gradient
-
-struct RgatBwdParams {
+struct RgatWalkParams {
   const float* P;       // [Vs, L*H]
   const float* s_src;   // [Vs, L*K]
   const float* s_tgt;   // [Vs, L*K]
@@ -266,16 +43,17 @@ struct RgatBwdParams {
   const int* src;
   long long V, tgt_off;
   int L, K, d, H;
-  const float* dz;      // [V, H]; NULL: the walk forms the pre-activation instead
+  int act;              // output mode: activation of out
+  float* out;           // output mode: [V, H]
+  const float* dz;      // [V, H]; NULL: output mode
   float* stat;          // [V, 3K]: m, den, g per head
   float* a1;            // [V, L*K]: flushed A1 of regular targets, then ds_tgt
   float* a2;            // [V, L*K]: flushed A2
   float* ml;            // [V, L*K]: the maximum A1, A2 refer to
-  float* pre;           // [V, H]   (pre-activation walk)
   const int2* items;    // hub chunks (target, chunk), the chunks of a hub consecutive
   const int* item_count;
   float* hstat;         // [items, 3K]: m_c, den_c, G_c
-  float* ha1;           // [items, L*K] (pre-activation walk: hacc [items, H])
+  float* ha1;           // [items, L*K] (output mode: the un-normalised row acc_c [items, H])
   float* ha2;
   float* hml;
 };
@@ -323,9 +101,9 @@ __device__ __forceinline__ float dot4(float4 a, float4 b) {
   return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x)));
 }
 
-// Hub discovery of the backward: one thread per target; a hub gets ceil(deg / kHubChunk) consecutive work items.
-__global__ void rgat_bwd_hub_scan_kernel(const int* __restrict__ row_ptr, long long V, int L, int2* __restrict__ items,
-                                         int* __restrict__ item_count) {
+// Hub discovery: one thread per target; a hub gets ceil(deg / kHubChunk) consecutive work items.
+__global__ void rgat_hub_scan_kernel(const int* __restrict__ row_ptr, long long V, int L, int2* __restrict__ items,
+                                     int* __restrict__ item_count) {
   for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += (long long)gridDim.x * blockDim.x) {
     int deg = 0;
     for (int l = 0; l < L; ++l) deg += row_ptr[(long long)l * V + v + 1] - row_ptr[(long long)l * V + v];
@@ -336,11 +114,15 @@ __global__ void rgat_bwd_hub_scan_kernel(const int* __restrict__ row_ptr, long l
   }
 }
 
-// Target pass: one warp per regular target (w < V) or hub chunk (w >= V), lanes over float4 column groups, NV groups per
-// lane.  PRE: the same walk forms the pre-activation o = sum alpha_e P_l[u] (gelu's derivative needs it) with the forward's
-// operations, so it has the forward's bits on regular targets.
-template <int NV, bool PRE>
-__global__ void __launch_bounds__(256) rgat_bwd_target_kernel(const RgatBwdParams p) {
+// The target walk: one warp per (work item, column block of 32 NV float4 groups, blockIdx.y), where a work item is a
+// regular target (w < V) or a hub chunk (w >= V); NV groups per lane.
+//   output mode (!STATS, the forward): act(o) of regular rows into out, the partial (m_c, den_c, acc_c) of hub chunks; the
+//     score and P-row loads of 4 edges are issued before they are used.
+//   statistics mode (STATS, the backward; one column block, so a head's dot product stays in the warp): stat and ds_tgt.
+// Both modes apply the same operations per edge, so the backward's statistics refer to the forward's bits.
+template <int NV, bool STATS>
+__global__ void __launch_bounds__(256) rgat_warp_kernel(const RgatWalkParams p) {
+  constexpr int EB = STATS ? 1 : 4;   // edges per batch of loads
   __shared__ float red_all[8][32 * NV];
   const int lane = threadIdx.x & 31;
   float* red = red_all[threadIdx.x >> 5];
@@ -351,7 +133,7 @@ __global__ void __launch_bounds__(256) rgat_bwd_target_kernel(const RgatBwdParam
   bool ok[NV], lead[NV];
 #pragma unroll
   for (int j = 0; j < NV; ++j) {
-    q[j] = lane + 32 * j;
+    q[j] = lane + 32 * (blockIdx.y * NV + j);
     ok[j] = q[j] < C4;
     k[j] = ok[j] ? q[j] / g : 0;
     lead[j] = ok[j] && q[j] % g == 0;   // the head's first lane writes its per-head values
@@ -360,7 +142,7 @@ __global__ void __launch_bounds__(256) rgat_bwd_target_kernel(const RgatBwdParam
        w += ((long long)gridDim.x * blockDim.x) >> 5) {
     const bool hub = w >= p.V;
     long long v;
-    int r_lo = 0, r_hi = 0x7fffffff;   // rank range in the joint edge list of v
+    int r_lo = 0, r_hi = 0x7fffffff;   // rank range in the joint edge list of v, then in the rest of it
     if (!hub) {
       v = w;
       int deg = 0;
@@ -380,17 +162,17 @@ __global__ void __launch_bounds__(256) rgat_bwd_target_kernel(const RgatBwdParam
     float m[NV], den[NV], G[NV], A1[NV], A2[NV];
 #pragma unroll
     for (int j = 0; j < NV; ++j) {
-      z[j] = (!PRE && ok[j]) ? ldg_f4(p.dz + v * p.H + 4 * q[j]) : make_float4(0.f, 0.f, 0.f, 0.f);
+      z[j] = (STATS && ok[j]) ? ldg_f4(p.dz + v * p.H + 4 * q[j]) : make_float4(0.f, 0.f, 0.f, 0.f);
       acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
       m[j] = kLowestFloat;
       den[j] = G[j] = 0.f;
     }
-    int rank0 = 0;
     for (int l = 0; l < p.L; ++l) {
       const long long seg = (long long)l * p.V + v;
       const int beg = __ldg(p.row_ptr + seg), end = __ldg(p.row_ptr + seg + 1);
-      const int e_lo = beg + max(r_lo - rank0, 0), e_hi = beg + min(r_hi - rank0, end - beg);
-      rank0 += end - beg;
+      const int e_lo = beg + max(r_lo, 0), e_hi = beg + min(r_hi, end - beg);
+      r_lo -= end - beg;
+      r_hi -= end - beg;
       float st[NV];
 #pragma unroll
       for (int j = 0; j < NV; ++j) {
@@ -400,50 +182,63 @@ __global__ void __launch_bounds__(256) rgat_bwd_target_kernel(const RgatBwdParam
       for (int base = e_lo; base < e_hi; base += 32) {
         const int n = min(32, e_hi - base);
         const int my_src = lane < n ? __ldg(p.src + base + lane) : 0;
-        for (int e = 0; e < n; ++e) {
-          const long long u = __shfl_sync(0xffffffffu, my_src, e);
-          float sc[NV], da[NV];
-          float4 x[NV];
+        for (int e0 = 0; e0 < n; e0 += EB) {
+          float sc[EB][NV];
+          float4 x[EB][NV];
 #pragma unroll
-          for (int j = 0; j < NV; ++j) {
-            sc[j] = ok[j] ? __ldg(p.s_src + u * LK + l * p.K + k[j]) : 0.f;
-            x[j] = ok[j] ? ldg_f4(p.P + u * LH + (long long)l * p.H + 4 * q[j]) : make_float4(0.f, 0.f, 0.f, 0.f);
-            da[j] = PRE ? 0.f : dot4(z[j], x[j]);
+          for (int i = 0; i < EB; ++i) {
+            const long long u = __shfl_sync(0xffffffffu, my_src, (e0 + i) & 31);
+#pragma unroll
+            for (int j = 0; j < NV; ++j) {
+              const bool in = ok[j] && e0 + i < n;
+              sc[i][j] = in ? __ldg(p.s_src + u * LK + l * p.K + k[j]) : 0.f;
+              x[i][j] = in ? ldg_f4(p.P + u * LH + (long long)l * p.H + 4 * q[j]) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
           }
-          if (!PRE) rgat_head_sum<NV>(da, lane, g, red);
 #pragma unroll
-          for (int j = 0; j < NV; ++j) {
-            const float xs = sc[j] + st[j];
-            const float score = rgat_leaky(xs);
-            const float lp = xs > 0.f ? 1.f : kLeakyReluAlpha;
-            if (score > m[j]) {   // as rgat_warp_kernel: this edge weighs 1, the sums so far are rescaled
-              const float r = expf(m[j] - score);
-              m[j] = score;
-              den[j] = fmaf(den[j], r, 1.0f);
-              if (PRE) {
-                acc[j].x = fmaf(acc[j].x, r, x[j].x); acc[j].y = fmaf(acc[j].y, r, x[j].y);
-                acc[j].z = fmaf(acc[j].z, r, x[j].z); acc[j].w = fmaf(acc[j].w, r, x[j].w);
+          for (int i = 0; i < EB; ++i) {
+            if (e0 + i >= n) break;
+            float da[NV];
+            if (STATS) {
+#pragma unroll
+              for (int j = 0; j < NV; ++j) da[j] = dot4(z[j], x[i][j]);
+              rgat_head_sum<NV>(da, lane, g, red);
+            }
+#pragma unroll
+            for (int j = 0; j < NV; ++j) {
+              const float xs = sc[i][j] + st[j];
+              const float score = rgat_leaky(xs);
+              const float lp = xs > 0.f ? 1.f : kLeakyReluAlpha;
+              const float4 xe = x[i][j];
+              if (score > m[j]) {   // this edge weighs exp(0) = 1, the sums so far are rescaled (the first edge: by 0)
+                const float r = expf(m[j] - score);
+                m[j] = score;
+                den[j] = fmaf(den[j], r, 1.0f);
+                if (STATS) {
+                  G[j] = fmaf(G[j], r, da[j]);
+                  A1[j] = fmaf(A1[j], r, lp * da[j]);
+                  A2[j] = fmaf(A2[j], r, lp);
+                } else {
+                  acc[j].x = fmaf(acc[j].x, r, xe.x); acc[j].y = fmaf(acc[j].y, r, xe.y);
+                  acc[j].z = fmaf(acc[j].z, r, xe.z); acc[j].w = fmaf(acc[j].w, r, xe.w);
+                }
               } else {
-                G[j] = fmaf(G[j], r, da[j]);
-                A1[j] = fmaf(A1[j], r, lp * da[j]);
-                A2[j] = fmaf(A2[j], r, lp);
-              }
-            } else {
-              const float wt = expf(score - m[j]);
-              den[j] += wt;
-              if (PRE) {
-                acc[j].x = fmaf(wt, x[j].x, acc[j].x); acc[j].y = fmaf(wt, x[j].y, acc[j].y);
-                acc[j].z = fmaf(wt, x[j].z, acc[j].z); acc[j].w = fmaf(wt, x[j].w, acc[j].w);
-              } else {
-                G[j] = fmaf(wt, da[j], G[j]);
-                A1[j] = fmaf(wt, lp * da[j], A1[j]);
-                A2[j] = fmaf(wt, lp, A2[j]);
+                const float wt = expf(score - m[j]);
+                den[j] += wt;
+                if (STATS) {
+                  G[j] = fmaf(wt, da[j], G[j]);
+                  A1[j] = fmaf(wt, lp * da[j], A1[j]);
+                  A2[j] = fmaf(wt, lp, A2[j]);
+                } else {
+                  acc[j].x = fmaf(wt, xe.x, acc[j].x); acc[j].y = fmaf(wt, xe.y, acc[j].y);
+                  acc[j].z = fmaf(wt, xe.z, acc[j].z); acc[j].w = fmaf(wt, xe.w, acc[j].w);
+                }
               }
             }
           }
         }
       }
-      if (!PRE) {
+      if (STATS) {
 #pragma unroll
         for (int j = 0; j < NV; ++j)
           if (lead[j]) {
@@ -454,17 +249,18 @@ __global__ void __launch_bounds__(256) rgat_bwd_target_kernel(const RgatBwdParam
           }
       }
     }
-    if (PRE) {
+    if (!STATS) {
 #pragma unroll
       for (int j = 0; j < NV; ++j) {
         if (!ok[j]) continue;
         if (!hub) {
           const float inv = den[j] > 0.f ? 1.0f / den[j] : 0.f;
-          *reinterpret_cast<float4*>(p.pre + v * p.H + 4 * q[j]) =
-              make_float4(acc[j].x * inv, acc[j].y * inv, acc[j].z * inv, acc[j].w * inv);
+          float o[4] = {acc[j].x * inv, acc[j].y * inv, acc[j].z * inv, acc[j].w * inv};
+          apply_act_vec<4>(o, p.act);
+          *reinterpret_cast<float4*>(p.out + v * p.H + 4 * q[j]) = make_float4(o[0], o[1], o[2], o[3]);
         } else {
           *reinterpret_cast<float4*>(p.ha1 + row * p.H + 4 * q[j]) = acc[j];
-          if (lead[j]) {
+          if (lead[j]) {   // every column block holding the head computes the same m_c, den_c bits
             p.hstat[row * K3 + k[j]] = m[j];
             p.hstat[row * K3 + p.K + k[j]] = den[j];
           }
@@ -497,9 +293,9 @@ __global__ void __launch_bounds__(256) rgat_bwd_target_kernel(const RgatBwdParam
   }
 }
 
-// The chunks of every hub combined in chunk order: stat and ds_tgt (or the pre-activation) of the hub's row.
-template <bool PRE>
-__global__ void rgat_bwd_hub_combine_kernel(const RgatBwdParams p) {
+// The chunks of every hub combined in chunk order: act(o) of the hub's row (output mode) or its stat and ds_tgt.
+template <bool STATS>
+__global__ void rgat_hub_combine_kernel(const RgatWalkParams p) {
   const int count = *p.item_count;
   const long long LK = (long long)p.L * p.K;
   const int K3 = 3 * p.K;
@@ -510,7 +306,7 @@ __global__ void rgat_bwd_hub_combine_kernel(const RgatBwdParams p) {
     int deg = 0;
     for (int l = 0; l < p.L; ++l) deg += p.row_ptr[(long long)l * p.V + v + 1] - p.row_ptr[(long long)l * p.V + v];
     const int nch = (deg + kHubChunk - 1) / kHubChunk;
-    if (PRE) {
+    if (!STATS) {
       for (int c = threadIdx.x; c < p.H; c += blockDim.x) {
         const int k = c / p.d;
         float m = kLowestFloat;
@@ -521,7 +317,9 @@ __global__ void rgat_bwd_hub_combine_kernel(const RgatBwdParams p) {
           den = fmaf(p.hstat[(it + i) * K3 + p.K + k], s, den);
           acc = fmaf(p.ha1[(long long)(it + i) * p.H + c], s, acc);
         }
-        p.pre[v * p.H + c] = den > 0.f ? acc * (1.0f / den) : 0.f;
+        float o[1] = {den > 0.f ? acc * (1.0f / den) : 0.f};
+        apply_act_vec<1>(o, p.act);
+        p.out[v * p.H + c] = o[0];
       }
       continue;
     }
@@ -680,28 +478,27 @@ static int rgat_bwd_blocks(long long warps) {
   return g < 1 ? 1 : (g > 132 * 64 ? 132 * 64 : (int)g);
 }
 
-int launch_rgat_target_pass(tfgnn_batch* b, const float* P, const float* s_src, const float* s_tgt, int K, int d,
-                            const float* dz, float* stat, float* ds_tgt, float* pre, cudaStream_t st) {
-  const bool pre_walk = dz == nullptr;
-  TFGNN_REQUIRE(pre_walk ? pre != nullptr : (stat && ds_tgt), "rgat target pass: NULL pointer");
-  RgatBwdParams p{};
-  p.P = P; p.s_src = s_src; p.s_tgt = s_tgt; p.row_ptr = b->row_ptr; p.src = b->src_sorted;
-  p.V = b->V; p.tgt_off = b->tgt_off; p.L = b->L; p.K = K; p.d = d; p.H = K * d;
-  p.dz = dz; p.stat = stat; p.a1 = ds_tgt; p.pre = pre;
-  const long long LK = (long long)p.L * K;
+// One target walk over the batch (rgat_warp_kernel) and the chunk-order combine of its hub partials; p.dz NULL: output mode.
+static int rgat_target_walk(tfgnn_batch* b, RgatWalkParams& p, cudaStream_t st) {
+  const bool stats = p.dz != nullptr;
+  p.row_ptr = b->row_ptr; p.src = b->src_sorted;
+  p.V = b->V; p.tgt_off = b->tgt_off; p.L = b->L; p.H = p.K * p.d;
+  const long long LK = (long long)p.L * p.K;
+  // a hub has more than kHubThreshold edges and at most deg / kHubChunk + 1 chunks
   const long long max_items = b->M_in / kHubChunk + b->M_in / kHubThreshold + 2;
-  PoolBuffer items{st}, flush{st}, hub{st};
+  PoolBuffer items{st}, hub{st}, flush{st};
   int rc = items.alloc((size_t)max_items * sizeof(int2) + 16);
   if (rc) return rc;
-  // per hub chunk: m_c, den_c, G_c and A1_c, A2_c, their maximum (pre-activation walk: m_c, den_c and an [H] row)
-  const size_t hub_row = pre_walk ? (size_t)p.H : (size_t)3 * LK;
-  rc = hub.alloc((size_t)max_items * (3 * K + hub_row) * sizeof(float));
+  // per hub chunk: A1_c, A2_c and their maximum (output mode: the [H] row acc_c, stored as float4: so the rows come first),
+  // then m_c, den_c, G_c
+  const size_t hub_row = stats ? (size_t)3 * LK : (size_t)p.H;
+  rc = hub.alloc((size_t)max_items * (hub_row + 3 * p.K) * sizeof(float));
   if (rc) return rc;
-  p.hstat = hub.f();
-  p.ha1 = hub.f() + (size_t)max_items * 3 * K;
-  p.ha2 = p.ha1 + (size_t)max_items * LK;
-  p.hml = p.ha2 + (size_t)max_items * LK;
-  if (!pre_walk) {
+  p.ha1 = hub.f();
+  p.hstat = hub.f() + (size_t)max_items * hub_row;
+  if (stats) {
+    p.ha2 = p.ha1 + (size_t)max_items * LK;
+    p.hml = p.ha2 + (size_t)max_items * LK;
     rc = flush.alloc((size_t)2 * p.V * LK * sizeof(float));
     if (rc) return rc;
     p.a2 = flush.f();
@@ -710,28 +507,44 @@ int launch_rgat_target_pass(tfgnn_batch* b, const float* P, const float* s_src, 
   p.item_count = (int*)items.p;
   p.items = reinterpret_cast<const int2*>(reinterpret_cast<char*>(items.p) + 16);
   TFGNN_CUDA(cudaMemsetAsync(items.p, 0, sizeof(int), st));
-  rgat_bwd_hub_scan_kernel<<<grid_for(p.V), 256, 0, st>>>(p.row_ptr, p.V, p.L, const_cast<int2*>(p.items),
-                                                         const_cast<int*>(p.item_count));
+  rgat_hub_scan_kernel<<<grid_for(p.V), 256, 0, st>>>(p.row_ptr, p.V, p.L, const_cast<int2*>(p.items),
+                                                     const_cast<int*>(p.item_count));
   TFGNN_LAUNCH_CHECK();
-  const int blocks = rgat_bwd_blocks(p.V + max_items);
-#define TFGNN_RGAT_TGT(NV)                                                                   \
-  do {                                                                                       \
-    if (pre_walk) rgat_bwd_target_kernel<NV, true><<<blocks, 256, 0, st>>>(p);               \
-    else rgat_bwd_target_kernel<NV, false><<<blocks, 256, 0, st>>>(p);                       \
-  } while (0)
-  switch ((p.H + 127) / 128) {
-    case 1: TFGNN_RGAT_TGT(1); break;
-    case 2: TFGNN_RGAT_TGT(2); break;
-    case 3: TFGNN_RGAT_TGT(3); break;
-    case 4: TFGNN_RGAT_TGT(4); break;
-    default: return unsupported("rgat_bwd: hidden_dim above 512 is not built");
+  if (stats) {
+    const int blocks = rgat_bwd_blocks(p.V + max_items);
+    switch ((p.H + 127) / 128) {
+      case 1: rgat_warp_kernel<1, true><<<blocks, 256, 0, st>>>(p); break;
+      case 2: rgat_warp_kernel<2, true><<<blocks, 256, 0, st>>>(p); break;
+      case 3: rgat_warp_kernel<3, true><<<blocks, 256, 0, st>>>(p); break;
+      case 4: rgat_warp_kernel<4, true><<<blocks, 256, 0, st>>>(p); break;
+      default: return unsupported("rgat_bwd: hidden_dim above 512 is not built");
+    }
+    TFGNN_LAUNCH_CHECK();
+    rgat_hub_combine_kernel<true><<<132, 128, 0, st>>>(p);
+  } else {
+    // one warp per (work item, 128-column block)
+    const dim3 grid((unsigned)ceil_div((p.V + max_items) * 32, 256), (unsigned)ceil_div(p.H, 128));
+    rgat_warp_kernel<1, false><<<grid, 256, 0, st>>>(p);
+    TFGNN_LAUNCH_CHECK();
+    rgat_hub_combine_kernel<false><<<132, 128, 0, st>>>(p);
   }
-#undef TFGNN_RGAT_TGT
-  TFGNN_LAUNCH_CHECK();
-  if (pre_walk) rgat_bwd_hub_combine_kernel<true><<<132, 128, 0, st>>>(p);
-  else rgat_bwd_hub_combine_kernel<false><<<132, 128, 0, st>>>(p);
   TFGNN_LAUNCH_CHECK();
   return 0;
+}
+
+int launch_rgat_aggregate(tfgnn_batch* b, const float* P, const float* s_src, const float* s_tgt, int K, int d,
+                          int activation, float* out, cudaStream_t st) {
+  RgatWalkParams p{};
+  p.P = P; p.s_src = s_src; p.s_tgt = s_tgt; p.K = K; p.d = d; p.act = activation; p.out = out;
+  return rgat_target_walk(b, p, st);
+}
+
+int launch_rgat_target_pass(tfgnn_batch* b, const float* P, const float* s_src, const float* s_tgt, int K, int d,
+                            const float* dz, float* stat, float* ds_tgt, cudaStream_t st) {
+  TFGNN_REQUIRE(dz && stat && ds_tgt, "rgat target pass: NULL pointer");
+  RgatWalkParams p{};
+  p.P = P; p.s_src = s_src; p.s_tgt = s_tgt; p.K = K; p.d = d; p.dz = dz; p.stat = stat; p.a1 = ds_tgt;
+  return rgat_target_walk(b, p, st);
 }
 
 int launch_rgat_source_pass(const tfgnn_batch* b, const tfgnn_batch* bt, const float* P, const float* s_src,

@@ -342,18 +342,16 @@ __device__ __forceinline__ float leaky(float x) { return x > 0.f ? x : kLeakyRel
 // One thread per (target v, output column c): segment softmax over ALL incoming edges of v (all
 // types jointly, rgat.py:135-151) for head k = c/d, then the weighted sum of P_l[src, c].
 // Two passes over the node's CSR segments: running max, then exp-sum and weighted accumulate.
-// VEC: 4 columns per thread (needs d % 4 == 0).
-template <bool VEC>
+// The path of the shapes the target walk (rgat.cu) does not take: d % 4 != 0, L == 0 or an unaligned out.
 __global__ void rgat_aggregate_kernel(const float* __restrict__ P, const float* __restrict__ s_src,
                                       const float* __restrict__ s_tgt, const int* __restrict__ row_ptr,
                                       const int* __restrict__ src, long long V, long long tgt_off, int L, int K,
                                       int d, int act, float* __restrict__ out) {
   const int H = K * d;
-  const int cols = VEC ? H / 4 : H;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= V * cols) return;
-  const long long v = idx / cols;
-  const int c = (int)(idx % cols) * (VEC ? 4 : 1);
+  if (idx >= V * H) return;
+  const long long v = idx / H;
+  const int c = (int)(idx % H);
   const int k = c / d;
   const long long LK = (long long)L * K, LH = (long long)L * H;
   float m = kLowestFloat;
@@ -364,8 +362,7 @@ __global__ void rgat_aggregate_kernel(const float* __restrict__ P, const float* 
     for (int e = beg; e < end; ++e)
       m = fmaxf(m, leaky(__ldg(s_src + (long long)__ldg(src + e) * LK + l * K + k) + st));
   }
-  float den = 0.f;
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  float den = 0.f, acc = 0.f;
   for (int l = 0; l < L; ++l) {
     const long long seg = (long long)l * V + v;
     const int beg = __ldg(row_ptr + seg), end = __ldg(row_ptr + seg + 1);
@@ -374,24 +371,11 @@ __global__ void rgat_aggregate_kernel(const float* __restrict__ P, const float* 
       const long long u = __ldg(src + e);
       const float w = expf(leaky(__ldg(s_src + u * LK + l * K + k) + st) - m);
       den += w;
-      const float* prow = P + u * LH + (long long)l * H + c;
-      if (VEC) {
-        const float4 x = ldg_f4(prow);
-        acc.x = fmaf(w, x.x, acc.x); acc.y = fmaf(w, x.y, acc.y);
-        acc.z = fmaf(w, x.z, acc.z); acc.w = fmaf(w, x.w, acc.w);
-      } else {
-        acc.x = fmaf(w, __ldg(prow), acc.x);
-      }
+      acc = fmaf(w, __ldg(P + u * LH + (long long)l * H + c), acc);
     }
   }
   const float inv = den > 0.f ? 1.0f / den : 0.f;
-  float* o = out + v * H + c;
-  if (VEC) {
-    *reinterpret_cast<float4*>(o) = make_float4(apply_act(acc.x * inv, act), apply_act(acc.y * inv, act),
-                                                apply_act(acc.z * inv, act), apply_act(acc.w * inv, act));
-  } else {
-    o[0] = apply_act(acc.x * inv, act);
-  }
+  out[v * H + c] = apply_act(acc * inv, act);
 }
 
 // P_l = h W_l for every one of the Vs nodes and the score halves s_src, s_tgt [Vs, L*K], into the caller's buffers.  The
@@ -460,7 +444,7 @@ extern "C" int tfgnn_b200_rgat_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   const bool vec = (d % 4 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) && L > 0;
   if (vec) return launch_rgat_aggregate(b, P.f(), ss.f(), stt.f(), K, d, activation, out, st);
   const long long threads = V * H;
-  rgat_aggregate_kernel<false><<<ceil_div(threads, 128), 128, 0, st>>>(
+  rgat_aggregate_kernel<<<ceil_div(threads, 128), 128, 0, st>>>(
       P.f(), ss.f(), stt.f(), b->row_ptr, b->src_sorted, V, b->tgt_off, L, K, d, activation, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
