@@ -18,8 +18,10 @@
  *   - The output of a layer call must not overlap its node-state input (every target gathers arbitrary
  *     source rows); entries that work in place say so.
  *   - All work is enqueued on `stream` (a cudaStream_t passed as void*; NULL = legacy default
- *     stream).  No entry point synchronises the device except tfgnn_b200_prepare with
- *     TFGNN_PREPARE_VALIDATE and tfgnn_b200_free_batch.
+ *     stream).  No entry point synchronises the device; tfgnn_b200_prepare with
+ *     TFGNN_PREPARE_VALIDATE (and tfgnn_b200_graph_offsets with validate != 0) synchronise
+ *     their stream.  tfgnn_b200_free_batch returns the batch's CSR to the pool stream-ordered,
+ *     behind the work of the last stream the batch was used on.
  *   - Return value 0 = success; otherwise a TFGNN_ERR_* code and tfgnn_b200_last_error()
  *     (thread-local) describes it.  There is NO CPU fallback anywhere in this library.
  */
@@ -119,7 +121,8 @@ TFGNN_API int tfgnn_b200_batch_info(const tfgnn_batch_t* batch, int64_t* num_nod
                           const int32_t** src_sorted);
 
 /* Copy the CSR into caller-owned device buffers (row_ptr_out int32[L*V+1], src_sorted_out
- * int32[num_edges_total]); either may be NULL. */
+ * int32[num_edges_total]); either may be NULL.  Like tfgnn_b200_in_degree and every layer call,
+ * this moves the batch to `stream` (see "Threading" below). */
 TFGNN_API int tfgnn_b200_batch_export_csr(const tfgnn_batch_t* batch, int32_t* row_ptr_out,
                                 int32_t* src_sorted_out, void* stream);
 
@@ -499,7 +502,11 @@ TFGNN_API int tfgnn_b200_assemble_batch(const int64_t* node_offsets, const int64
  * tfgnn_b200_release_device_state() restores the saved L2 limit on every device and trims the pool; the Python
  * shim registers it with atexit.
  * Threading: entry points are re-entrant; ONE tfgnn_batch_t must not be used by two host threads or on two
- * streams at the same time (it may move to another stream between calls: the library orders the streams). */
+ * streams at the same time (it may move to another stream between calls: the library orders the streams).  Every
+ * call that takes a batch orders it: tfgnn_b200_prepare*, the layer forwards and backwards, tfgnn_b200_in_degree and
+ * tfgnn_b200_batch_export_csr make their stream wait for the work of the stream the batch was last used on, and
+ * tfgnn_b200_free_batch frees behind that last stream.  tfgnn_b200_batch_info enqueues nothing: a caller that reads
+ * the pointers it returns orders its stream itself. */
 TFGNN_API int tfgnn_b200_set_l2_persist_mb(int32_t megabytes);
 TFGNN_API int tfgnn_b200_release_device_state(void);
 

@@ -198,20 +198,29 @@ def test_rgcn_parity(V, D, H, L, E, opts, path):
 
 @pytest.mark.parametrize("chunk_rows,V", [(256, 3000), (128, 1000), (None, 160000)])
 def test_rgcn_pipelined_two_stream(chunk_rows, V, monkeypatch):
-    """gather || tensor-core-GEMM pipeline over node chunks (triple-buffered) == oracle."""
+    """gather || tensor-core-GEMM pipeline over node chunks (triple-buffered) == oracle.  D = 36 (D % 4 == 0, D % 32 != 0):
+    the fused kernel refuses the shape, so `auto` takes the pipeline, which makes one gather and one GEMM launch per chunk
+    more than the one-shot path."""
+    from tf2_gnn_b200 import _ffi
     _need_gpu()
+    rows = chunk_rows if chunk_rows is not None else 2 * 132 * 128
     if chunk_rows is not None:
         monkeypatch.setenv("TFGNN_B200_PIPE_CHUNK_ROWS", str(chunk_rows))
     rng = np.random.default_rng(V)
-    D = H = 64
+    D, H = 36, 64
     L = 3
     adjs = random_graph(rng, V, L, V * 3, hub=True, self_loops=True)
     p = mo.default_hyperparameters("rgcn")
     p.update(hidden_dim=H, aggregation_function="mean", message_activation_function="tanh")
+    n0 = _ffi.launch_count()
     a = run_case("rgcn", p, V, D, L, adjs, seed=2, path="auto")
+    n1 = _ffi.launch_count()
     monkeypatch.setenv("TFGNN_B200_PIPE_CHUNK_ROWS", str(1 << 24))   # disables the pipeline
     b = run_case("rgcn", p, V, D, L, adjs, seed=2, path="sorted_tc")
+    n2 = _ffi.launch_count()
     assert_states_close(a.cpu().numpy(), b.cpu().numpy().astype(np.float64), tol=1e-6)
+    chunks = -(-V // rows)
+    assert (n1 - n0) - (n2 - n1) >= 2 * (chunks - 1), f"{n1 - n0} vs {n2 - n1} launches: the pipeline did not run"
 
 
 @pytest.mark.parametrize("V,D,H,L,E,opts,agg", [

@@ -436,6 +436,10 @@ extern "C" int tfgnn_b200_batch_export_csr(const tfgnn_batch_t* b, int32_t* row_
                                            void* stream) {
   TFGNN_REQUIRE(b != nullptr, "batch is NULL");
   cudaStream_t st = (cudaStream_t)stream;
+  // a read of the CSR enters the batch like a layer call: it waits for the prepare on another stream, and the free
+  // (on the last stream entered) waits for it.  The stream fields are bookkeeping, not the batch's contents.
+  const int rc = batch_enter(const_cast<tfgnn_batch*>(b), st);
+  if (rc) return rc;
   const long long S = (long long)b->L * b->V;
   if (row_ptr_out)
     TFGNN_CUDA(cudaMemcpyAsync(row_ptr_out, b->row_ptr, (size_t)(S + 1) * sizeof(int), cudaMemcpyDeviceToDevice, st));
@@ -449,6 +453,8 @@ extern "C" int tfgnn_b200_in_degree(const tfgnn_batch_t* b, float* out, void* st
   const long long S = (long long)b->L * b->V;
   if (S == 0) return 0;
   TFGNN_REQUIRE(out != nullptr, "out is NULL");
+  const int rc = batch_enter(const_cast<tfgnn_batch*>(b), (cudaStream_t)stream);   // as in tfgnn_b200_batch_export_csr
+  if (rc) return rc;
   int blocks = ceil_div(S, 256);
   if (blocks > 132 * 32) blocks = 132 * 32;
   in_degree_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(b->row_ptr, S, out);
