@@ -223,9 +223,11 @@ TFGNN_API int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* batch, const float* h, int32_t 
 
 /* Backward of tfgnn_b200_ggnn_fwd (SURVEY.md section 8f-1; the reference differentiates through GGNN with
  * tf.GradientTape, models/graph_task_model.py:338-365).  Recomputes the forward intermediates from h; batch_t is
- * the TFGNN_PREPARE_TRANSPOSE batch of the same adjacency lists.  Writes grad_h [V,H], grad_W[l] [H,H],
- * grad_gru_kernel [H,3H], grad_gru_recurrent_kernel [H,3H], grad_gru_bias [2,3H].
- * Supported: 0 hidden layers in the message MLPs, source state only, sum / mean / sqrt_n aggregation, H % 4 == 0.
+ * the TFGNN_PREPARE_TRANSPOSE batch of the same adjacency lists.  Writes grad_h [V,H], grad_W[l] [H,H] ([2H,H] with
+ * TFGNN_FLAG_USE_TARGET_STATE), grad_gru_kernel [H,3H], grad_gru_recurrent_kernel [H,3H], grad_gru_bias [2,3H].
+ * Supported: 0 hidden layers in the message MLPs, source-only or source+target state input, sum / mean / sqrt_n / max
+ * aggregation (max up to H = 512), H % 4 == 0.  Other message MLPs compose tfgnn_b200_edge_mlp_fwd / its backward with
+ * tfgnn_b200_gru_update_fwd / tfgnn_b200_gru_update_bwd.
  * On a target-range shard the pair (batch, batch_t) is as for tfgnn_b200_rgcn_bwd: h is the full [num_nodes_total, H]
  * table, grad_out has hi-lo rows, the GRU reads its state from rows [lo, hi) of h, and the call writes this shard's
  * contribution to grad_h [num_nodes_total, H] (GRU direct and recurrent terms on rows [lo, hi)), to grad_W and to the GRU
@@ -235,6 +237,24 @@ TFGNN_API int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, 
                         const float* gru_kernel, const float* gru_recurrent_kernel, const float* gru_bias,
                         const float* grad_out, float* grad_h, float* const* grad_W, float* grad_gru_kernel,
                         float* grad_gru_recurrent_kernel, float* grad_gru_bias, void* stream);
+
+/* GGNN's node update on its own (ggnn.py:84-87): out = GRUCell(agg, h), Keras reset_after=True, over num_rows rows.
+ * agg [num_rows,H] (the aggregated messages), h [num_rows,H] (the state rows; on a target-range shard rows [lo, hi) of the full
+ * table), gru_kernel / gru_recurrent_kernel [H,3H], gru_bias [2,3H]; out [num_rows,H] may overlap h (an in-place update).
+ * tfgnn_b200_ggnn_fwd runs exactly this after its aggregation, so the same agg gives the same bits.  path as for the layer
+ * entries (TFGNN_PATH_ATOMIC: TFGNN_ERR_UNSUPPORTED). */
+TFGNN_API int tfgnn_b200_gru_update_fwd(const float* agg, const float* h, int64_t num_rows, int32_t H,
+                                        const float* gru_kernel, const float* gru_recurrent_kernel, const float* gru_bias,
+                                        int32_t path, float* out, void* stream);
+
+/* Backward of tfgnn_b200_gru_update_fwd from the given agg (tfgnn_b200_ggnn_bwd runs the same steps): writes grad_agg
+ * [num_rows,H], grad_h [num_rows,H] (the direct path through z * h plus the recurrent path through h U), grad_gru_kernel
+ * [H,3H], grad_gru_recurrent_kernel [H,3H], grad_gru_bias [2,3H].  No atomics: run-to-run reproducible.  num_rows == 0
+ * writes zero weight gradients.  H % 4 != 0: TFGNN_ERR_UNSUPPORTED. */
+TFGNN_API int tfgnn_b200_gru_update_bwd(const float* agg, const float* h, int64_t num_rows, int32_t H,
+                                        const float* gru_kernel, const float* gru_recurrent_kernel, const float* gru_bias,
+                                        const float* grad_out, float* grad_agg, float* grad_h, float* grad_gru_kernel,
+                                        float* grad_gru_recurrent_kernel, float* grad_gru_bias, void* stream);
 
 /* RGIN (rgin.py:88-106): edge MLP messages, aggregation, optional aggregation MLP
  * (aggr_weights: host array of num_aggr_layers device pointers [H,H], may be NULL/0), activation. */

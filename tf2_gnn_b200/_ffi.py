@@ -46,6 +46,7 @@ EXPORTED_SYMBOLS = (
     "tfgnn_b200_gru_gate_bwd", "tfgnn_b200_rgcn_ln_fwd", "tfgnn_b200_film_bwd",
     "tfgnn_b200_edge_mlp_bwd", "tfgnn_b200_rgat_bwd",
     "tfgnn_b200_segment_sum_rows", "tfgnn_b200_readout_bwd", "tfgnn_b200_gru_gate_bwd_indexed",
+    "tfgnn_b200_gru_update_fwd", "tfgnn_b200_gru_update_bwd",
 )
 
 _PP = POINTER(c_void_p)
@@ -107,6 +108,10 @@ def lib() -> ctypes.CDLL:
     L.tfgnn_b200_ggnn_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, _PP, c_int32, c_uint32, c_int32,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, _PP, c_void_p, c_void_p,
                                       c_void_p, c_void_p]
+    L.tfgnn_b200_gru_update_fwd.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_int32,
+                                            c_void_p, c_void_p]
+    L.tfgnn_b200_gru_update_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.tfgnn_b200_process_adjacency_sizes.argtypes = [POINTER(c_int64), c_int32, c_int64, c_int32, POINTER(c_int32),
                                                      c_int32, POINTER(c_int64), POINTER(c_int32)]
     L.tfgnn_b200_process_adjacency.argtypes = [_PP, POINTER(c_int64), c_int32, c_int64, c_int32, POINTER(c_int32),

@@ -587,11 +587,62 @@ extern "C" int tfgnn_b200_rgcn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   return 0;
 }
 
+namespace tfgnn {
+
+// Backward of the GRU update out = GRUCell(agg, h) over V rows (gru_update), from the given agg:
+//   1. gx = agg K + b0, gh = h U + b1 (tensor-core GEMMs);  2. gate backward in place -> dgx, dgh, dh_direct;
+//   3. db = column sums;  4. dK = agg^T dgx, dU = h^T dgh (TN GEMM, fixed-order partials);
+//   5. dagg = dgx K^T, dh_rec = dgh U^T (tensor-core GEMMs).
+// dh_rec == nullptr: the recurrent term is added onto dh_direct instead.  Every temporary is freed on return.
+static int gru_update_bwd(const float* agg, const float* h, int ldh, const float* gru_kernel,
+                          const float* gru_recurrent_kernel, const float* gru_bias, const float* grad_out, long long V, int H,
+                          float* dagg, float* dh_direct, float* dh_rec, float* grad_gru_kernel,
+                          float* grad_gru_recurrent_kernel, float* grad_gru_bias, cudaStream_t st) {
+  const int N3 = 3 * H;
+  PoolBuffer gx{st}, gh{st}, wT{st}, part{st};
+  int rc = gx.alloc((size_t)V * N3 * sizeof(float));
+  if (!rc) rc = gh.alloc((size_t)V * N3 * sizeof(float));
+  if (!rc) rc = wT.alloc((size_t)N3 * H * sizeof(float));
+  if (!rc) rc = part.alloc((tn_partial_floats(V, H, N3) + (size_t)tn_chunks(V) * N3) * sizeof(float));
+  if (rc) return rc;
+  // 1. forward quantities gx, gh
+  GemmEpilogue e0, e1;
+  e0.bias = gru_bias;
+  e1.bias = gru_bias + N3;
+  rc = node_gemm(agg, H, gru_kernel, N3, gx.f(), N3, V, N3, H, e0, TFGNN_PATH_AUTO, st);
+  if (rc) return rc;
+  rc = node_gemm(h, ldh, gru_recurrent_kernel, N3, gh.f(), N3, V, N3, H, e1, TFGNN_PATH_AUTO, st);
+  if (rc) return rc;
+  // 2. gates, in place
+  gru_gate_bwd_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), nullptr, gh.f(), h, ldh, grad_out, V, H, gx.f(), gh.f(),
+                                                       dh_direct);
+  TFGNN_LAUNCH_CHECK();
+  // 3. bias gradients: rows 0 / 1 of gru_bias belong to gx / gh
+  float* cpart = part.f() + tn_partial_floats(V, H, N3);
+  rc = column_sums(gx.f(), V, N3, grad_gru_bias, cpart, st);
+  if (rc) return rc;
+  rc = column_sums(gh.f(), V, N3, grad_gru_bias + N3, cpart, st);
+  if (rc) return rc;
+  // 4. dK = agg^T dgx, dU = h^T dgh
+  rc = weight_grad(agg, H, gx.f(), N3, V, H, N3, part.f(), one_table(grad_gru_kernel), 1, H, 0, st);
+  if (rc) return rc;
+  rc = weight_grad(h, ldh, gh.f(), N3, V, H, N3, part.f(), one_table(grad_gru_recurrent_kernel), 1, H, 0, st);
+  if (rc) return rc;
+  // 5. dagg = dgx K^T, dh_rec = dgh U^T
+  rc = gemm_transposed(gx.f(), N3, {one_table(gru_kernel), 1, H, N3}, wT.f(), dagg, H, V, H, GemmEpilogue{}, st);
+  if (rc) return rc;
+  GemmEpilogue rec;
+  rec.accumulate = dh_rec == nullptr;
+  return gemm_transposed(gh.f(), N3, {one_table(gru_recurrent_kernel), 1, H, N3}, wT.f(), dh_rec ? dh_rec : dh_direct, H, V,
+                         H, rec, st);
+}
+
+}  // namespace tfgnn
+
 // GGNN backward (SURVEY.md section 8f-1): gradient of tfgnn_b200_ggnn_fwd w.r.t. the node states, the per-type message
 // weights and the GRU parameters.  Everything is recomputed from h (nothing but h is saved by the forward pass):
-//   agg = sum_l s A_l W_l (forward kernel), gx = agg K + b0, gh = h U + b1 (tensor-core GEMMs),
-//   gate backward in place -> dgx, dgh, dh_direct;  db = column sums;  dK = agg^T dgx, dU = h^T dgh (TN GEMM, fixed-order
-//   partials);  dagg = dgx K^T, dh_rec = dgh U^T (tensor-core GEMMs);  messages: tfgnn_b200_rgcn_bwd with dagg.
+//   agg = sum_l s A_l W_l (forward kernel), then the GRU update's backward (gru_update_bwd) -> dagg, dh_direct, dh_rec and
+//   the GRU gradients;  messages: tfgnn_b200_rgcn_bwd with dagg.
 extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int32_t D,
                                    const float* const* W, int32_t H, uint32_t flags, int32_t aggregation,
                                    const float* gru_kernel, const float* gru_recurrent_kernel, const float* gru_bias,
@@ -604,7 +655,7 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
   if (int rc = check_backward_pair(b, bt)) return rc;
-  if (flags & TFGNN_FLAG_USE_TARGET_STATE) return unsupported("ggnn_bwd: target-state input is not built yet");
+  const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // W_l is then [2D, H], as for tfgnn_b200_rgcn_bwd
   if (H % 4 != 0) return unsupported("ggnn_bwd needs hidden_dim to be a multiple of 4");
   if (aggregation == TFGNN_AGG_MAX && H > 512)
     return unsupported("ggnn_bwd: max aggregation above hidden_dim 512 is not built");
@@ -617,12 +668,10 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     return zero_contribution({{&grad_gru_kernel, 1, (size_t)H * N3},
                               {&grad_gru_recurrent_kernel, 1, (size_t)H * N3},
                               {&grad_gru_bias, 1, (size_t)2 * N3},
-                              {grad_W, L, (size_t)D * H}},
+                              {grad_W, L, (size_t)(use_target ? 2 * D : D) * H}},
                              grad_h, (size_t)Vs * D, st);
   TFGNN_REQUIRE(h && grad_out, "NULL pointer");
   TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
-  const float* h_tgt = h + (size_t)lo * D;
-  const int chunks = tn_chunks(V);
   int rc = enter_both(b, bt, st);
   if (rc) return rc;
   PoolBuffer dagg{st}, dhd{st}, tmp{st};
@@ -631,45 +680,15 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   if (!rc) rc = tmp.alloc((size_t)V * H * sizeof(float));
   if (rc) return rc;
   {
-    // the forward quantities and the GRU's own gradients are freed before the message backward below
-    PoolBuffer agg{st}, gx{st}, gh{st}, wT{st}, part{st};
+    // agg and the GRU's own temporaries are freed before the message backward below
+    PoolBuffer agg{st};
     rc = agg.alloc((size_t)V * H * sizeof(float));
-    if (!rc) rc = gx.alloc((size_t)V * N3 * sizeof(float));
-    if (!rc) rc = gh.alloc((size_t)V * N3 * sizeof(float));
-    if (!rc) rc = wT.alloc((size_t)N3 * H * sizeof(float));
-    if (!rc) rc = part.alloc((tn_partial_floats(V, H, N3) + (size_t)chunks * N3) * sizeof(float));
     if (rc) return rc;
-    // 1. forward quantities: agg (no message activation, ggnn.py:68-83), gx, gh
+    // agg: no message activation (ggnn.py:68-83)
     rc = edge_mlp_core(b, h, D, W, 0, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION, aggregation, TFGNN_ACT_NONE,
                        TFGNN_PATH_AUTO, agg.f(), H, st);
-    if (rc) return rc;
-    GemmEpilogue e0, e1;
-    e0.bias = gru_bias;
-    e1.bias = gru_bias + N3;
-    rc = node_gemm(agg.f(), H, gru_kernel, N3, gx.f(), N3, V, N3, H, e0, TFGNN_PATH_AUTO, st);
-    if (rc) return rc;
-    rc = node_gemm(h_tgt, D, gru_recurrent_kernel, N3, gh.f(), N3, V, N3, H, e1, TFGNN_PATH_AUTO, st);
-    if (rc) return rc;
-    // 2. gates, in place
-    gru_gate_bwd_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), nullptr, gh.f(), h_tgt, D, grad_out, V, H, gx.f(), gh.f(),
-                                                         dhd.f());
-    TFGNN_LAUNCH_CHECK();
-    // 3. bias gradients: rows 0 / 1 of gru_bias belong to gx / gh
-    float* cpart = part.f() + tn_partial_floats(V, H, N3);
-    rc = column_sums(gx.f(), V, N3, grad_gru_bias, cpart, st);
-    if (rc) return rc;
-    rc = column_sums(gh.f(), V, N3, grad_gru_bias + N3, cpart, st);
-    if (rc) return rc;
-    // 4. dK = agg^T dgx, dU = h^T dgh
-    rc = weight_grad(agg.f(), H, gx.f(), N3, V, H, N3, part.f(), one_table(grad_gru_kernel), 1, H, 0, st);
-    if (rc) return rc;
-    rc = weight_grad(h_tgt, D, gh.f(), N3, V, H, N3, part.f(), one_table(grad_gru_recurrent_kernel), 1, H, 0, st);
-    if (rc) return rc;
-    // 5. dagg = dgx K^T, dh_rec = dgh U^T
-    rc = gemm_transposed(gx.f(), N3, {one_table(gru_kernel), 1, H, N3}, wT.f(), dagg.f(), H, V, H, GemmEpilogue{}, st);
-    if (rc) return rc;
-    rc = gemm_transposed(gh.f(), N3, {one_table(gru_recurrent_kernel), 1, H, N3}, wT.f(), tmp.f(), H, V, H,
-                         GemmEpilogue{}, st);
+    if (!rc) rc = gru_update_bwd(agg.f(), h + (size_t)lo * D, D, gru_kernel, gru_recurrent_kernel, gru_bias, grad_out, V, H,
+                                 dagg.f(), dhd.f(), tmp.f(), grad_gru_kernel, grad_gru_recurrent_kernel, grad_gru_bias, st);
     if (rc) return rc;
   }
   // 6. messages: dagg -> grad_h (through the edges) and grad_W
@@ -680,6 +699,26 @@ extern "C" int tfgnn_b200_ggnn_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   add3_kernel<<<grid_for(V * H), 256, 0, st>>>(grad_h + (size_t)lo * D, dhd.f(), tmp.f(), V * H);
   TFGNN_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int tfgnn_b200_gru_update_bwd(const float* agg, const float* h, int64_t num_rows, int32_t H,
+                                         const float* gru_kernel, const float* gru_recurrent_kernel, const float* gru_bias,
+                                         const float* grad_out, float* grad_agg, float* grad_h, float* grad_gru_kernel,
+                                         float* grad_gru_recurrent_kernel, float* grad_gru_bias, void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && H > 0, "bad gru_update_bwd sizes");
+  if (H % 4 != 0) return unsupported("gru_update_bwd needs hidden_dim to be a multiple of 4");
+  TFGNN_REQUIRE(grad_gru_kernel && grad_gru_recurrent_kernel && grad_gru_bias, "GRU gradient pointer is NULL");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int N3 = 3 * H;
+  if (num_rows == 0)
+    return zero_contribution({{&grad_gru_kernel, 1, (size_t)H * N3},
+                              {&grad_gru_recurrent_kernel, 1, (size_t)H * N3},
+                              {&grad_gru_bias, 1, (size_t)2 * N3}},
+                             nullptr, 0, st);
+  TFGNN_REQUIRE(agg && h && grad_out && grad_agg && grad_h, "NULL pointer");
+  TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
+  return gru_update_bwd(agg, h, H, gru_kernel, gru_recurrent_kernel, gru_bias, grad_out, num_rows, H, grad_agg, grad_h,
+                        nullptr, grad_gru_kernel, grad_gru_recurrent_kernel, grad_gru_bias, st);
 }
 
 extern "C" int tfgnn_b200_gru_gate_bwd(const float* gx, const float* gh, const float* h, const float* grad_out,

@@ -16,6 +16,10 @@ int transform_aggregate_tables(tfgnn_batch* b, const float* h, int D, const PtrT
                                EdgeReduceParams* p, cudaStream_t st);
 int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                   uint32_t flags, int aggregation, int activation, int path, float* out, int ldo, cudaStream_t st);
+// GGNN's node update out = GRUCell(agg, h) over V rows (variants.cu): agg [V, H], state rows h [V, ldh], out [V, H];
+// in_place: out overlaps the caller's state table (the update then keeps the two GEMMs and the gate kernel)
+int gru_update(const float* agg, const float* h, int ldh, const float* gru_kernel, const float* gru_recurrent_kernel,
+               const float* gru_bias, long long V, int H, int path, bool in_place, float* out, cudaStream_t st);
 // literal per-edge path (literal.cu); FB = optional FiLM table [V, L*2H] (gamma | beta per type)
 int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                      uint32_t flags, int aggregation, int activation, const float* FB, int ldf, int path, float* out,

@@ -24,9 +24,56 @@ __global__ void gru_gate_kernel(const float* __restrict__ gx, const int* __restr
   }
 }
 
+int gru_update(const float* agg, const float* h, int ldh, const float* gru_kernel, const float* gru_recurrent_kernel,
+               const float* gru_bias, long long V, int H, int path, bool in_place, float* out, cudaStream_t st) {
+  {
+    // The GRU update as ONE tensor-core contraction over [agg | h] with the gate math in its epilogue: no [V,3H] tables.
+    // TFGNN_B200_GGNN_FUSED_GRU=0 keeps the two GEMMs + gate kernel (read per call: the tests compare the two).
+    const char* e = getenv("TFGNN_B200_GGNN_FUSED_GRU");
+    const bool want = !(e && atoi(e) == 0) &&
+                      (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
+    // the contraction reads whole rows of h for every 32-unit column tile while earlier tiles' epilogues already store new
+    // states: an in-place update (the gate kernel below tolerates it) must not take this form
+    if (want && !in_place && gemm_tc_gru_supported(V, H, agg, H, h, ldh, out, H)) {
+      PoolBuffer packed{st};
+      int rc = packed.alloc(gemm_tc_gru_packed_bytes(H));
+      if (rc) return rc;
+      return launch_gemm_tc_gru(agg, H, h, ldh, gru_kernel, gru_recurrent_kernel, gru_bias, packed.f(), out, H, V, H, st);
+    }
+  }
+  PoolBuffer gx{st}, gh{st};
+  int rc = gx.alloc((size_t)V * 3 * H * sizeof(float));
+  if (!rc) rc = gh.alloc((size_t)V * 3 * H * sizeof(float));
+  if (rc) return rc;
+  GemmEpilogue ex, eh;
+  ex.bias = gru_bias;
+  eh.bias = gru_bias + 3 * H;
+  rc = node_gemm(agg, H, gru_kernel, 3 * H, gx.f(), 3 * H, V, 3 * H, H, ex, path, st);
+  if (rc) return rc;
+  rc = node_gemm(h, ldh, gru_recurrent_kernel, 3 * H, gh.f(), 3 * H, V, 3 * H, H, eh, path, st);
+  if (rc) return rc;
+  gru_gate_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), nullptr, gh.f(), h, ldh, V, H, out);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace tfgnn
 
 using namespace tfgnn;
+
+extern "C" int tfgnn_b200_gru_update_fwd(const float* agg, const float* h, int64_t num_rows, int32_t H,
+                                         const float* gru_kernel, const float* gru_recurrent_kernel, const float* gru_bias,
+                                         int32_t path, float* out, void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && H > 0, "bad gru_update sizes");
+  TFGNN_REQUIRE(path >= TFGNN_PATH_AUTO && path <= TFGNN_PATH_FUSED_TC, "unknown path code");
+  if (path == TFGNN_PATH_ATOMIC) return unsupported("TFGNN_PATH_ATOMIC is not available for the GRU update");
+  if (num_rows == 0) return 0;
+  TFGNN_REQUIRE(agg && h && out, "NULL pointer");
+  TFGNN_REQUIRE(gru_kernel && gru_recurrent_kernel && gru_bias, "GRU weight pointer is NULL");
+  const bool in_place = out < h + (size_t)num_rows * H && h < out + (size_t)num_rows * H;   // out overlaps the state rows
+  return gru_update(agg, h, H, gru_kernel, gru_recurrent_kernel, gru_bias, num_rows, H, path, in_place, out,
+                    (cudaStream_t)stream);
+}
 
 extern "C" int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* b, const float* h, int32_t D, const float* const* mlp_weights,
                                    int32_t num_hidden_layers, int32_t H, uint32_t flags, int32_t aggregation,
@@ -47,39 +94,9 @@ extern "C" int tfgnn_b200_ggnn_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   rc = edge_mlp_core(b, h, D, mlp_weights, num_hidden_layers, H, flags & ~TFGNN_FLAG_ACT_BEFORE_AGGREGATION,
                      aggregation, TFGNN_ACT_NONE, path, agg.f(), H, st);
   if (rc) return rc;
-  {
-    // The GRU update as ONE tensor-core contraction over [agg | h] with the gate math in its epilogue: no [V,3H] tables.
-    // TFGNN_B200_GGNN_FUSED_GRU=0 keeps the two GEMMs + gate kernel (read per call: the tests compare the two).
-    const char* e = getenv("TFGNN_B200_GGNN_FUSED_GRU");
-    const bool want = !(e && atoi(e) == 0) &&
-                      (path == TFGNN_PATH_AUTO || path == TFGNN_PATH_SORTED_TC || path == TFGNN_PATH_FUSED_TC);
-    const float* h_tgt0 = h + (size_t)b->tgt_off * D;
-    // the contraction reads whole rows of h for every 32-unit column tile while earlier tiles' epilogues already store new
-    // states: an in-place update (out overlapping h; the gate kernel below tolerates it) must not take this form
-    const bool in_place = out < h + (size_t)b->V_src * D && h < out + (size_t)V * H;
-    if (want && !in_place && gemm_tc_gru_supported(V, H, agg.f(), H, h_tgt0, D, out, H)) {
-      PoolBuffer packed{st};
-      rc = packed.alloc(gemm_tc_gru_packed_bytes(H));
-      if (rc) return rc;
-      return launch_gemm_tc_gru(agg.f(), H, h_tgt0, D, gru_kernel, gru_recurrent_kernel, gru_bias, packed.f(), out, H, V,
-                                H, st);
-    }
-  }
-  PoolBuffer gx{st}, gh{st};
-  rc = gx.alloc((size_t)V * 3 * H * sizeof(float));
-  if (!rc) rc = gh.alloc((size_t)V * 3 * H * sizeof(float));
-  if (rc) return rc;
-  GemmEpilogue ex, eh;
-  ex.bias = gru_bias;
-  eh.bias = gru_bias + 3 * H;
-  rc = node_gemm(agg.f(), H, gru_kernel, 3 * H, gx.f(), 3 * H, V, 3 * H, H, ex, path, st);
-  if (rc) return rc;
-  const float* h_tgt = h + (size_t)b->tgt_off * D;
-  rc = node_gemm(h_tgt, D, gru_recurrent_kernel, 3 * H, gh.f(), 3 * H, V, 3 * H, H, eh, path, st);
-  if (rc) return rc;
-  gru_gate_kernel<<<grid_for(V * H), 256, 0, st>>>(gx.f(), nullptr, gh.f(), h_tgt, D, V, H, out);
-  TFGNN_LAUNCH_CHECK();
-  return 0;
+  const bool in_place = out < h + (size_t)b->V_src * D && h < out + (size_t)V * H;   // out overlaps the state table
+  return gru_update(agg.f(), h + (size_t)b->tgt_off * D, D, gru_kernel, gru_recurrent_kernel, gru_bias, V, H, path, in_place,
+                    out, st);
 }
 
 extern "C" int tfgnn_b200_gru_gate_fwd(const float* gx, const int32_t* gx_row_index, const float* gh, const float* h,

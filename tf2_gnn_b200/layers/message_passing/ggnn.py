@@ -7,7 +7,8 @@ import torch
 
 from ... import _ffi
 from ...runtime import PreparedBatch, stream_ptr
-from .gnn_edge_mlp import GNN_Edge_MLP
+from ..differentiable import edge_mlp_family_forward, gru_cell
+from .gnn_edge_mlp import GNN_Edge_MLP, _EdgeMLPLayerFunction
 from .message_passing import MessagePassingInput, _last_dim, register_message_passing_implementation
 
 
@@ -42,6 +43,33 @@ class _GGNNFunction(torch.autograd.Function):
             gru_bias.data_ptr(), grad_out.data_ptr(), grad_h.data_ptr(), _ffi.ptr_array(grad_w), g_k.data_ptr(),
             g_u.data_ptr(), g_b.data_ptr(), stream_ptr()))
         return (grad_h, None, None, g_k, g_u, g_b, *grad_w)
+
+
+class _GruUpdateFunction(torch.autograd.Function):
+    """GGNN's node update out = GRUCell(agg, h) on its own (ggnn.py:84-87): forward = tfgnn_b200_gru_update_fwd (the update
+    tfgnn_b200_ggnn_fwd runs), backward = tfgnn_b200_gru_update_bwd.  h = the layer's state rows."""
+
+    @staticmethod
+    def forward(ctx, agg, h, path, gru_kernel, gru_recurrent_kernel, gru_bias):
+        agg, h = agg.contiguous(), h.contiguous()
+        out = torch.empty_like(agg)
+        _ffi.check(_ffi.lib().tfgnn_b200_gru_update_fwd(
+            agg.data_ptr(), h.data_ptr(), int(agg.shape[0]), int(agg.shape[1]), gru_kernel.data_ptr(),
+            gru_recurrent_kernel.data_ptr(), gru_bias.data_ptr(), path, out.data_ptr(), stream_ptr()))
+        ctx.save_for_backward(agg, h, gru_kernel, gru_recurrent_kernel, gru_bias)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        agg, h, gru_kernel, gru_recurrent_kernel, gru_bias = ctx.saved_tensors
+        grad_out = grad_out.contiguous()
+        g_agg, g_h = torch.empty_like(agg), torch.empty_like(h)
+        g_k, g_u, g_b = (torch.empty_like(t) for t in (gru_kernel, gru_recurrent_kernel, gru_bias))
+        _ffi.check(_ffi.lib().tfgnn_b200_gru_update_bwd(
+            agg.data_ptr(), h.data_ptr(), int(agg.shape[0]), int(agg.shape[1]), gru_kernel.data_ptr(),
+            gru_recurrent_kernel.data_ptr(), gru_bias.data_ptr(), grad_out.data_ptr(), g_agg.data_ptr(), g_h.data_ptr(),
+            g_k.data_ptr(), g_u.data_ptr(), g_b.data_ptr(), stream_ptr()))
+        return g_agg, g_h, None, g_k, g_u, g_b
 
 
 @register_message_passing_implementation
@@ -86,9 +114,11 @@ class GGNN(GNN_Edge_MLP):
         gru = (self._gru_kernel.value, self._gru_recurrent_kernel.value, self._gru_bias.value)
         _ptrs, weights = self._mlp_weight_ptrs()
         if torch.is_grad_enabled() and (h.requires_grad or any(t.requires_grad for t in (*gru, *weights))):
-            cfg = {"H": self._hidden_dim, "n_hidden": int(self._num_edge_MLP_hidden_layers), "flags": self._flags(),
-                   "agg": self._aggregation_fn.code, "path": _ffi.PATH[self._path]}
-            return _GGNNFunction.apply(h, prepared, cfg, *gru, *weights)
+            if self._ggnn_bwd_takes_it():
+                cfg = {"H": self._hidden_dim, "n_hidden": int(self._num_edge_MLP_hidden_layers), "flags": self._flags(),
+                       "agg": self._aggregation_fn.code, "path": _ffi.PATH[self._path]}
+                return _GGNNFunction.apply(h, prepared, cfg, *gru, *weights)
+            return self._composed_forward(h, prepared, gru, weights)
         out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
         ptrs, _keep = self._mlp_weight_ptrs()
         _ffi.check(_ffi.lib().tfgnn_b200_ggnn_fwd(
@@ -97,6 +127,29 @@ class GGNN(GNN_Edge_MLP):
             self._gru_recurrent_kernel.value.data_ptr(), self._gru_bias.value.data_ptr(),
             _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
         return out
+
+    def _ggnn_bwd_takes_it(self) -> bool:
+        """The configurations _GGNNFunction trains (tfgnn_b200_ggnn_bwd): linear messages from the source state only,
+        hidden_dim % 4 == 0, max aggregation up to hidden_dim 512."""
+        H = self._hidden_dim
+        return (int(self._num_edge_MLP_hidden_layers) == 0 and not self._use_target_state_as_input and H % 4 == 0
+                and (self._aggregation_fn.name != "max" or H <= 512))
+
+    def _composed_forward(self, h: torch.Tensor, prepared: PreparedBatch, gru, weights) -> torch.Tensor:
+        """Every other message MLP under autograd: the messages through GNN_Edge_MLP's own routing without activation
+        (GGNN ignores activation-before, as its forward does), then the GRU update.  On the fused message paths this runs
+        the kernels of tfgnn_b200_ggnn_fwd in the same order, so training and inference give the same bits."""
+        if self._has_fused_backward(int(h.shape[1])):
+            cfg = dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers),
+                       flags=self._flags() & ~_ffi.FLAG_ACT_BEFORE_AGG, agg=self._aggregation_fn.code, act=_ffi.ACT[None],
+                       path=_ffi.PATH[self._path])
+            agg = _EdgeMLPLayerFunction.apply(h, prepared, cfg, *weights)
+        else:
+            agg = edge_mlp_family_forward(self, h, prepared, final_activation=False, activation_before=False)
+        lo, hi = prepared.target_range
+        if self._hidden_dim % 4 == 0:   # the shapes tfgnn_b200_gru_update_bwd differentiates
+            return _GruUpdateFunction.apply(agg, h[lo:hi], _ffi.PATH[self._path], *gru)
+        return gru_cell(agg, h[lo:hi], *gru)
 
     def set_weights_from_oracle_dict(self, w: Dict[str, Any]) -> None:
         super().set_weights_from_oracle_dict(w)

@@ -1,7 +1,7 @@
 """Measurement of the backward pass (SURVEY.md §8f-1) at bench.py's workloads: forward and backward device time of one
 RGCN, GGNN or GNN-FiLM layer through the autograd hook, CUDA events, inputs resident in HBM.
   python tools/bench_backward.py [--workload cfg2] [--steps 10] [--warmup 3] [--shards N] [--film-literal]
-                                 [--kind rgin|gnn_edge_mlp] [--literal]
+                                 [--kind rgin|gnn_edge_mlp|ggnn] [--literal]
                                  [--aggregation sum|mean|sqrt_n|max] [--act-before] [--activation NAME]
   python tools/bench_backward.py --kind rgat --literal [--steps 5] [--warmup 2]
 With --aggregation / --act-before / --activation: the layer's hyper-parameters changed accordingly (e.g. the RGCN layer of
@@ -13,8 +13,8 @@ With --film-literal: a reduced FiLM graph on which the literal per-edge path (la
 6 x 666,667 edges / D = H = 320, with the fused and the literal training step alternated in one process.
 --workload cfg3 is RGAT (tfgnn_b200_rgat_bwd); with --kind rgat --literal: cfg3's graph and layer shape reduced to 250k
 nodes / 3 x 1M edges, where the literal per-edge path fits, with the fused and the literal step alternated in one process.
-With --kind rgin|gnn_edge_mlp: that layer (class defaults, one hidden layer in the edge MLPs; RGIN normalised as in
-PPI_RGIN.json) on the workload's graph, with D = H = the workload's hidden_dim; the line carries the device memory in use and
+With --kind rgin|gnn_edge_mlp|ggnn: that layer (class defaults, one hidden layer in the edge MLPs; RGIN normalised as in
+PPI_RGIN.json; GGNN trains through the fused edge-MLP backward and the GRU update pair) on the workload's graph, with D = H = the workload's hidden_dim; the line carries the device memory in use and
 the literal path's saved activations computed from shapes.  Adding --literal runs the fused and the literal path alternated
 on a reduced graph (250k nodes / 4 x 1M edges / D = H = 256).
 With --shards N: the per-rank compute of training on N target-range shards (DESIGN.md §6), on ONE GPU and without
@@ -67,6 +67,8 @@ def main():
     if args.literal:
         if not args.kind and not config_overrides(args):
             ap.error("--literal needs --kind, --aggregation or --act-before")
+        if args.kind == "ggnn":
+            ap.error("--kind ggnn has no --literal comparison")
         return bench_edge_mlp_literal(args)
     wl = bench.WORKLOADS[args.workload]
     V, H, L = wl["V"], wl["H"], len(wl["E"])
@@ -113,6 +115,8 @@ def main():
         "card": card(), "note": NOTES.get(kind, NOTES["rgcn"])}
     if args.kind:
         rec["params"] = EDGE_MLP_KINDS[kind]
+        if kind == "ggnn":
+            rec["note"] = NOTES["ggnn_mlp"]
         rec["literal_saved_activations_GB_from_shapes"] = literal_footprint_gb(M, H, H, params)
     else:
         rec["forward_algorithmic_bytes"] = bench.algorithmic_bytes(kind, V, wl["E"], H, H, params)
@@ -125,7 +129,7 @@ def main():
 
 
 # --kind: class defaults (one hidden layer in the edge MLPs); RGIN with PPI_RGIN.json's normalisation
-EDGE_MLP_KINDS = {"rgin": {"normalize_by_num_incoming": True}, "gnn_edge_mlp": {}}
+EDGE_MLP_KINDS = {"rgin": {"normalize_by_num_incoming": True}, "gnn_edge_mlp": {}, "ggnn": {"num_edge_MLP_hidden_layers": 1}}
 
 
 def config_overrides(args):
@@ -155,6 +159,9 @@ NOTES = {
             "autograd hook overhead included; not tuned (two-kernel form, SIMT dW)",
     "ggnn": "backward = recomputed GRU inputs + gate backward + TN GEMMs for the GRU kernels + the RGCN-style message backward; "
             "autograd hook overhead included",
+    "ggnn_mlp": "one hidden layer in the message MLPs: the messages through the rgin-style fused backward, then the GRU update "
+                "pair (recomputed gx / gh, gate backward, TN GEMMs for the GRU kernels, tensor-core GEMMs for dagg and dh); "
+                "autograd hook overhead included",
     "rgin": "one hidden layer: backward = recompute Xs (= h U^s) and A_l (hidden_relu CSR reduce), dW2 (TN, fp32 FFMA), "
             "dA (tensor-core GEMM), dXs over the source-keyed CSR (one warp per (type, source)), dU (TN), grad_h "
             "(tensor-core GEMM, K = L*H); autograd hook overhead included",
