@@ -366,6 +366,11 @@ TFGNN_API int tfgnn_b200_layer_norm_bwd(const float* x, const float* gamma, cons
 TFGNN_API int tfgnn_b200_dropout(const float* x, int64_t n, float rate, uint64_t seed, uint64_t offset, float* out,
                                  void* stream);
 TFGNN_API int tfgnn_b200_axpby(const float* a, float alpha, const float* b, float beta, int64_t n, float* out, void* stream);
+/*   dropout_at       the masks of tfgnn_b200_dropout for elements [first_element, first_element + n) of the table a call with
+ *                    the same (seed, offset) masks: x and out hold those n elements.  A target-range shard passes
+ *                    first_element = lo * H and draws exactly the masks of its global rows. */
+TFGNN_API int tfgnn_b200_dropout_at(const float* x, int64_t n, float rate, uint64_t seed, uint64_t offset,
+                                    int64_t first_element, float* out, void* stream);
 
 /* ---- Differentiable generic path (SURVEY.md section 8f-1) -----------------------------------------------------------
  * The reference trains every variant by differentiating its literal op sequence (message_passing.py:95-218) with
@@ -460,6 +465,27 @@ TFGNN_API int tfgnn_b200_readout_bwd(const float* node_reprs, const float* weigh
                                      int32_t num_graphs, int32_t repr_dim, int32_t num_heads, int32_t mode, float lower,
                                      float upper, int32_t has_lower, int32_t has_upper, float* grad_reprs,
                                      float* grad_scores, void* stream);
+/* The readout on target-range shards (a rank owns rows [lo, hi) of the node table; a graph may span ranks).
+ *   readout_partial        over the rank's rows (node_to_graph_map, graph_ptr: those rows, GLOBAL graph ids, graph_ptr
+ *                          from tfgnn_b200_graph_offsets over them) the partial row of every graph, partial [G, P] with
+ *                          P = 2K + GD: K maxima m, K sums s = sum exp(w - m), GD sums S = sum exp(w - m) R (softmax:
+ *                          `scores` are the raw scores [V,K]); for sigmoid (`scores` = the weights [V,K]) S = sum w R and
+ *                          for none (scores NULL, K = 1) S = sum R, m and s unused.  R = node_reprs after the clamp.  A
+ *                          graph without rows on the rank gets the neutral partial (m = -inf, s = 0, S = 0).  Rows in
+ *                          fixed 256-row chunks, pieces combined in chunk order: no atomics, a function of the rows alone.
+ *   readout_merge          partials [world, G, P] (every rank's, in rank order) -> out [G, GD]: combined in rank order with
+ *                          the online-softmax rescale m = max m_r, s = sum s_r e^(m_r - m), out = sum S_r e^(m_r - m) / s
+ *                          (sigmoid / none: out = sum S_r), and for softmax the normaliser graph_max, graph_sum [G, K].  Every
+ *                          rank that merges the same gathered partials gets the same bits.
+ * The backward on the rank's rows is tfgnn_b200_readout_bwd with the full-graph grad_out and out, and for softmax the
+ * weights exp(score - graph_max[g]) / graph_sum[g] (tfgnn_b200_softmax_apply on the gathered normaliser).  Average
+ * weighting is not built for shards (TFGNN_ERR_INVALID_ARGUMENT). */
+TFGNN_API int tfgnn_b200_readout_partial(const float* scores, const float* node_reprs, const int32_t* node_to_graph_map,
+                                         const int32_t* graph_ptr, int64_t num_rows, int32_t num_graphs, int32_t repr_dim,
+                                         int32_t num_heads, int32_t mode, float* partial, void* stream);
+TFGNN_API int tfgnn_b200_readout_merge(const float* partials, int32_t world_size, int32_t num_graphs, int32_t repr_dim,
+                                       int32_t num_heads, int32_t mode, float* out, float* graph_max, float* graph_sum,
+                                       void* stream);
 TFGNN_API int tfgnn_b200_gru_gate_bwd_indexed(const float* gx, const int32_t* node_to_graph_map, const int32_t* graph_ptr,
                                               const float* gh, const float* h, const float* grad_out, int64_t num_rows,
                                               int32_t num_graphs, int32_t H, float* grad_gx, float* grad_gh,

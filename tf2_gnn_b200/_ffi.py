@@ -47,6 +47,7 @@ EXPORTED_SYMBOLS = (
     "tfgnn_b200_edge_mlp_bwd", "tfgnn_b200_rgat_bwd",
     "tfgnn_b200_segment_sum_rows", "tfgnn_b200_readout_bwd", "tfgnn_b200_gru_gate_bwd_indexed",
     "tfgnn_b200_gru_update_fwd", "tfgnn_b200_gru_update_bwd",
+    "tfgnn_b200_dropout_at", "tfgnn_b200_readout_partial", "tfgnn_b200_readout_merge",
 )
 
 _PP = POINTER(c_void_p)
@@ -135,6 +136,12 @@ def lib() -> ctypes.CDLL:
     L.tfgnn_b200_layer_norm_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_float, c_void_p, c_void_p,
                                             c_void_p, c_void_p]
     L.tfgnn_b200_dropout.argtypes = [c_void_p, c_int64, c_float, ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_void_p]
+    L.tfgnn_b200_dropout_at.argtypes = [c_void_p, c_int64, c_float, ctypes.c_uint64, ctypes.c_uint64, c_int64, c_void_p,
+                                        c_void_p]
+    L.tfgnn_b200_readout_partial.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32,
+                                             c_int32, c_void_p, c_void_p]
+    L.tfgnn_b200_readout_merge.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
+                                           c_void_p, c_void_p]
     L.tfgnn_b200_axpby.argtypes = [c_void_p, c_float, c_void_p, c_float, c_int64, c_void_p, c_void_p]
     L.tfgnn_b200_activation_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p]
     L.tfgnn_b200_row_scale.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p]

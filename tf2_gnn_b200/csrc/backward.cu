@@ -1364,20 +1364,22 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
 }
 
 // tf.nn.dropout(x, rate): keep with probability 1 - rate, scale kept values by 1 / (1 - rate)   (gnn.py:285-289)
+// x[i] is element first + i of the masked table: its mask is word (first + i) % 4 of Philox counter offset + (first + i) / 4.
 __global__ void dropout_kernel(const float* __restrict__ x, long long n, float rate, unsigned long long seed,
-                               unsigned long long offset, float* __restrict__ out) {
+                               unsigned long long offset, long long first, float* __restrict__ out) {
   const float scale = 1.0f / (1.0f - rate);
-  const long long groups = (n + 3) >> 2;
+  const long long g0 = first >> 2;
+  const long long groups = ((first + n + 3) >> 2) - g0;
   for (long long gi = (long long)blockIdx.x * blockDim.x + threadIdx.x; gi < groups;
        gi += (long long)gridDim.x * blockDim.x) {
-    const unsigned long long c = (unsigned long long)gi + offset;
+    const unsigned long long c = (unsigned long long)(g0 + gi) + offset;
     const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), 0u, 0u),
                                   make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
     const uint32_t w[4] = {r.x, r.y, r.z, r.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const long long i = gi * 4 + j;
-      if (i < n) {
+      const long long i = (g0 + gi) * 4 + j - first;
+      if (i >= 0 && i < n) {
         const float u = (float)(w[j] >> 8) * (1.0f / 16777216.0f);   // uniform in [0, 1)
         out[i] = u >= rate ? x[i] * scale : 0.0f;
       }
@@ -1466,7 +1468,21 @@ extern "C" int tfgnn_b200_dropout(const float* x, int64_t n, float rate, uint64_
   TFGNN_REQUIRE(n >= 0 && rate >= 0.0f && rate < 1.0f, "dropout rate must lie in [0, 1)");
   if (n == 0) return 0;
   TFGNN_REQUIRE(x && out, "NULL pointer");
-  dropout_kernel<<<grid_for((n + 3) / 4), 256, 0, (cudaStream_t)stream>>>(x, n, rate, seed, offset, out);
+  dropout_kernel<<<grid_for((n + 3) / 4), 256, 0, (cudaStream_t)stream>>>(x, n, rate, seed, offset, 0, out);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+// The same masks for a slice of a larger table: x is elements [first_element, first_element + n) of the table a call of
+// tfgnn_b200_dropout with the same (seed, offset) would mask (a target-range shard's rows of a [V, H] table).
+extern "C" int tfgnn_b200_dropout_at(const float* x, int64_t n, float rate, uint64_t seed, uint64_t offset,
+                                     int64_t first_element, float* out, void* stream) {
+  TFGNN_REQUIRE(n >= 0 && rate >= 0.0f && rate < 1.0f, "dropout rate must lie in [0, 1)");
+  TFGNN_REQUIRE(first_element >= 0, "dropout_at: first_element must not be negative");
+  if (n == 0) return 0;
+  TFGNN_REQUIRE(x && out, "NULL pointer");
+  dropout_kernel<<<grid_for((first_element % 4 + n + 3) / 4), 256, 0, (cudaStream_t)stream>>>(x, n, rate, seed, offset,
+                                                                                               first_element, out);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }

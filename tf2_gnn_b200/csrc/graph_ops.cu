@@ -11,6 +11,8 @@
 //   dense_bias_fwd          Dense with bias (readout MLPs with use_biases, GRU cell halves)
 //   segment_sum_rows        out[g] = sum_{v in g} data[v]: adjoint of table[node_to_graph_map], fixed 64-row chunks
 //   readout_bwd             gradients of weighted_segment_sum through the weighting and the clamp, one pass over the nodes
+//   readout_partial / _merge  the readout of a target-range shard: per-graph (max, sum, weighted sum) partials of the
+//                           owned rows, and the rank-ordered online-softmax merge of every rank's partials
 // All HBM-bound and tiny next to the message-passing layers; deterministic (fixed reduction orders).
 #include "layers.cuh"
 
@@ -285,9 +287,210 @@ __global__ void readout_bwd_kernel(const float* __restrict__ reprs, const float*
   }
 }
 
+// ---- target-range shards: per-graph readout partials and their rank-ordered merge ------------------------------------
+// The partial row of graph g (P = 2K + GD floats): K running maxima m, K sums s = sum exp(w - m) and GD weighted row sums
+// S = sum exp(w - m) t (softmax); S = sum w t (sigmoid, w = 1 for none), m and s unused.  Neutral: m = -inf, s = 0, S = 0.
+// Two partials combine as m = max(m1, m2), s = s1 e^(m1-m) + s2 e^(m2-m), S likewise: the online-softmax rescale of the
+// RGAT hub-chunk combine.  Rows are cut into fixed kPartRows chunks (the result is a function of the rows and the cut only);
+// a graph that crosses a chunk border leaves pieces in head / tail slots that the finish kernel combines in chunk order.
+constexpr int kPartRows = 256, kPartThreads = 64, kPartLanes = 8, kPartCols = 32;
+
+template <bool SOFTMAX>
+__device__ __forceinline__ void part_combine(float& m, float& s, float& S, float m2, float s2, float S2) {
+  if (!SOFTMAX) { S += S2; return; }
+  const float mn = fmaxf(m, m2);
+  if (mn == -INFINITY) return;                 // both neutral
+  const float a = expf(m - mn), b = expf(m2 - mn);
+  s = s * a + s2 * b;
+  S = S * a + S2 * b;
+  m = mn;
+}
+
+// writes column c of a partial row: S always, m and s from the first column of each head
+__device__ __forceinline__ void part_store(float* row, int c, int d, int K, float m, float s, float S) {
+  row[2 * K + c] = S;
+  if (c % d == 0) {
+    row[c / d] = m;
+    row[K + c / d] = s;
+  }
+}
+
+// grid = (chunks, column tiles of kPartThreads); scratch [chunks][2][P] (head slot 0, tail slot 1)
+template <bool SOFTMAX>
+__global__ void __launch_bounds__(kPartThreads)
+readout_partial_chunks_kernel(const float* __restrict__ w, const float* __restrict__ reprs, const int* __restrict__ n2g,
+                              const int* __restrict__ graph_ptr, long long V, int GD, int K,
+                              float* __restrict__ partial, float* __restrict__ scratch) {
+  __shared__ int row_graph[kPartRows];
+  const long long r0 = (long long)blockIdx.x * kPartRows;
+  const int rows = (int)(V - r0 < kPartRows ? V - r0 : kPartRows);
+  for (int j = threadIdx.x; j < rows; j += kPartThreads) row_graph[j] = __ldg(n2g + r0 + j);
+  __syncthreads();
+  const int c = blockIdx.y * kPartThreads + threadIdx.x;
+  if (c >= GD) return;
+  const int d = GD / K, k = c / d, P = 2 * K + GD;
+  auto emit = [&](int g, float m, float s, float S) {
+    const long long beg = graph_ptr[g], end = graph_ptr[g + 1];
+    float* dst = beg < r0 ? scratch + ((long long)blockIdx.x * 2) * P
+                          : (end > r0 + rows ? scratch + ((long long)blockIdx.x * 2 + 1) * P : partial + (long long)g * P);
+    part_store(dst, c, d, K, m, s, S);
+  };
+  int cur = row_graph[0];
+  float m = -INFINITY, s = 0.f, S = 0.f;
+  for (int j = 0; j < rows; ++j) {
+    const int g = row_graph[j];
+    if (g != cur) {
+      emit(cur, m, s, S);
+      m = -INFINITY; s = 0.f; S = 0.f;
+      cur = g;
+    }
+    const long long v = r0 + j;
+    const float t = __ldg(reprs + v * GD + c);
+    const float x = w ? __ldg(w + v * K + k) : 1.f;
+    if (SOFTMAX) {
+      const float mn = fmaxf(m, x);
+      const float a = expf(m - mn), e = expf(x - mn);
+      s = s * a + e;
+      S = S * a + e * t;
+      m = mn;
+    } else {
+      S += x * t;
+    }
+  }
+  emit(cur, m, s, S);
+}
+
+// Graphs that cross a chunk border: the tail slot of their first chunk, then the head slots of the chunks that follow, by
+// kPartLanes lanes (lane j takes pieces j, j + kPartLanes, ... in order) whose results are combined in lane order.  Graphs
+// without rows get the neutral partial.  block = (kPartCols, kPartLanes); grid = (graphs, strided; column tiles)
+template <bool SOFTMAX>
+__global__ void __launch_bounds__(kPartCols * kPartLanes)
+readout_partial_finish_kernel(const float* __restrict__ scratch, const int* __restrict__ graph_ptr, int G, int GD, int K,
+                              float* __restrict__ partial) {
+  __shared__ float pm[kPartLanes][kPartCols], ps[kPartLanes][kPartCols], pS[kPartLanes][kPartCols];
+  const int c = blockIdx.y * kPartCols + threadIdx.x;
+  const int j = threadIdx.y;
+  const int d = GD / K, P = 2 * K + GD;
+  for (int g = blockIdx.x; g < G; g += gridDim.x) {
+    const int beg = graph_ptr[g], end = graph_ptr[g + 1];
+    if (beg == end) {
+      if (j == 0 && c < GD) part_store(partial + (long long)g * P, c, d, K, -INFINITY, 0.f, 0.f);
+      continue;
+    }
+    const int first = beg / kPartRows, last = (end - 1) / kPartRows;
+    if (first == last) continue;   // final since the chunk kernel
+    float m = -INFINITY, s = 0.f, S = 0.f;
+    if (c < GD)
+      for (int t = j; t <= last - first; t += kPartLanes) {
+        const float* piece = scratch + ((long long)(first + t) * 2 + (t == 0 ? 1 : 0)) * P;
+        part_combine<SOFTMAX>(m, s, S, __ldg(piece + c / d), __ldg(piece + K + c / d), __ldg(piece + 2 * K + c));
+      }
+    pm[j][threadIdx.x] = m;
+    ps[j][threadIdx.x] = s;
+    pS[j][threadIdx.x] = S;
+    __syncthreads();
+    if (j == 0 && c < GD) {
+      for (int t = 1; t < kPartLanes; ++t) part_combine<SOFTMAX>(m, s, S, pm[t][threadIdx.x], ps[t][threadIdx.x], pS[t][threadIdx.x]);
+      part_store(partial + (long long)g * P, c, d, K, m, s, S);
+    }
+    __syncthreads();
+  }
+}
+
+// One thread per (graph, column): the world's partials combined in rank order, then out = S / s (softmax) or S.
+template <bool SOFTMAX>
+__global__ void readout_merge_kernel(const float* __restrict__ partials, int world, int G, int GD, int K,
+                                     float* __restrict__ out, float* __restrict__ gmax, float* __restrict__ gsum) {
+  const int d = GD / K, P = 2 * K + GD;
+  const long long total = (long long)G * GD;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long g = i / GD;
+    const int c = (int)(i - g * GD), k = c / d;
+    float m = -INFINITY, s = 0.f, S = 0.f;
+    for (int r = 0; r < world; ++r) {
+      const float* row = partials + ((long long)r * G + g) * P;
+      part_combine<SOFTMAX>(m, s, S, __ldg(row + k), __ldg(row + K + k), __ldg(row + 2 * K + c));
+    }
+    if (SOFTMAX) {
+      out[i] = s > 0.f ? S / s : 0.f;
+      if (c % d == 0) {
+        gmax[g * K + k] = m;
+        gsum[g * K + k] = s;
+      }
+    } else {
+      out[i] = S;
+    }
+  }
+}
+
 }  // namespace tfgnn
 
 using namespace tfgnn;
+
+extern "C" int tfgnn_b200_readout_partial(const float* scores, const float* node_reprs, const int32_t* node_to_graph_map,
+                                          const int32_t* graph_ptr, int64_t num_rows, int32_t num_graphs, int32_t repr_dim,
+                                          int32_t num_heads, int32_t mode, float* partial, void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && num_rows < (1ll << 31) && num_graphs >= 0 && repr_dim > 0 && num_heads > 0 &&
+                    repr_dim % num_heads == 0,
+                "bad readout_partial sizes (num_heads must divide the representation size)");
+  TFGNN_REQUIRE(mode >= TFGNN_READOUT_SOFTMAX && mode <= TFGNN_READOUT_NONE,
+                "readout_partial: weighting mode must be softmax, sigmoid or none (average is not built for shards)");
+  if (num_graphs == 0) return 0;
+  TFGNN_REQUIRE(graph_ptr && partial, "NULL pointer");
+  const bool weighted = mode != TFGNN_READOUT_NONE;
+  TFGNN_REQUIRE(num_rows == 0 || (node_reprs && node_to_graph_map && (!weighted || scores)), "NULL pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool softmax = mode == TFGNN_READOUT_SOFTMAX;
+  const int K = weighted ? num_heads : 1;
+  const int chunks = ceil_div(num_rows, kPartRows);
+  const int P = 2 * K + repr_dim;
+  PoolBuffer scratch{st};
+  if (chunks) {
+    int rc = scratch.alloc((size_t)chunks * 2 * P * sizeof(float));
+    if (rc) return rc;
+    dim3 grid((unsigned)chunks, (unsigned)ceil_div(repr_dim, kPartThreads));
+    const float* w = weighted ? scores : nullptr;
+    if (softmax)
+      readout_partial_chunks_kernel<true><<<grid, kPartThreads, 0, st>>>(w, node_reprs, node_to_graph_map, graph_ptr,
+                                                                        num_rows, repr_dim, K, partial, scratch.f());
+    else
+      readout_partial_chunks_kernel<false><<<grid, kPartThreads, 0, st>>>(w, node_reprs, node_to_graph_map, graph_ptr,
+                                                                         num_rows, repr_dim, K, partial, scratch.f());
+    TFGNN_LAUNCH_CHECK();
+  }
+  dim3 grid((unsigned)(num_graphs < 132 * 8 ? num_graphs : 132 * 8), (unsigned)ceil_div(repr_dim, kPartCols));
+  if (softmax)
+    readout_partial_finish_kernel<true><<<grid, dim3(kPartCols, kPartLanes), 0, st>>>(scratch.f(), graph_ptr, num_graphs,
+                                                                                      repr_dim, K, partial);
+  else
+    readout_partial_finish_kernel<false><<<grid, dim3(kPartCols, kPartLanes), 0, st>>>(scratch.f(), graph_ptr, num_graphs,
+                                                                                       repr_dim, K, partial);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int tfgnn_b200_readout_merge(const float* partials, int32_t world_size, int32_t num_graphs, int32_t repr_dim,
+                                        int32_t num_heads, int32_t mode, float* out, float* graph_max, float* graph_sum,
+                                        void* stream) {
+  TFGNN_REQUIRE(world_size > 0 && num_graphs >= 0 && repr_dim > 0 && num_heads > 0 && repr_dim % num_heads == 0,
+                "bad readout_merge sizes (num_heads must divide the representation size)");
+  TFGNN_REQUIRE(mode >= TFGNN_READOUT_SOFTMAX && mode <= TFGNN_READOUT_NONE,
+                "readout_merge: weighting mode must be softmax, sigmoid or none (average is not built for shards)");
+  if (num_graphs == 0) return 0;
+  const bool softmax = mode == TFGNN_READOUT_SOFTMAX;
+  TFGNN_REQUIRE(partials && out && (!softmax || (graph_max && graph_sum)), "NULL pointer (softmax needs graph_max, graph_sum)");
+  const int K = mode == TFGNN_READOUT_NONE ? 1 : num_heads;
+  const long long total = (long long)num_graphs * repr_dim;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (softmax)
+    readout_merge_kernel<true><<<grid_for(total), 256, 0, st>>>(partials, world_size, num_graphs, repr_dim, K, out,
+                                                                graph_max, graph_sum);
+  else
+    readout_merge_kernel<false><<<grid_for(total), 256, 0, st>>>(partials, world_size, num_graphs, repr_dim, K, out,
+                                                                 nullptr, nullptr);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
 
 extern "C" int tfgnn_b200_segment_sum_rows(const float* data, const int32_t* node_to_graph_map, const int32_t* graph_ptr,
                                            int64_t num_rows, int32_t num_graphs, int32_t C, float* out, void* stream) {

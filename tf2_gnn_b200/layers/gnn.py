@@ -166,29 +166,57 @@ class GNN:
     trainable_variables = variables
     weights = variables
 
-    def __call__(self, inputs: GNNInput, training: bool = False, return_all_representations: bool = False):
+    def __call__(self, inputs: GNNInput, training: bool = False, return_all_representations: bool = False, shard=None):
         if not self.built:
             self.build(GNNInput(tuple(inputs.node_features.shape),
                                 tuple(tuple(a.shape) for a in inputs.adjacency_lists), None, None))
-        return self.call(inputs, training=training, return_all_representations=return_all_representations)
+        return self.call(inputs, training=training, return_all_representations=return_all_representations, shard=shard)
 
-    def call(self, inputs: GNNInput, training: bool = False, return_all_representations: bool = False):
-        """gnn.py:234-274."""
-        cur, all_reps = self._internal_call(inputs, training, want_all_representations=return_all_representations)
+    def call(self, inputs: GNNInput, training: bool = False, return_all_representations: bool = False, shard=None):
+        """gnn.py:234-274.
+
+        shard (sharding.TargetRangeShard): run on one rank of a graph cut by target range.  node_features and
+        node_to_graph_map are the rank's rows [lo, hi), the adjacency lists hold global node ids (all edges, or those into
+        [lo, hi)), num_graphs is the global count; the result is the rank's rows.  Every message-passing layer reads the
+        all-gathered table (sharding.gather_node_states); the node-level glue runs on the rank's rows and dropout draws the
+        unsharded masks of those rows; the readout of a global exchange is merged over the ranks in rank order.  Collective
+        in forward and backward: every rank of the shard's group makes the same calls.  Weight gradients come out as the
+        rank's part: sharding.sum_gradients_over_ranks(gnn.trainable_variables) sums them."""
+        cur, all_reps = self._internal_call(inputs, training, want_all_representations=return_all_representations,
+                                            shard=shard)
         if return_all_representations:
             return cur, all_reps
         return cur
 
-    def _internal_call(self, inputs: GNNInput, training: bool = False, want_all_representations: bool = True):
+    def _internal_call(self, inputs: GNNInput, training: bool = False, want_all_representations: bool = True, shard=None):
         """gnn.py:276-329.  When the caller does not ask for the per-layer representations (the reference's traced function
         always returns them and `call` drops them), a message-passing layer that is directly followed by its LayerNorm runs
         both in one fused call (`call_with_layernorm`) and the tuple holds None for that layer."""
+        if shard is not None and self._message_passing_class.__name__ == "GNN_FiLM":
+            raise NotImplementedError(
+                "GNN: a GNN-FiLM stack on target-range shards is not built (its sharded gradients do not yet meet the "
+                "float64 bar the unsharded stack meets); GNN_FiLM layers themselves train on shards through "
+                "sharding.gather_node_states and PreparedBatch(..., target_range=(lo, hi))")
         feats = to_device_f32(inputs.node_features)
         adjs = tuple(to_device_adj(a, feats.device) for a in inputs.adjacency_lists)
-        if all(a is b for a, b in zip(adjs, inputs.adjacency_lists)):
-            prepared = prepared_batch_for(adjs, int(feats.shape[0]))
+        rows = None
+        if shard is not None:
+            if int(feats.shape[0]) != shard.hi - shard.lo:
+                raise ValueError(f"a shard's node_features hold its {shard.hi - shard.lo} rows, got {int(feats.shape[0])}")
+            from .. import sharding
+            prepared = PreparedBatch(adjs, shard.num_nodes, target_range=(shard.lo, shard.hi))
+            rows = shard.rows
+
+            def layer_input(h):
+                return sharding.gather_node_states(h, shard.bounds, shard.group)
         else:
-            prepared = PreparedBatch(adjs, int(feats.shape[0]))
+            if all(a is b for a, b in zip(adjs, inputs.adjacency_lists)):
+                prepared = prepared_batch_for(adjs, int(feats.shape[0]))
+            else:
+                prepared = PreparedBatch(adjs, int(feats.shape[0]))
+
+            def layer_input(h):
+                return h
         cur = self._initial_projection_layer(feats)
         last = cur
         all_reps = [cur]
@@ -201,7 +229,7 @@ class GNN:
         dropout_rate = float(self._params.get("layer_input_dropout_rate", 0.0))
         for layer_idx, mp_layer in enumerate(self._mp_layers):
             if training:                                                             # gnn.py:285-289
-                cur = node_ops.dropout(cur, dropout_rate, self.dropout_state)
+                cur = node_ops.dropout(cur, dropout_rate, self.dropout_state, rows)
             if layer_idx % self._residual_every_num_layers == 0:                     # gnn.py:291-296
                 tmp = cur
                 if layer_idx > 0:
@@ -213,15 +241,16 @@ class GNN:
                 ln = self._inter_layer_layernorms[layer_idx]
                 if not mp_layer.built:
                     mp_layer.build(MessagePassingInput(tuple(cur.shape), tuple(tuple(a.shape) for a in adjs)))
-                cur = mp_layer.call_with_layernorm(MessagePassingInput(cur, adjs), ln.gamma.value, ln.beta.value, ln.epsilon,
+                cur = mp_layer.call_with_layernorm(MessagePassingInput(layer_input(cur), adjs), ln.gamma.value,
+                                                   ln.beta.value, ln.epsilon,
                                                    prepared=prepared)     # gnn.py:299-304 + 317-321 in one call
                 all_reps.append(None)
             else:
-                cur = mp_layer(MessagePassingInput(cur, adjs), training=training, prepared=prepared)
+                cur = mp_layer(MessagePassingInput(layer_input(cur), adjs), training=training, prepared=prepared)
                 all_reps.append(cur)
                 if has_exchange:                                                         # gnn.py:307-315
                     cur = self._global_exchange_layers[str(layer_idx)](
-                        GraphGlobalExchangeInput(cur, n2g, int(inputs.num_graphs)), training=training)
+                        GraphGlobalExchangeInput(cur, n2g, int(inputs.num_graphs)), training=training, shard=shard)
                 if self._use_inter_layer_layernorm:
                     cur = self._inter_layer_layernorms[layer_idx](cur)
             if layer_idx % self._dense_every_num_layers == 0:

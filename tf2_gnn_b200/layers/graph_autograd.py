@@ -70,6 +70,82 @@ def readout(scores: Optional[torch.Tensor], reprs: torch.Tensor, n2g: torch.Tens
     return _ReadoutFunction.apply(scores, reprs, n2g, graph_ptr, int(num_heads), weighting_fun, lower, upper)
 
 
+# ---- readout on a target-range shard -------------------------------------------------------------------------------
+class _ShardReadoutFunction(torch.autograd.Function):
+    """The readout of graphs whose rows may lie on several ranks.  Forward: tfgnn_b200_readout_partial over the rank's rows,
+    an all-gather of the [G, 2K + GD] partials, tfgnn_b200_readout_merge in rank order: every rank gets the same [G, GD]
+    bits.  Backward: the gradient arriving at the graph rows on each rank is that rank's part (e.g. the segment sum over its
+    own rows of what it broadcast to them); the parts are all-gathered and added in rank order, and tfgnn_b200_readout_bwd
+    runs on the rank's rows with the full-graph gradient, the merged result and, for softmax, the weights from the global
+    normaliser."""
+
+    @staticmethod
+    def forward(ctx, scores, reprs, n2g, graph_ptr, num_graphs, num_heads, weighting_fun, lower, upper, shard):
+        from .. import sharding
+        mode = _ffi.READOUT_MODE[weighting_fun]
+        reprs = reprs.contiguous()
+        clamped = reprs if lower is None and upper is None else node_ops.clamp_(reprs.clone(), lower, upper)
+        weights = None
+        if weighting_fun == "softmax":
+            scores = scores.contiguous()
+        elif weighting_fun == "sigmoid":
+            scores = scores.contiguous()
+            weights = torch.empty_like(scores)
+            _ffi.check(_ffi.lib().tfgnn_b200_activation(scores.data_ptr(), scores.numel(), _ffi.ACT_SIGMOID,
+                                                        weights.data_ptr(), stream_ptr()))
+        G, GD, V = int(num_graphs), int(reprs.shape[1]), int(reprs.shape[0])
+        K = 1 if weighting_fun == "none" else int(num_heads)
+        partial = torch.empty((G, 2 * K + GD), dtype=torch.float32, device=reprs.device)
+        w_in = scores if weighting_fun == "softmax" else weights
+        _ffi.check(_ffi.lib().tfgnn_b200_readout_partial(_ptr(w_in), clamped.data_ptr(), n2g.data_ptr(),
+                                                         graph_ptr.data_ptr(), V, G, GD, int(num_heads), mode,
+                                                         partial.data_ptr(), stream_ptr()))
+        parts = sharding.all_gather_stacked(partial, shard.group)
+        out = torch.empty((G, GD), dtype=torch.float32, device=reprs.device)
+        gmax = gsum = None
+        if weighting_fun == "softmax":
+            gmax = torch.empty((G, K), dtype=torch.float32, device=reprs.device)
+            gsum = torch.empty_like(gmax)
+        _ffi.check(_ffi.lib().tfgnn_b200_readout_merge(parts.data_ptr(), int(parts.shape[0]), G, GD, int(num_heads), mode,
+                                                       out.data_ptr(), _ptr(gmax), _ptr(gsum), stream_ptr()))
+        ctx.cfg = (n2g, graph_ptr, int(num_heads), weighting_fun, lower, upper, shard)
+        ctx.save_for_backward(reprs, scores if weighting_fun == "softmax" else weights, out, gmax, gsum)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from .. import sharding
+        reprs, w_saved, out, gmax, gsum = ctx.saved_tensors
+        n2g, graph_ptr, num_heads, weighting_fun, lower, upper, shard = ctx.cfg
+        grad_full = sharding.sum_over_ranks(grad_out.contiguous(), shard.group)
+        V = int(reprs.shape[0])
+        weights = w_saved
+        if weighting_fun == "softmax":                    # exp(score - max_g) / sum_g with the merged normaliser
+            weights = torch.empty_like(w_saved)
+            m_rows, s_rows = _gather_graph_rows(gmax, n2g), _gather_graph_rows(gsum, n2g)
+            _ffi.check(_ffi.lib().tfgnn_b200_softmax_apply(w_saved.data_ptr(), m_rows.data_ptr(), s_rows.data_ptr(),
+                                                           weights.numel(), weights.data_ptr(), stream_ptr()))
+        grad_reprs = torch.empty_like(reprs)
+        grad_scores = torch.empty_like(weights) if weights is not None else None
+        _ffi.check(_ffi.lib().tfgnn_b200_readout_bwd(
+            reprs.data_ptr(), _ptr(weights), n2g.data_ptr(), graph_ptr.data_ptr(), out.data_ptr(), grad_full.data_ptr(),
+            V, int(out.shape[0]), int(reprs.shape[1]), num_heads, _ffi.READOUT_MODE[weighting_fun],
+            float(lower or 0.0), float(upper or 0.0), 0 if lower is None else 1, 0 if upper is None else 1,
+            grad_reprs.data_ptr(), _ptr(grad_scores), stream_ptr()))
+        return grad_scores, grad_reprs, None, None, None, None, None, None, None, None
+
+
+def shard_readout(scores: Optional[torch.Tensor], reprs: torch.Tensor, n2g: torch.Tensor, graph_ptr: torch.Tensor,
+                  num_graphs: int, num_heads: int, weighting_fun: str, lower: Optional[float], upper: Optional[float],
+                  shard) -> torch.Tensor:
+    """The readout of the rank's rows (n2g, graph_ptr: those rows, global graph ids) merged over the ranks of `shard`:
+    [num_graphs, GD], the same bits on every rank.  Collective: every rank calls it, forward and backward."""
+    if weighting_fun == "average":
+        raise NotImplementedError("average weighting is not built for target-range shards")
+    return _ShardReadoutFunction.apply(scores, reprs, n2g, graph_ptr, int(num_graphs), int(num_heads), weighting_fun, lower,
+                                       upper, shard)
+
+
 # ---- per-node copies (only where a per-node dropout mask needs them) ----------------------------------------------
 def _gather_graph_rows(table: torch.Tensor, n2g: torch.Tensor) -> torch.Tensor:
     V, H = int(n2g.shape[0]), int(table.shape[1])

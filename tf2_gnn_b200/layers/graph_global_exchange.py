@@ -56,15 +56,20 @@ class GraphGlobalExchange:
 
     trainable_variables = variables
 
-    def __call__(self, inputs: GraphGlobalExchangeInput, training: bool = False):
+    def __call__(self, inputs: GraphGlobalExchangeInput, training: bool = False, shard=None):
         if not self.built:
             self.build(GraphGlobalExchangeInput((None, self._hidden_dim), (None,), ()))
-        return self.call(inputs, training=training)
+        return self.call(inputs, training=training, shard=shard)
 
-    def _prepare(self, inputs: GraphGlobalExchangeInput, training: bool):
+    def _prepare(self, inputs: GraphGlobalExchangeInput, training: bool, shard=None):
         """graph_global_exchange.py:83-103: the node states, the per-graph representations [G, H], node_to_graph_map and
         graph_ptr.  With the exchange's own dropout active the representations come back per NODE ([V, H]) and the map is
-        None: tf.nn.dropout acts on the per-node copies (:98-101), the mask differs per node."""
+        None: tf.nn.dropout acts on the per-node copies (:98-101), the mask differs per node.
+
+        shard (sharding.TargetRangeShard): node_embeddings and node_to_graph_map are the rank's rows (global graph ids),
+        num_graphs the global count.  The per-graph rows are merged over the ranks (the same on every rank), the combine
+        runs on the rank's rows, and graph_ptr indexes those rows.  Every backward step that sums over a graph's rows
+        gives the rank's part, which the readout's backward sums over the ranks."""
         x = to_device_f32(inputs.node_embeddings)
         n2g = inputs.node_to_graph_map
         if not isinstance(n2g, torch.Tensor):
@@ -74,18 +79,19 @@ class GraphGlobalExchange:
         graph_ptr = node_ops.graph_offsets(n2g, num_graphs)
         self._node_to_graph_representation_layer.dropout_state = self.dropout_state
         graph_reprs = self._node_to_graph_representation_layer.call(
-            NodesToGraphRepresentationInput(x, n2g, num_graphs), training=training, graph_ptr=graph_ptr)
+            NodesToGraphRepresentationInput(x, n2g, num_graphs), training=training, graph_ptr=graph_ptr, shard=shard)
         if training and self._dropout_rate > 0.0:
             per_node = graph_autograd.gather_graph_rows(graph_reprs, n2g, graph_ptr)
-            return x, node_ops.dropout(per_node, self._dropout_rate, self.dropout_state), None, graph_ptr
+            rows = shard.rows if shard is not None else None
+            return x, node_ops.dropout(per_node, self._dropout_rate, self.dropout_state, rows), None, graph_ptr
         return x, graph_reprs, n2g, graph_ptr
 
 
 class GraphGlobalMeanExchange(GraphGlobalExchange):
     """(x + g[node_to_graph_map]) / 2 (graph_global_exchange.py:106-124)."""
 
-    def call(self, inputs: GraphGlobalExchangeInput, training: bool = False):
-        x, g, index, graph_ptr = self._prepare(inputs, training)
+    def call(self, inputs: GraphGlobalExchangeInput, training: bool = False, shard=None):
+        x, g, index, graph_ptr = self._prepare(inputs, training, shard)
         if node_ops._needs_grad(x, g):
             if index is None:
                 from .differentiable import _AddFunction
@@ -112,8 +118,8 @@ class GraphGlobalGRUExchange(GraphGlobalExchange):
 
     trainable_variables = variables
 
-    def call(self, inputs: GraphGlobalExchangeInput, training: bool = False):
-        x, g, index, graph_ptr = self._prepare(inputs, training)
+    def call(self, inputs: GraphGlobalExchangeInput, training: bool = False, shard=None):
+        x, g, index, graph_ptr = self._prepare(inputs, training, shard)
         if node_ops._needs_grad(x, g, self._gru_kernel.value, self._gru_recurrent_kernel.value, self._gru_bias.value):
             if index is None:
                 from .differentiable import gru_cell
@@ -140,14 +146,15 @@ class GraphGlobalMLPExchange(GraphGlobalExchange):
 
     trainable_variables = variables
 
-    def call(self, inputs: GraphGlobalExchangeInput, training: bool = False):
-        x, g, index, graph_ptr = self._prepare(inputs, training)
+    def call(self, inputs: GraphGlobalExchangeInput, training: bool = False, shard=None):
+        x, g, index, graph_ptr = self._prepare(inputs, training, shard)
         H = self._hidden_dim
         W1, W2 = self._mlp.kernels[0].value, self._mlp.kernels[1].value
         needs_grad = node_ops._needs_grad(x, g, W1, W2)
         if needs_grad and index is None:
             # tf.concat([per_node_graph_representations, node_embeddings], -1) -> MLP (graph_global_exchange.py:176-181)
-            return self._mlp(torch.cat([g, x], dim=-1), training, self.dropout_state)
+            return self._mlp(torch.cat([g, x], dim=-1), training, self.dropout_state,
+                             shard.rows if shard is not None else None)
         # first layer split by rows: [g || x] W1 = g W1[:H] + x W1[H:]; the graph half once per graph (or per node when the
         # training-time dropout already materialised per-node copies: index is None then).  The slices of W1 are views: under
         # autograd the two halves' gradients land in the one variable.

@@ -8,6 +8,7 @@ cutting the gradient (ADVICE r1: "training through the GNN stack silently trunca
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
@@ -79,16 +80,16 @@ def dense(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor] = None,
 
 
 def mlp(x: torch.Tensor, kernels, biases=None, hidden_activation=None, training: bool = False, dropout_rate: float = 0.0,
-        rng: Optional["DropoutState"] = None) -> torch.Tensor:
+        rng: Optional["DropoutState"] = None, rows=None) -> torch.Tensor:
     """dpu_utils.tf2utils.MLP: hidden Dense layers with `hidden_activation` (ReLU by default), linear output layer;
-    under training, dropout on the input of every layer."""
+    under training, dropout on the input of every layer (`rows`: see dropout)."""
     from ..utils.param_helpers import get_activation_function
     act = hidden_activation or get_activation_function("relu")
     cur = x
     n = len(kernels)
     for i, W in enumerate(kernels):
         if training and dropout_rate > 0.0:
-            cur = dropout(cur, dropout_rate, rng)
+            cur = dropout(cur, dropout_rate, rng, rows)
         b = biases[i] if biases is not None else None
         cur = dense(cur, W, b, act if i < n - 1 else None)
     return cur
@@ -180,35 +181,52 @@ class DropoutState:
 _default_dropout_state = DropoutState(0x5EED)
 
 
-def _dropout_apply(x, rate, seed, offset):
+def _dropout_apply(x, rate, seed, offset, first=0):
     out = torch.empty_like(x)
-    _ffi.check(_ffi.lib().tfgnn_b200_dropout(x.data_ptr(), x.numel(), float(rate), seed, offset, out.data_ptr(),
-                                             stream_ptr()))
+    if first:
+        _ffi.check(_ffi.lib().tfgnn_b200_dropout_at(x.data_ptr(), x.numel(), float(rate), seed, offset, first,
+                                                    out.data_ptr(), stream_ptr()))
+    else:
+        _ffi.check(_ffi.lib().tfgnn_b200_dropout(x.data_ptr(), x.numel(), float(rate), seed, offset, out.data_ptr(),
+                                                 stream_ptr()))
     return out
 
 
 class _DropoutFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, rate, seed, offset):
-        ctx.cfg = (rate, seed, offset)
-        return _dropout_apply(x, rate, seed, offset)
+    def forward(ctx, x, rate, seed, offset, first):
+        ctx.cfg = (rate, seed, offset, first)
+        return _dropout_apply(x, rate, seed, offset, first)
 
     @staticmethod
     def backward(ctx, grad_out):
-        rate, seed, offset = ctx.cfg
-        return _dropout_apply(grad_out.contiguous(), rate, seed, offset), None, None, None
+        rate, seed, offset, first = ctx.cfg
+        return _dropout_apply(grad_out.contiguous(), rate, seed, offset, first), None, None, None, None
 
 
-def dropout(x: torch.Tensor, rate: float, state: Optional[DropoutState] = None) -> torch.Tensor:
-    """tf.nn.dropout(x, rate) (gnn.py:285-289).  rate == 0 is the identity, as in TensorFlow."""
+def dropout(x: torch.Tensor, rate: float, state: Optional[DropoutState] = None, rows=None) -> torch.Tensor:
+    """tf.nn.dropout(x, rate) (gnn.py:285-289).  rate == 0 is the identity, as in TensorFlow.
+
+    rows=(first_row, total_rows): x is rows [first_row, first_row + len(x)) of a [total_rows, C] table (a target-range
+    shard, sharding.TargetRangeShard.rows).  The call then consumes the stream of the whole table and draws exactly the
+    masks the unsharded call draws for those rows, so every rank of a sharded model stays in step with the unsharded run."""
     if rate <= 0.0:
         return x
     state = state or _default_dropout_state
     x = x.contiguous()
-    offset = state.take(x.numel())
+    first = 0
+    if rows is None:
+        offset = state.take(x.numel())
+    else:
+        cols = math.prod(int(n) for n in x.shape[1:])
+        if not 0 <= int(rows[0]) <= int(rows[0]) + int(x.shape[0]) <= int(rows[1]):
+            raise ValueError(f"dropout rows={tuple(rows)}: rows [{int(rows[0])}, {int(rows[0]) + int(x.shape[0])}) of x "
+                             f"must lie inside a table of {int(rows[1])} rows")
+        first = int(rows[0]) * cols
+        offset = state.take(int(rows[1]) * cols)
     if _needs_grad(x):
-        return _DropoutFunction.apply(x, float(rate), state.seed, offset)
-    return _dropout_apply(x, float(rate), state.seed, offset)
+        return _DropoutFunction.apply(x, float(rate), state.seed, offset, first)
+    return _dropout_apply(x, float(rate), state.seed, offset, first)
 
 
 # ---- graph-level primitives (forward only) ----------------------------------------------------------------------

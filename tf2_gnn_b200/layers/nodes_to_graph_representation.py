@@ -52,10 +52,10 @@ class _MLP:
     def variables(self) -> List[Variable]:
         return self.kernels + (self.biases or [])
 
-    def __call__(self, x: torch.Tensor, training: bool = False, rng=None) -> torch.Tensor:
+    def __call__(self, x: torch.Tensor, training: bool = False, rng=None, rows=None) -> torch.Tensor:
         return node_ops.mlp(x, [k.value for k in self.kernels],
                             [b.value for b in self.biases] if self.biases else None, self.activation, training,
-                            self.dropout_rate, rng)
+                            self.dropout_rate, rng, rows)
 
 
 class NodesToGraphRepresentation:
@@ -65,10 +65,10 @@ class NodesToGraphRepresentation:
         self._graph_representation_size = int(graph_representation_size)
         self.built = False
 
-    def __call__(self, inputs: NodesToGraphRepresentationInput, training: bool = False):
+    def __call__(self, inputs: NodesToGraphRepresentationInput, training: bool = False, **kwargs):
         if not self.built:
             self.build(NodesToGraphRepresentationInput(tuple(inputs.node_embeddings.shape), None, None))
-        return self.call(inputs, training=training)
+        return self.call(inputs, training=training, **kwargs)
 
 
 class WeightedSumGraphRepresentation(NodesToGraphRepresentation):
@@ -116,7 +116,12 @@ class WeightedSumGraphRepresentation(NodesToGraphRepresentation):
 
     trainable_variables = variables
 
-    def call(self, inputs: NodesToGraphRepresentationInput, training: bool = False, graph_ptr=None):
+    def call(self, inputs: NodesToGraphRepresentationInput, training: bool = False, graph_ptr=None, shard=None):
+        """shard (sharding.TargetRangeShard): node_embeddings and node_to_graph_map are the rank's rows [lo, hi) (global
+        graph ids), num_graphs the global count; the result [num_graphs, size] is merged over the ranks in rank order and is
+        the same on every rank.  Collective, forward and backward (see graph_autograd.shard_readout)."""
+        if shard is not None:
+            return self._call_shard(inputs, training, graph_ptr, shard)
         x = to_device_f32(inputs.node_embeddings)
         n2g = inputs.node_to_graph_map
         if not isinstance(n2g, torch.Tensor):
@@ -142,6 +147,29 @@ class WeightedSumGraphRepresentation(NodesToGraphRepresentation):
         node_ops.clamp_(reprs, lower, upper)
         return node_ops.weighted_segment_sum(reprs, weights, graph_ptr, self._num_heads,      # (3) aggregate by graph
                                              mean=self._weighting_fun == "average")
+
+    def _call_shard(self, inputs: NodesToGraphRepresentationInput, training: bool, graph_ptr, shard):
+        if self._weighting_fun == "average":
+            raise NotImplementedError("WeightedSumGraphRepresentation: average weighting is not built for target-range shards")
+        x = to_device_f32(inputs.node_embeddings)
+        n2g = inputs.node_to_graph_map
+        if not isinstance(n2g, torch.Tensor):
+            n2g = torch.as_tensor(n2g)
+        n2g = n2g.to(device=x.device, dtype=torch.int32).contiguous()
+        if int(x.shape[0]) != shard.hi - shard.lo or int(n2g.shape[0]) != shard.hi - shard.lo:
+            raise ValueError(f"a shard's node_embeddings and node_to_graph_map hold its {shard.hi - shard.lo} rows, got "
+                             f"{int(x.shape[0])} and {int(n2g.shape[0])}")
+        num_graphs = int(inputs.num_graphs)
+        if graph_ptr is None:
+            graph_ptr = node_ops.graph_offsets(n2g, num_graphs)
+        scores = None
+        if self._weighting_fun != "none":
+            scores = self._scoring_mlp(x, training, self.dropout_state, shard.rows)
+        reprs = self._transformation_mlp(x, training, self.dropout_state, shard.rows)
+        reprs = differentiable.activation(reprs, self._transformation_mlp_activation_fun)
+        return graph_autograd.shard_readout(scores, reprs, n2g, graph_ptr, num_graphs, self._num_heads, self._weighting_fun,
+                                            self._transformation_mlp_result_lower_bound,
+                                            self._transformation_mlp_result_upper_bound, shard)
 
 
 class WASGraphRepresentation(NodesToGraphRepresentation):

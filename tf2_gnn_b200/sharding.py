@@ -14,7 +14,8 @@ Two cases, both with host-side index bookkeeping only (numpy; bit-exact, tested 
    Training (DESIGN.md §6): gather_node_states is the differentiable all-gather, its backward the
    reduce-scatter reduce_scatter_node_grads; regather_saved_tables() keeps only a rank's own rows of
    every gathered table until backward.  Weight gradients come out partial per rank: sum them with
-   torch.distributed.all_reduce before the optimiser step.
+   sum_gradients_over_ranks (or torch.distributed.all_reduce) before the optimiser step.  A whole GNN, readout and
+   global exchange included, runs on a TargetRangeShard (section 2c).
 """
 from __future__ import annotations
 
@@ -128,6 +129,22 @@ def assemble_gathered(gathered: np.ndarray, bounds: Sequence[Tuple[int, int]]) -
     return np.concatenate(parts, axis=0) if parts else gathered[:0]
 
 
+# ------------------------------------------------------------------------------------------------
+# the two collectives every function of this module goes through.  A caller may replace them (module attributes), e.g. with
+# host-staged versions over gloo for several ranks on one device, where NCCL refuses to run.
+# ------------------------------------------------------------------------------------------------
+def all_gather_into_tensor(out, inp, group=None) -> None:
+    """out [world * n, ...] = every rank's inp [n, ...], in rank order."""
+    import torch.distributed as dist
+    dist.all_gather_into_tensor(out, inp, group=group)
+
+
+def reduce_scatter_tensor(out, inp, group=None) -> None:
+    """out [n, ...] = the sum over ranks of block `rank` of inp [world * n, ...]."""
+    import torch.distributed as dist
+    dist.reduce_scatter_tensor(out, inp, op=dist.ReduceOp.SUM, group=group)
+
+
 def all_gather_node_states(h_local, bounds: Sequence[Tuple[int, int]], group=None):
     """torch tensors on any device/backend: all-gather the per-rank row ranges into the full [V, D] table."""
     import torch
@@ -140,7 +157,7 @@ def all_gather_node_states(h_local, bounds: Sequence[Tuple[int, int]], group=Non
         send = torch.zeros((rows, D), dtype=h_local.dtype, device=h_local.device)
         send[: h_local.shape[0]] = h_local
     recv = torch.empty((world * rows, D), dtype=h_local.dtype, device=h_local.device)
-    dist.all_gather_into_tensor(recv, send.contiguous(), group=group)
+    all_gather_into_tensor(recv, send.contiguous(), group)
     if all((hi - lo) == rows for lo, hi in bounds):
         return recv
     return torch.cat([recv[r * rows: r * rows + (hi - lo)] for r, (lo, hi) in enumerate(bounds)], dim=0)
@@ -165,7 +182,7 @@ def reduce_scatter_node_grads(partial_full, bounds: Sequence[Tuple[int, int]], g
         for r, (lo, hi) in enumerate(bounds):
             send[r * rows: r * rows + (hi - lo)] = partial_full[lo:hi]
     recv = torch.empty((rows, D), dtype=partial_full.dtype, device=partial_full.device)
-    dist.reduce_scatter_tensor(recv, send, op=dist.ReduceOp.SUM, group=group)
+    reduce_scatter_tensor(recv, send, group)
     lo, hi = bounds[rank]
     return recv[: hi - lo]
 
@@ -229,6 +246,84 @@ class regather_saved_tables(torch.autograd.graph.saved_tensors_hooks):
 
     def _unpack(self, saved):
         return saved.gather() if isinstance(saved, _Regather) else saved
+
+
+# ------------------------------------------------------------------------------------------------
+# 2c. a model on target-range shards: per-graph values and weight gradients the same on every rank
+# ------------------------------------------------------------------------------------------------
+class TargetRangeShard:
+    """One rank's part of a graph cut by target range: `bounds[r] = (lo_r, hi_r)` for every rank r of `group` (contiguous,
+    covering [0, num_nodes)), this process is `rank`.  Pass it as `shard=` to GNN, WeightedSumGraphRepresentation and the
+    GraphGlobal*Exchange layers; they then take the rank's rows [lo, hi) of every node table."""
+
+    def __init__(self, bounds: Sequence[Tuple[int, int]], rank: int, group=None):
+        self.bounds = tuple((int(lo), int(hi)) for lo, hi in bounds)
+        if not self.bounds or self.bounds[0][0] != 0 or any(a[1] != b[0] for a, b in zip(self.bounds, self.bounds[1:])):
+            raise ValueError(f"shard bounds must be contiguous ranges starting at 0, got {self.bounds}")
+        if any(hi < lo for lo, hi in self.bounds):
+            raise ValueError(f"shard bounds must have lo <= hi, got {self.bounds}")
+        self.rank = int(rank)
+        if not 0 <= self.rank < len(self.bounds):
+            raise ValueError(f"rank {rank} outside a world of {len(self.bounds)}")
+        self.group = group
+        self.lo, self.hi = self.bounds[self.rank]
+        self.num_nodes = self.bounds[-1][1]
+        self.world_size = len(self.bounds)
+
+    @property
+    def rows(self) -> Tuple[int, int]:
+        """(first global row, rows of the whole table): what node_ops.dropout takes to draw the unsharded masks."""
+        return self.lo, self.num_nodes
+
+    def __repr__(self) -> str:
+        return f"TargetRangeShard(bounds={self.bounds}, rank={self.rank})"
+
+
+def all_gather_stacked(t, group=None):
+    """[world, *t.shape]: every rank's t (the same shape on every rank), in rank order."""
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    flat = t.contiguous().reshape(-1)
+    out = torch.empty((world * flat.numel(),), dtype=t.dtype, device=t.device)
+    if flat.numel():
+        all_gather_into_tensor(out, flat, group)
+    return out.view((world,) + tuple(t.shape))
+
+
+def sum_in_rank_order(stacked):
+    """stacked[0] + stacked[1] + ... added left to right on the device (tfgnn_b200_axpby): every rank that holds the same
+    gathered parts gets the same bits, whatever the collective backend's own reduction order."""
+    from .layers.node_ops import _axpby
+    acc = stacked[0].contiguous()
+    if int(stacked.shape[0]) == 1:
+        return acc.clone()
+    for r in range(1, int(stacked.shape[0])):
+        acc = _axpby(acc, 1.0, stacked[r].contiguous(), 1.0)
+    return acc
+
+
+def sum_over_ranks(t, group=None):
+    """The sum over ranks of every rank's t, added in rank order: bitwise the same on every rank."""
+    return sum_in_rank_order(all_gather_stacked(t, group))
+
+
+def sum_gradients_over_ranks(variables, group=None) -> None:
+    """After a backward on target-range shards every weight gradient is the rank's part.  Replace each variable's `.grad`
+    by the sum over ranks, added in rank order (one all-gather of all gradients, then a fixed-order sum on the device), so
+    that every rank holds the same bits before the optimiser step.  A variable without a gradient on a rank counts as zeros
+    there; every rank must pass the same variables in the same order.  `variables`: tensors or objects with `.value`."""
+    tensors = [getattr(v, "value", v) for v in variables]
+    if not tensors:
+        return
+    dev = tensors[0].device
+    flat = torch.cat([(t.grad if t.grad is not None else torch.zeros_like(t)).reshape(-1).to(torch.float32)
+                      for t in tensors]).to(dev)
+    total = sum_over_ranks(flat, group)
+    off = 0
+    for t in tensors:
+        n = t.numel()
+        t.grad = total[off: off + n].view_as(t).to(t.dtype).clone()
+        off += n
 
 
 # ------------------------------------------------------------------------------------------------

@@ -13,6 +13,14 @@ forward, reduce-scatter backward) under sharding.regather_saved_tables() (a rank
 input until backward), weight gradients summed with all_reduce.  Rank 0 checks the input and weight gradients against
 unsharded autograd on its own GPU; the JSON line reports ms per step (max over ranks) and each rank's peak
 torch.cuda.max_memory_allocated.
+
+With --stack every step trains a whole GNN (GNN.get_default_hyperparameters(): RGCN layers, a GRU global exchange every
+second layer with its readout merged over the ranks in rank order; every step restarts the dropout stream so that rank 0
+can compare with the same masks) on the
+rank's target range (`GNN(..., shard=sharding.TargetRangeShard(bounds, rank))`), sums the weight gradients with
+sharding.sum_gradients_over_ranks and checks on rank 0 the output rows and every gradient against unsharded autograd, and
+that every rank holds the same weight-gradient bits.  The graph is --graphs graphs of equal size, so that cuts fall inside
+graphs.  Multi-GPU step times of this mode are reported by the tool but have not been measured for the documentation.
 """
 import argparse
 import json
@@ -38,6 +46,8 @@ def main():
     ap.add_argument("--layers", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--train", action="store_true", help="forward + backward per step (gradient check on rank 0)")
+    ap.add_argument("--stack", action="store_true", help="train a whole GNN stack with global exchange (check on rank 0)")
+    ap.add_argument("--graphs", type=int, default=64, help="--stack: number of equal-size graphs in the node table")
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
@@ -52,6 +62,8 @@ def main():
     deg = sum(np.bincount(a[:, 1], minlength=V) for a in adjs)
     bounds = sharding.partition_target_range(V, world, deg)
     lo, hi = bounds[rank]
+    if args.stack:
+        return train_stack(args, rank, world, bounds, adjs, h0)
     adj_dev = tuple(torch.from_numpy(a).cuda() for a in adjs)
     params = RGCN.get_default_hyperparameters()
     params["hidden_dim"] = H
@@ -166,6 +178,80 @@ def train(args, rank, world, bounds, layers, adj_dev, shard, h0, h_local0):
                           "max_rel_err_grad_h": err_h, "max_rel_err_grad_w": err_w, "ok": ok,
                           "ms_per_step_max_over_ranks": float(t.item()),
                           "max_memory_allocated_per_rank": [int(p.item()) for p in peaks]}), flush=True)
+    dist.barrier()
+    dist.destroy_process_group()
+    if not ok:
+        raise SystemExit(1)
+
+
+def train_stack(args, rank, world, bounds, adjs, h0):
+    from tf2_gnn_b200.layers import GNN, GNNInput
+    V, H = args.nodes, args.hidden
+    G = args.graphs
+    n2g = np.minimum(np.arange(V, dtype=np.int64) * G // V, G - 1).astype(np.int32)
+    shard = sharding.TargetRangeShard(bounds, rank)
+    lo, hi = shard.lo, shard.hi
+    params = GNN.get_default_hyperparameters()
+    params.update(hidden_dim=H, layer_input_dropout_rate=0.0, global_exchange_dropout_rate=0.0)
+    torch.manual_seed(0)                                  # the same weights on every rank
+    gnn = GNN(params)
+    gnn.build(GNNInput((None, H), tuple((None, 2) for _ in adjs), None, None))
+    for v in gnn.variables:
+        v.requires_grad_(True)
+    adj_dev = tuple(torch.from_numpy(a).cuda() for a in sharding.filter_edges_by_target(adjs, lo, hi))
+    g_full = torch.from_numpy(np.random.default_rng(8).random((V, H), dtype=np.float32) * 2 - 1).cuda()
+    x0 = torch.from_numpy(h0[lo:hi]).cuda()
+    n2g_local = torch.from_numpy(n2g[lo:hi]).cuda()
+
+    def step():
+        for v in gnn.variables:
+            v.value.grad = None
+        gnn.dropout_state.offset = 0                      # the readout MLPs' dropout: the same masks every step
+        x = x0.clone().requires_grad_()
+        with sharding.regather_saved_tables():
+            out = gnn(GNNInput(x, adj_dev, n2g_local, G), training=True, shard=shard)
+        out.backward(g_full[lo:hi])
+        sharding.sum_gradients_over_ranks(gnn.variables)
+        return out.detach(), x.grad
+
+    step()
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    dist.barrier()
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    for _ in range(args.steps):
+        out_local, grad_local = step()
+    ev1.record()
+    torch.cuda.synchronize()
+    t = torch.tensor([ev0.elapsed_time(ev1) / args.steps], device="cuda")
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    out_full = sharding.all_gather_node_states(out_local, bounds)
+    grad_h = sharding.all_gather_node_states(grad_local, bounds)
+    flat = torch.cat([v.value.grad.reshape(-1) for v in gnn.variables])
+    same_bits = bool(torch.equal(sharding.all_gather_stacked(flat).amax(0), sharding.all_gather_stacked(flat).amin(0)))
+    ok = True
+    if rank == 0:
+        sharded_w = [v.value.grad.clone() for v in gnn.variables]
+        for v in gnn.variables:
+            v.value.grad = None
+        gnn.dropout_state.offset = 0
+        x = torch.from_numpy(h0).cuda().requires_grad_()
+        out = gnn(GNNInput(x, tuple(torch.from_numpy(a).cuda() for a in adjs), torch.from_numpy(n2g).cuda(), G),
+                  training=True)
+        out.backward(g_full)
+
+        def rel(a, b):
+            return float((a - b).norm() / b.norm().clamp(min=1e-30))
+
+        err_out, err_h = rel(out_full, out.detach()), rel(grad_h, x.grad)
+        err_w = max(rel(a, v.value.grad) for a, v in zip(sharded_w, gnn.variables))
+        ok = err_out <= 3e-5 and err_h <= 3e-5 and err_w <= 3e-5 and same_bits
+        print(json.dumps({"check": "target-range sharded GNN stack training == unsharded autograd", "world_size": world,
+                          "nodes": V, "graphs": G, "edges": len(adjs) * args.edges_per_type, "hidden": H,
+                          "rel_err_out": err_out, "rel_err_grad_h": err_h, "max_rel_err_grad_w": err_w,
+                          "weight_grads_same_bits_on_every_rank": same_bits, "ok": ok,
+                          "ms_per_step_max_over_ranks": float(t.item())}), flush=True)
     dist.barrier()
     dist.destroy_process_group()
     if not ok:
