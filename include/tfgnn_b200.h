@@ -491,6 +491,60 @@ TFGNN_API int tfgnn_b200_gru_gate_bwd_indexed(const float* gx, const int32_t* no
                                               int32_t num_graphs, int32_t H, float* grad_gx, float* grad_gh,
                                               float* grad_h_direct, void* stream);
 
+/* ---- Task losses and the optimizer step (tf2_gnn/models, SURVEY.md row 13) -------------------------------------------
+ * Each loss has a forward and a backward entry.  The forward writes its scalars to device memory; the backward reads the
+ * upstream scalar gradient grad_loss (one float) from device memory, so a training step never waits on the host.  Sums run
+ * over fixed 4096-element chunks (row-major: whole rows in row order) whose partials are combined in chunk order: no float
+ * atomics, every result a function of its inputs alone.  An empty batch gives a NaN loss (tf.reduce_mean of nothing) and
+ * zero counts; its backward is a no-op.
+ *   node_multiclass_loss   logits, labels [V, C] (0/1 float; node_multiclass_task.py:57-70):
+ *                            loss = (1/V) sum_v sum_c max(x,0) - x y + log1p(exp(-|x|))
+ *                            f1_counts int64[3] = (tp, fp, fn) of the prediction rint(sigmoid(x)) (a logit of 0 predicts 0)
+ *                            f1_score = 2 P R / (P + R), P = tp / (tp + fp), R = tp / (tp + fn) in float64 (NaN when tp == 0)
+ *                            grad_logits = g (sigmoid(x) - y) / V
+ *   graph_regression_loss  pred, target [G] (graph_regression_task.py:152-166): mse = mean (p-t)^2, mae = mean |p-t|;
+ *                            grad_pred = g 2 (p - t) / G
+ *   graph_binary_loss      prob = sigmoid(x), target [G] (graph_binary_classification_task.py:33-58), Keras
+ *                          binary_crossentropy(from_logits=False), TF >= 2.2: q = clip(p, 1e-7, 1 - 1e-7),
+ *                            loss = -mean[t log(q + 1e-7) + (1 - t) log(1 - q + 1e-7)], num_correct int64[1] = #(t == rint(p));
+ *                            grad_prob is zero where the clip cut (p < 1e-7 or p > 1 - 1e-7) */
+TFGNN_API int tfgnn_b200_node_multiclass_loss_fwd(const float* logits, const float* labels, int64_t num_nodes,
+                                                  int32_t num_labels, float* loss, float* f1_score, int64_t* f1_counts,
+                                                  void* stream);
+TFGNN_API int tfgnn_b200_node_multiclass_loss_bwd(const float* logits, const float* labels, int64_t num_nodes,
+                                                  int32_t num_labels, const float* grad_loss, float* grad_logits,
+                                                  void* stream);
+TFGNN_API int tfgnn_b200_graph_regression_loss_fwd(const float* pred, const float* target, int64_t num_graphs,
+                                                   float* mse, float* mae, void* stream);
+TFGNN_API int tfgnn_b200_graph_regression_loss_bwd(const float* pred, const float* target, int64_t num_graphs,
+                                                   const float* grad_loss, float* grad_pred, void* stream);
+TFGNN_API int tfgnn_b200_graph_binary_loss_fwd(const float* prob, const float* target, int64_t num_graphs, float* loss,
+                                               int64_t* num_correct, void* stream);
+TFGNN_API int tfgnn_b200_graph_binary_loss_bwd(const float* prob, const float* target, int64_t num_graphs,
+                                               const float* grad_loss, float* grad_prob, void* stream);
+
+/* One optimizer step over num_tensors variables (graph_task_model.py:224-324): Keras optimizer_v2 with epsilon 1e-7,
+ * beta_1 0.9, beta_2 0.999, each rule as TF's training-op functor writes it.  params, grads, slot_a, slot_b and sizes are
+ * HOST arrays of num_tensors entries (device pointers, element counts); the table goes to the device through the call's
+ * pool buffer and ONE launch updates every tensor.  A size of 0 skips the tensor (its pointers may be NULL).
+ *   SGD       momentum > 0: a = a momentum - lr g; w += a (slot_a = accumulator).  momentum == 0: w -= lr g (no slots)
+ *   RMSPROP   a += (g^2 - a)(1 - rho) (slot_a = mean square); momentum > 0: b = momentum b + lr g / sqrt(a + eps), w -= b
+ *             (slot_b); momentum == 0: w -= lr g / (sqrt(a) + eps)
+ *   ADAM      t = step + 1 (step = Keras' 0-based iterations), alpha = lr sqrt(1 - beta_2^t) / (1 - beta_1^t);
+ *             a += (g - a)(1 - beta_1); b += (g^2 - b)(1 - beta_2); w -= alpha a / (sqrt(b) + eps)
+ * The gradient is first clipped (clip_mode, clip = c):
+ *   VALUE        clip(g, -c, c)
+ *   NORM         per tensor: g c / max(||g||, c)
+ *   GLOBAL_NORM  g c min(1 / gn, 1 / c), gn = sqrt(sum over tensors of ||g||^2); a non-finite gn gives NaN (as TF)
+ * Norms add one reduction launch before the update: per-chunk sums of squares (4096-element chunks) written to device
+ * memory, combined by the update in chunk order per tensor and, for the global norm, in tensor order.  The same gradients
+ * give the same bits on every call.  Slots are zero-initialised by the caller before the first step. */
+enum { TFGNN_OPT_SGD = 0, TFGNN_OPT_RMSPROP = 1, TFGNN_OPT_ADAM = 2 };
+enum { TFGNN_CLIP_NONE = 0, TFGNN_CLIP_VALUE = 1, TFGNN_CLIP_NORM = 2, TFGNN_CLIP_GLOBAL_NORM = 3 };
+TFGNN_API int tfgnn_b200_optimizer_step(int32_t kind, int32_t num_tensors, float* const* params, const float* const* grads,
+                                        float* const* slot_a, float* const* slot_b, const int64_t* sizes, float lr,
+                                        float momentum, float rho, int64_t step, int32_t clip_mode, float clip, void* stream);
+
 /* ---- On-device batch builder (SURVEY.md section 8f-2) ------------------------------------------------------
  * Bit-exact int32 bookkeeping of the data layer, so that a training loop never leaves the device between the
  * packed dataset and the layer call.

@@ -28,6 +28,8 @@ PREPARE_VALIDATE = 1
 PREPARE_TRANSPOSE = 2
 PREPARE_TRANSPOSE_OWNED = 4
 MAX_EDGE_TYPES = 32
+OPTIMIZER = {"sgd": 0, "rmsprop": 1, "adam": 2}
+CLIP_NONE, CLIP_VALUE, CLIP_NORM, CLIP_GLOBAL_NORM = 0, 1, 2, 3
 
 EXPORTED_SYMBOLS = (
     "tfgnn_b200_abi_version", "tfgnn_b200_last_error", "tfgnn_b200_prepare", "tfgnn_b200_prepare_sharded", "tfgnn_b200_free_batch",
@@ -48,6 +50,9 @@ EXPORTED_SYMBOLS = (
     "tfgnn_b200_segment_sum_rows", "tfgnn_b200_readout_bwd", "tfgnn_b200_gru_gate_bwd_indexed",
     "tfgnn_b200_gru_update_fwd", "tfgnn_b200_gru_update_bwd",
     "tfgnn_b200_dropout_at", "tfgnn_b200_readout_partial", "tfgnn_b200_readout_merge",
+    "tfgnn_b200_node_multiclass_loss_fwd", "tfgnn_b200_node_multiclass_loss_bwd", "tfgnn_b200_graph_regression_loss_fwd",
+    "tfgnn_b200_graph_regression_loss_bwd", "tfgnn_b200_graph_binary_loss_fwd", "tfgnn_b200_graph_binary_loss_bwd",
+    "tfgnn_b200_optimizer_step",
 )
 
 _PP = POINTER(c_void_p)
@@ -164,6 +169,15 @@ def lib() -> ctypes.CDLL:
                                          c_void_p]
     L.tfgnn_b200_gru_gate_bwd_indexed.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                                   c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.tfgnn_b200_node_multiclass_loss_fwd.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p,
+                                                      c_void_p]
+    L.tfgnn_b200_node_multiclass_loss_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]
+    L.tfgnn_b200_graph_regression_loss_fwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
+    L.tfgnn_b200_graph_regression_loss_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
+    L.tfgnn_b200_graph_binary_loss_fwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
+    L.tfgnn_b200_graph_binary_loss_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
+    L.tfgnn_b200_optimizer_step.argtypes = [c_int32, c_int32, _PP, _PP, _PP, _PP, POINTER(c_int64), c_float, c_float,
+                                            c_float, c_int64, c_int32, c_float, c_void_p]
     L.tfgnn_b200_set_l2_persist_mb.argtypes = [c_int32]
     L.tfgnn_b200_release_device_state.argtypes = []
     for name in EXPORTED_SYMBOLS:

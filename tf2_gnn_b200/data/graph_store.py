@@ -22,11 +22,29 @@ from ..runtime import require_cuda, stream_ptr
 
 class DeviceGraphStore:
     """graphs: sequence of samples with ``node_features`` ([n, F] array-like) and ``adjacency_lists`` (list of
-    num_edge_types arrays reshapeable to [e, 2], graph-local node ids), as ``GraphSample`` in graph_dataset.py:17-41."""
+    num_edge_types arrays reshapeable to [e, 2], graph-local node ids), as ``GraphSample`` in graph_dataset.py:17-41.
+    Optional labels, given by every sample or by none: ``node_labels`` ([n, C], e.g. PPI's PPIGraphSample) and
+    ``target_value`` (one float per graph, e.g. the JSONL property datasets); ``batch_labels`` assembles them."""
 
     def __init__(self, graphs: Sequence[Any], num_edge_types: int):
         self.device = require_cuda()
         self.num_edge_types = int(num_edge_types)
+        node_labels = [_get(s, "node_labels", None) for s in graphs]
+        targets = [_get(s, "target_value", None) for s in graphs]
+        for what, vals in (("node_labels", node_labels), ("target_value", targets)):
+            if any(v is None for v in vals) and any(v is not None for v in vals):
+                raise ValueError(f"{what} must be given for every graph or for none")
+        self.node_labels: Optional[torch.Tensor] = None
+        self.target_value: Optional[torch.Tensor] = None
+        self.num_node_target_labels: Optional[int] = None
+        if graphs and node_labels[0] is not None:
+            labels = [np.asarray(v, dtype=np.float32) for v in node_labels]
+            C = labels[0].reshape(len(labels[0]), -1).shape[1]
+            self.num_node_target_labels = int(C)
+            self.node_labels = torch.from_numpy(np.concatenate([l.reshape(-1, C) for l in labels], axis=0)).to(self.device)
+        if graphs and targets[0] is not None:
+            self.target_value = torch.from_numpy(np.asarray(targets, dtype=np.float32).reshape(-1)).to(self.device)
+        self._last_rows = None   # (graph ids, node source rows) of the last batch(): batch_labels gathers through them
         feats, node_counts = [], []
         edges: List[List[np.ndarray]] = [[] for _ in range(self.num_edge_types)]
         edge_counts = np.zeros((self.num_edge_types, len(graphs)), dtype=np.int64)
@@ -62,9 +80,7 @@ class DeviceGraphStore:
     def batch(self, graph_ids, with_node_features: bool = True) -> Dict[str, Any]:
         """batch_features of graph_dataset.py:226-246 as CUDA tensors: node_features, node_to_graph_map,
         num_graphs_in_batch, adjacency_list_{t}."""
-        ids_host = np.asarray(graph_ids, dtype=np.int32).reshape(-1)
-        if ids_host.size and (ids_host.min() < 0 or ids_host.max() >= self.num_graphs):
-            raise IndexError("graph id out of range")
+        ids_host = self._check_ids(graph_ids)
         dev = self.device
         Gb = int(ids_host.size)
         T = self.num_edge_types
@@ -94,9 +110,43 @@ class DeviceGraphStore:
                 _ffi.check(lib.tfgnn_b200_gather_rows(self.node_features.data_ptr(), int(self.node_features.shape[0]), F,
                                                       rows.data_ptr(), 1, Vb, nf.data_ptr(), stream_ptr()))
             features["node_features"] = nf
+            self._last_rows = (ids_host, rows)
         for t in range(T):
             features[f"adjacency_list_{t}"] = adj[t]
         return features
+
+    def batch_labels(self, graph_ids) -> Dict[str, Any]:
+        """batch_labels of graph_dataset.py:226-246 as CUDA tensors: ``node_labels`` [num_nodes_in_batch, C] gathered through
+        the node rows that assemble node_features, and ``target_value`` [num_graphs_in_batch] by graph id, for the labels
+        the store holds.  Call it after batch(graph_ids), whose node rows it reuses (otherwise it assembles them)."""
+        ids_host = self._check_ids(graph_ids)
+        labels: Dict[str, Any] = {}
+        lib = _ffi.lib()
+        if self.node_labels is not None:
+            if self._last_rows is None or not np.array_equal(self._last_rows[0], ids_host):
+                self.batch(ids_host)
+            rows = self._last_rows[1]
+            Vb, C = int(rows.shape[0]), int(self.node_labels.shape[1])
+            out = torch.empty((Vb, C), dtype=torch.float32, device=self.device)
+            if Vb:
+                _ffi.check(lib.tfgnn_b200_gather_rows(self.node_labels.data_ptr(), int(self.node_labels.shape[0]), C,
+                                                      rows.data_ptr(), 1, Vb, out.data_ptr(), stream_ptr()))
+            labels["node_labels"] = out
+        if self.target_value is not None:
+            Gb = int(ids_host.size)
+            out = torch.empty((Gb,), dtype=torch.float32, device=self.device)
+            if Gb:
+                ids = torch.from_numpy(ids_host).to(self.device, non_blocking=True)
+                _ffi.check(lib.tfgnn_b200_gather_rows(self.target_value.data_ptr(), self.num_graphs, 1, ids.data_ptr(), 1, Gb,
+                                                      out.data_ptr(), stream_ptr()))
+            labels["target_value"] = out
+        return labels
+
+    def _check_ids(self, graph_ids) -> np.ndarray:
+        ids_host = np.asarray(graph_ids, dtype=np.int32).reshape(-1)
+        if ids_host.size and (ids_host.min() < 0 or ids_host.max() >= self.num_graphs):
+            raise IndexError("graph id out of range")
+        return ids_host
 
 
 def greedy_batches(node_counts: Sequence[int], max_nodes_per_batch: int,
@@ -121,5 +171,10 @@ def greedy_batches(node_counts: Sequence[int], max_nodes_per_batch: int,
         yield np.asarray(cur, dtype=np.int32)
 
 
-def _get(sample, name):
-    return sample[name] if isinstance(sample, dict) else getattr(sample, name)
+_REQUIRED = object()
+
+
+def _get(sample, name, default=_REQUIRED):
+    if isinstance(sample, dict):
+        return sample[name] if default is _REQUIRED else sample.get(name, default)
+    return getattr(sample, name) if default is _REQUIRED else getattr(sample, name, default)
