@@ -514,6 +514,21 @@ TFGNN_API int tfgnn_b200_node_multiclass_loss_fwd(const float* logits, const flo
 TFGNN_API int tfgnn_b200_node_multiclass_loss_bwd(const float* logits, const float* labels, int64_t num_nodes,
                                                   int32_t num_labels, const float* grad_loss, float* grad_logits,
                                                   void* stream);
+/* The node loss of a batch cut by target range across `world` ranks (rank r holds num_rows_r of the batch's total_rows):
+ *   _partial    the pass of _fwd over the rank's rows: loss_sum float[1] = the raw sum (not divided), f1_counts int64[3]
+ *   _merge      loss_sums float[world], counts int64[world][3]: every rank's partial (e.g. all-gathered), in rank order.  One
+ *               thread adds them left to right in rank order and finishes as _fwd with total_rows: the same gathered inputs
+ *               give the same bits on every rank; world == 1 gives the bits of _fwd.  total_rows == 0: NaN loss.
+ *   _bwd_rows   grad_logits [num_rows, C] = g (sigmoid(x) - y) / total_rows: a rank's logits enter its own partial only */
+TFGNN_API int tfgnn_b200_node_multiclass_loss_partial(const float* logits, const float* labels, int64_t num_rows,
+                                                      int32_t num_labels, float* loss_sum, int64_t* f1_counts,
+                                                      void* stream);
+TFGNN_API int tfgnn_b200_node_multiclass_loss_merge(const float* loss_sums, const int64_t* counts, int32_t world,
+                                                    int64_t total_rows, float* loss, float* f1_score, int64_t* f1_counts,
+                                                    void* stream);
+TFGNN_API int tfgnn_b200_node_multiclass_loss_bwd_rows(const float* logits, const float* labels, int64_t num_rows,
+                                                       int32_t num_labels, int64_t total_rows, const float* grad_loss,
+                                                       float* grad_logits, void* stream);
 TFGNN_API int tfgnn_b200_graph_regression_loss_fwd(const float* pred, const float* target, int64_t num_graphs,
                                                    float* mse, float* mae, void* stream);
 TFGNN_API int tfgnn_b200_graph_regression_loss_bwd(const float* pred, const float* target, int64_t num_graphs,
@@ -588,6 +603,24 @@ TFGNN_API int tfgnn_b200_assemble_batch(const int64_t* node_offsets, const int64
                               int64_t num_nodes_in_batch, const int64_t* num_edges_in_batch,
                               int32_t* node_to_graph_map, int32_t* node_source_rows,
                               int32_t* const* adjacency_lists, void* workspace, void* stream);
+
+/* One rank's part of that batch on target-range shards: batch rows [row_begin, row_begin + row_count).  The arguments of
+ * tfgnn_b200_assemble_batch (the same workspace size), plus the window; row_begin + row_count <= num_nodes_in_batch.
+ *   node_to_graph_map, node_source_rows   out int32[row_count]: entries row_begin ... of the whole batch's arrays (batch-level
+ *                        graph ids), or NULL
+ *   adjacency_lists[t]   out [num_edges_in_window[t], 2]: every edge of every graph that overlaps the window, in batch ids
+ *                        and in the order assemble_batch emits them: its sub-list [eoff[g_first], eoff[g_last + 1]) where
+ *                        g_first / g_last hold rows row_begin / row_begin + row_count - 1.  Edges of a boundary graph whose
+ *                        targets lie outside the window are included; tfgnn_b200_prepare_sharded with that target range
+ *                        drops them, so its CSR is the one of the edges filtered by target.
+ * An empty window writes nothing. */
+TFGNN_API int tfgnn_b200_assemble_batch_rows(const int64_t* node_offsets, const int64_t* const* edge_offsets,
+                                   const int32_t* const* edges, int32_t num_edge_types, int64_t num_graphs_total,
+                                   const int32_t* graph_ids, int32_t num_graphs_in_batch,
+                                   int64_t num_nodes_in_batch, const int64_t* num_edges_in_window,
+                                   int64_t row_begin, int64_t row_count, int32_t* node_to_graph_map,
+                                   int32_t* node_source_rows, int32_t* const* adjacency_lists, void* workspace,
+                                   void* stream);
 
 /* ---- Device-global state --------------------------------------------------------------------------------------
  * Two things in this library outlive a call and are shared with the host framework's CUDA context:

@@ -52,7 +52,8 @@ EXPORTED_SYMBOLS = (
     "tfgnn_b200_dropout_at", "tfgnn_b200_readout_partial", "tfgnn_b200_readout_merge",
     "tfgnn_b200_node_multiclass_loss_fwd", "tfgnn_b200_node_multiclass_loss_bwd", "tfgnn_b200_graph_regression_loss_fwd",
     "tfgnn_b200_graph_regression_loss_bwd", "tfgnn_b200_graph_binary_loss_fwd", "tfgnn_b200_graph_binary_loss_bwd",
-    "tfgnn_b200_optimizer_step",
+    "tfgnn_b200_optimizer_step", "tfgnn_b200_node_multiclass_loss_partial", "tfgnn_b200_node_multiclass_loss_merge",
+    "tfgnn_b200_node_multiclass_loss_bwd_rows", "tfgnn_b200_assemble_batch_rows",
 )
 
 _PP = POINTER(c_void_p)
@@ -126,6 +127,9 @@ def lib() -> ctypes.CDLL:
     L.tfgnn_b200_assemble_batch_workspace_bytes.restype = ctypes.c_size_t
     L.tfgnn_b200_assemble_batch.argtypes = [c_void_p, _PP, _PP, c_int32, c_int64, c_void_p, c_int32, c_int64,
                                             POINTER(c_int64), c_void_p, c_void_p, _PP, c_void_p, c_void_p]
+    L.tfgnn_b200_assemble_batch_rows.argtypes = [c_void_p, _PP, _PP, c_int32, c_int64, c_void_p, c_int32, c_int64,
+                                                 POINTER(c_int64), c_int64, c_int64, c_void_p, c_void_p, _PP, c_void_p,
+                                                 c_void_p]
     L.tfgnn_b200_graph_offsets.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p]
     L.tfgnn_b200_segment_softmax.argtypes = [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]
     L.tfgnn_b200_weighted_segment_sum.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
@@ -172,6 +176,12 @@ def lib() -> ctypes.CDLL:
     L.tfgnn_b200_node_multiclass_loss_fwd.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p,
                                                       c_void_p]
     L.tfgnn_b200_node_multiclass_loss_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]
+    L.tfgnn_b200_node_multiclass_loss_partial.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p,
+                                                          c_void_p]
+    L.tfgnn_b200_node_multiclass_loss_merge.argtypes = [c_void_p, c_void_p, c_int32, c_int64, c_void_p, c_void_p, c_void_p,
+                                                        c_void_p]
+    L.tfgnn_b200_node_multiclass_loss_bwd_rows.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_int64, c_void_p,
+                                                           c_void_p, c_void_p]
     L.tfgnn_b200_graph_regression_loss_fwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
     L.tfgnn_b200_graph_regression_loss_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
     L.tfgnn_b200_graph_binary_loss_fwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]

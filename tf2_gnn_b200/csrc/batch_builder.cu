@@ -104,32 +104,81 @@ __device__ __forceinline__ int find_graph(const long long* __restrict__ off, int
   return lo;
 }
 
-// node_to_graph_map[v] = g (batch-local index, graph_dataset.py:211-217); src_row[v] = the node's row in the packed store
+// node_to_graph_map[v] = g (batch-local index, graph_dataset.py:211-217); src_row[v] = the node's row in the packed store.
+// v counts from batch row v0: a row window [v0, v0 + Vb) of the batch (v0 = 0 for the whole batch).
 __global__ void fill_nodes_kernel(const long long* __restrict__ node_off_batch, int Gb,
                                   const long long* __restrict__ node_offsets, const int* __restrict__ graph_ids,
-                                  long long Vb, int* __restrict__ node_to_graph_map, int* __restrict__ src_row) {
+                                  long long v0, long long Vb, int* __restrict__ node_to_graph_map, int* __restrict__ src_row) {
   const long long total = node_off_batch[Gb];   // a caller-supplied size larger than the real batch is not followed
-  if (Vb > total) Vb = total;
-  for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < Vb; v += (long long)gridDim.x * blockDim.x) {
+  if (Vb > total - v0) Vb = total - v0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < Vb; i += (long long)gridDim.x * blockDim.x) {
+    const long long v = v0 + i;
     const int g = find_graph(node_off_batch, Gb, v);
-    if (node_to_graph_map) node_to_graph_map[v] = g;
-    if (src_row) src_row[v] = (int)(node_offsets[graph_ids[g]] + (v - node_off_batch[g]));
+    if (node_to_graph_map) node_to_graph_map[i] = g;
+    if (src_row) src_row[i] = (int)(node_offsets[graph_ids[g]] + (v - node_off_batch[g]));
   }
 }
 
-// adjacency_list_t[e] = stored pair + running node count of its graph (graph_dataset.py:218-222)
+// adjacency_list_t[e] = stored pair + running node count of its graph (graph_dataset.py:218-222).  With row_end >= 0 only
+// the edges of the graphs that overlap batch rows [row_begin, row_end) are written, from out[0] on and in batch order:
+// the sub-range [edge_off_batch[g_first], edge_off_batch[g_last + 1]) of the whole batch's list.
 __global__ void fill_edges_kernel(const long long* __restrict__ edge_off_batch, const long long* __restrict__ node_off_batch,
                                   int Gb, const long long* __restrict__ edge_offsets, const int* __restrict__ graph_ids,
-                                  const int2* __restrict__ edges, long long Eb, int2* __restrict__ out) {
-  const long long total = edge_off_batch[Gb];
-  if (Eb > total) Eb = total;
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < Eb; e += (long long)gridDim.x * blockDim.x) {
+                                  const int2* __restrict__ edges, long long row_begin, long long row_end, long long Eb,
+                                  int2* __restrict__ out) {
+  long long e0 = 0, e1 = edge_off_batch[Gb];
+  if (row_end >= 0) {
+    if (row_end > node_off_batch[Gb]) row_end = node_off_batch[Gb];
+    e0 = e1 = 0;
+    if (row_begin < row_end) {
+      e0 = edge_off_batch[find_graph(node_off_batch, Gb, row_begin)];
+      e1 = edge_off_batch[find_graph(node_off_batch, Gb, row_end - 1) + 1];
+    }
+  }
+  if (Eb > e1 - e0) Eb = e1 - e0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < Eb; i += (long long)gridDim.x * blockDim.x) {
+    const long long e = e0 + i;
     const int g = find_graph(edge_off_batch, Gb, e);
     const long long src_e = edge_offsets[graph_ids[g]] + (e - edge_off_batch[g]);
     const int shift = (int)node_off_batch[g];
     const int2 p = edges[src_e];
-    out[e] = make_int2(p.x + shift, p.y + shift);
+    out[i] = make_int2(p.x + shift, p.y + shift);
   }
+}
+
+// The launches of assemble_batch over batch rows [row_begin, row_end); row_end < 0: the whole batch.  Arguments checked.
+static int assemble_launch(const int64_t* node_offsets, const int64_t* const* edge_offsets, const int32_t* const* edges,
+                           int num_edge_types, int64_t num_graphs_total, const int32_t* graph_ids, int Gb,
+                           long long row_begin, long long row_end, long long num_rows, const int64_t* num_edges,
+                           int32_t* node_to_graph_map, int32_t* node_source_rows, int32_t* const* adjacency_lists,
+                           void* workspace, cudaStream_t st) {
+  OffsetTables tabs{};
+  tabs.t[0] = reinterpret_cast<const long long*>(node_offsets);
+  for (int t = 0; t < num_edge_types; ++t) {
+    TFGNN_REQUIRE(edge_offsets[t] != nullptr, "NULL edge offset table");
+    tabs.t[1 + t] = reinterpret_cast<const long long*>(edge_offsets[t]);
+  }
+  long long* ws = reinterpret_cast<long long*>(workspace);
+  batch_scan_kernel<<<num_edge_types + 1, 1024, 0, st>>>(tabs, graph_ids, Gb, num_graphs_total, ws);
+  TFGNN_LAUNCH_CHECK();
+  if (num_rows > 0 && (node_to_graph_map || node_source_rows)) {
+    fill_nodes_kernel<<<bb_grid(num_rows), 256, 0, st>>>(ws, Gb, reinterpret_cast<const long long*>(node_offsets),
+                                                       graph_ids, row_begin, num_rows, node_to_graph_map,
+                                                       node_source_rows);
+    TFGNN_LAUNCH_CHECK();
+  }
+  for (int t = 0; t < num_edge_types; ++t) {
+    const long long Eb = num_edges[t];
+    TFGNN_REQUIRE(Eb >= 0, "negative edge count");
+    if (Eb == 0) continue;
+    TFGNN_REQUIRE(edges[t] && adjacency_lists[t], "NULL edge list");
+    fill_edges_kernel<<<bb_grid(Eb), 256, 0, st>>>(ws + (size_t)(1 + t) * (Gb + 1), ws, Gb,
+                                                 reinterpret_cast<const long long*>(edge_offsets[t]), graph_ids,
+                                                 reinterpret_cast<const int2*>(edges[t]), row_begin, row_end, Eb,
+                                                 reinterpret_cast<int2*>(adjacency_lists[t]));
+    TFGNN_LAUNCH_CHECK();
+  }
+  return 0;
 }
 
 }  // namespace tfgnn
@@ -249,33 +298,30 @@ extern "C" int tfgnn_b200_assemble_batch(const int64_t* node_offsets, const int6
   if (num_graphs_in_batch == 0) return 0;
   TFGNN_REQUIRE(node_offsets && graph_ids && workspace, "NULL pointer");
   TFGNN_REQUIRE(num_edge_types == 0 || (edge_offsets && edges && adjacency_lists && num_edges_in_batch), "NULL edge tables");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Gb = num_graphs_in_batch;
-  OffsetTables tabs{};
-  tabs.t[0] = reinterpret_cast<const long long*>(node_offsets);
-  for (int t = 0; t < num_edge_types; ++t) {
-    TFGNN_REQUIRE(edge_offsets[t] != nullptr, "NULL edge offset table");
-    tabs.t[1 + t] = reinterpret_cast<const long long*>(edge_offsets[t]);
-  }
-  long long* ws = reinterpret_cast<long long*>(workspace);
-  batch_scan_kernel<<<num_edge_types + 1, 1024, 0, st>>>(tabs, graph_ids, Gb, num_graphs_total, ws);
-  TFGNN_LAUNCH_CHECK();
-  if (num_nodes_in_batch > 0 && (node_to_graph_map || node_source_rows)) {
-    fill_nodes_kernel<<<bb_grid(num_nodes_in_batch), 256, 0, st>>>(ws, Gb, reinterpret_cast<const long long*>(node_offsets),
-                                                                 graph_ids, num_nodes_in_batch, node_to_graph_map,
-                                                                 node_source_rows);
-    TFGNN_LAUNCH_CHECK();
-  }
-  for (int t = 0; t < num_edge_types; ++t) {
-    const long long Eb = num_edges_in_batch[t];
-    TFGNN_REQUIRE(Eb >= 0, "negative edge count");
-    if (Eb == 0) continue;
-    TFGNN_REQUIRE(edges[t] && adjacency_lists[t], "NULL edge list");
-    fill_edges_kernel<<<bb_grid(Eb), 256, 0, st>>>(ws + (size_t)(1 + t) * (Gb + 1), ws, Gb,
-                                                 reinterpret_cast<const long long*>(edge_offsets[t]), graph_ids,
-                                                 reinterpret_cast<const int2*>(edges[t]), Eb,
-                                                 reinterpret_cast<int2*>(adjacency_lists[t]));
-    TFGNN_LAUNCH_CHECK();
-  }
-  return 0;
+  return assemble_launch(node_offsets, edge_offsets, edges, num_edge_types, num_graphs_total, graph_ids,
+                         num_graphs_in_batch, 0, -1, num_nodes_in_batch, num_edges_in_batch, node_to_graph_map,
+                         node_source_rows, adjacency_lists, workspace, (cudaStream_t)stream);
+}
+
+extern "C" int tfgnn_b200_assemble_batch_rows(const int64_t* node_offsets, const int64_t* const* edge_offsets,
+                                              const int32_t* const* edges, int32_t num_edge_types, int64_t num_graphs_total,
+                                              const int32_t* graph_ids, int32_t num_graphs_in_batch,
+                                              int64_t num_nodes_in_batch, const int64_t* num_edges_in_window,
+                                              int64_t row_begin, int64_t row_count, int32_t* node_to_graph_map,
+                                              int32_t* node_source_rows, int32_t* const* adjacency_lists, void* workspace,
+                                              void* stream) {
+  TFGNN_REQUIRE(num_edge_types >= 0 && num_edge_types <= TFGNN_MAX_EDGE_TYPES,
+                "tfgnn_b200_assemble_batch_rows: too many edge types");
+  TFGNN_REQUIRE(num_graphs_in_batch >= 0 && num_graphs_total >= 0 && num_nodes_in_batch >= 0,
+                "tfgnn_b200_assemble_batch_rows: negative size");
+  TFGNN_REQUIRE(num_nodes_in_batch < (1ll << 31), "tfgnn_b200_assemble_batch_rows: batch has too many nodes for int32 ids");
+  TFGNN_REQUIRE(row_begin >= 0 && row_count >= 0 && row_begin + row_count <= num_nodes_in_batch,
+                "tfgnn_b200_assemble_batch_rows: row window outside the batch");
+  if (num_graphs_in_batch == 0 || row_count == 0) return 0;
+  TFGNN_REQUIRE(node_offsets && graph_ids && workspace, "tfgnn_b200_assemble_batch_rows: NULL pointer");
+  TFGNN_REQUIRE(num_edge_types == 0 || (edge_offsets && edges && adjacency_lists && num_edges_in_window),
+                "tfgnn_b200_assemble_batch_rows: NULL edge tables");
+  return assemble_launch(node_offsets, edge_offsets, edges, num_edge_types, num_graphs_total, graph_ids,
+                         num_graphs_in_batch, row_begin, row_begin + row_count, row_count, num_edges_in_window,
+                         node_to_graph_map, node_source_rows, adjacency_lists, workspace, (cudaStream_t)stream);
 }

@@ -171,6 +171,22 @@ int loss_fwd(const Op& op, long long n, float rows, const LossOut& out, cudaStre
   return 0;
 }
 
+// ---- the node loss on target-range shards --------------------------------------------------------------------------
+// One CTA, one thread: the ranks' raw sums and counts added left to right in rank order, then the finish of _fwd over
+// the batch's total row count.  Every rank that holds the same gathered partials writes the same bits.
+__global__ void node_multiclass_merge_kernel(const float* __restrict__ loss_sums, const long long* __restrict__ counts,
+                                             int world, float n, LossOut o) {
+  if (threadIdx.x != 0) return;
+  float f[NodeMulticlassOp::NF] = {loss_sums[0]};
+  long long c[NodeMulticlassOp::NI] = {counts[0], counts[1], counts[2]};
+  for (int r = 1; r < world; ++r) {
+    f[0] += loss_sums[r];
+#pragma unroll
+    for (int k = 0; k < NodeMulticlassOp::NI; ++k) c[k] += counts[(long long)r * NodeMulticlassOp::NI + k];
+  }
+  NodeMulticlassOp::finish(f, c, n, o);
+}
+
 // ---- backward ----------------------------------------------------------------------------------------------------
 // grad = g * (sigmoid(x) - y) / V
 __global__ void node_multiclass_bwd_kernel(const float* __restrict__ x, const float* __restrict__ y, long long n, float inv_V,
@@ -224,6 +240,48 @@ extern "C" int tfgnn_b200_node_multiclass_loss_bwd(const float* logits, const fl
   TFGNN_REQUIRE(logits && labels && grad_loss && grad_logits, "tfgnn_b200_node_multiclass_loss_bwd: NULL pointer");
   const long long n = num_nodes * num_labels;
   node_multiclass_bwd_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(logits, labels, n, 1.f / (float)num_nodes,
+                                                                          grad_loss, grad_logits);
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+// The pass of _fwd over a rank's rows, finished over one row: f[0] / 1.0f is the raw sum, exactly.
+extern "C" int tfgnn_b200_node_multiclass_loss_partial(const float* logits, const float* labels, int64_t num_rows,
+                                                       int32_t num_labels, float* loss_sum, int64_t* f1_counts,
+                                                       void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && num_labels > 0,
+                "tfgnn_b200_node_multiclass_loss_partial: bad sizes (num_labels must be > 0)");
+  TFGNN_REQUIRE(loss_sum && f1_counts && (num_rows == 0 || (logits && labels)),
+                "tfgnn_b200_node_multiclass_loss_partial: NULL pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  PoolBuffer unused_f1{st};   // the finish writes an F1 of the rank's counts; only the merged one is meaningful
+  int rc = unused_f1.alloc(sizeof(float));
+  if (rc) return rc;
+  NodeMulticlassOp op{logits, labels};
+  return loss_fwd(op, num_rows * num_labels, 1.f, LossOut{loss_sum, unused_f1.f(), (long long*)f1_counts}, st);
+}
+
+extern "C" int tfgnn_b200_node_multiclass_loss_merge(const float* loss_sums, const int64_t* counts, int32_t world,
+                                                     int64_t total_rows, float* loss, float* f1_score, int64_t* f1_counts,
+                                                     void* stream) {
+  TFGNN_REQUIRE(world >= 1 && total_rows >= 0,
+                "tfgnn_b200_node_multiclass_loss_merge: bad sizes (world must be >= 1, total_rows >= 0)");
+  TFGNN_REQUIRE(loss_sums && counts && loss && f1_score && f1_counts, "tfgnn_b200_node_multiclass_loss_merge: NULL pointer");
+  node_multiclass_merge_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(
+      loss_sums, (const long long*)counts, world, (float)total_rows, LossOut{loss, f1_score, (long long*)f1_counts});
+  TFGNN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int tfgnn_b200_node_multiclass_loss_bwd_rows(const float* logits, const float* labels, int64_t num_rows,
+                                                        int32_t num_labels, int64_t total_rows, const float* grad_loss,
+                                                        float* grad_logits, void* stream) {
+  TFGNN_REQUIRE(num_rows >= 0 && num_labels > 0 && total_rows >= num_rows,
+                "tfgnn_b200_node_multiclass_loss_bwd_rows: bad sizes (num_labels must be > 0, total_rows >= num_rows)");
+  if (num_rows == 0) return 0;
+  TFGNN_REQUIRE(logits && labels && grad_loss && grad_logits, "tfgnn_b200_node_multiclass_loss_bwd_rows: NULL pointer");
+  const long long n = num_rows * num_labels;
+  node_multiclass_bwd_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(logits, labels, n, 1.f / (float)total_rows,
                                                                           grad_loss, grad_logits);
   TFGNN_LAUNCH_CHECK();
   return 0;

@@ -6,17 +6,20 @@ running node count, ``node_to_graph_map`` a constant block per graph, empty edge
 reference rebuilds these arrays with Python loops for every batch; here the graphs are uploaded ONCE (all graphs of
 an edge type back to back, graph-local ids) and ``batch(graph_ids)`` launches ``tfgnn_b200_assemble_batch``
 (batch_builder.cu).  Only the greedy "which graphs fit" rule (:181-188) stays on the host: it needs node counts only.
+
+On target-range shards each rank assembles only its rows of a batch: ``shard_bounds`` cuts the batch (by the in-degree
+table the store keeps on the host) and ``shard_batch`` launches ``tfgnn_b200_assemble_batch_rows``.
 """
 from __future__ import annotations
 
 import ctypes
 from ctypes import c_int64, c_void_p
-from typing import Any, Dict, Iterator, List, Optional, Sequence
+from typing import Any, Dict, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
-from .. import _ffi
+from .. import _ffi, sharding
 from ..runtime import require_cuda, stream_ptr
 
 
@@ -45,6 +48,7 @@ class DeviceGraphStore:
         if graphs and targets[0] is not None:
             self.target_value = torch.from_numpy(np.asarray(targets, dtype=np.float32).reshape(-1)).to(self.device)
         self._last_rows = None   # (graph ids, node source rows) of the last batch(): batch_labels gathers through them
+        self._last_shard_rows = None   # (graph ids, lo, hi, node source rows) of the last shard_batch()
         feats, node_counts = [], []
         edges: List[List[np.ndarray]] = [[] for _ in range(self.num_edge_types)]
         edge_counts = np.zeros((self.num_edge_types, len(graphs)), dtype=np.int64)
@@ -63,6 +67,8 @@ class DeviceGraphStore:
         self.node_offsets_host = np.concatenate([[0], np.cumsum(node_counts, dtype=np.int64)]).astype(np.int64)
         self.edge_offsets_host = [np.concatenate([[0], np.cumsum(edge_counts[t])]).astype(np.int64)
                                   for t in range(self.num_edge_types)]
+        # in-degree of every stored node, summed over edge types: shard cuts need no device round trip either
+        self.in_degree_host = stored_in_degree(self.node_offsets_host, edges)
         dev = self.device
         self.node_features = torch.from_numpy(
             np.concatenate(feats, axis=0) if feats else np.zeros((0, 0), np.float32)).to(dev)
@@ -81,15 +87,57 @@ class DeviceGraphStore:
         """batch_features of graph_dataset.py:226-246 as CUDA tensors: node_features, node_to_graph_map,
         num_graphs_in_batch, adjacency_list_{t}."""
         ids_host = self._check_ids(graph_ids)
-        dev = self.device
         Gb = int(ids_host.size)
         T = self.num_edge_types
         no, eo = self.node_offsets_host, self.edge_offsets_host
         Vb = int((no[ids_host + 1] - no[ids_host]).sum()) if Gb else 0
         Eb = [int((eo[t][ids_host + 1] - eo[t][ids_host]).sum()) if Gb else 0 for t in range(T)]
+        features, rows = self._assemble(ids_host, Vb, Eb, None, with_node_features)
+        if with_node_features:
+            self._last_rows = (ids_host, rows)
+        return features
+
+    def shard_bounds(self, graph_ids, world_size: int) -> List[Tuple[int, int]]:
+        """Batch rows [(lo, hi)] per rank of the batch of graph_ids: sharding.partition_target_range over the batch's node
+        count, balanced by the in-degree of its nodes (all edge types).  Host tables only."""
+        ids_host = self._check_ids(graph_ids)
+        return shard_bounds_from_tables(self.node_offsets_host, self.in_degree_host, ids_host, world_size)
+
+    def shard_batch(self, graph_ids, shard, with_node_features: bool = True) -> Dict[str, Any]:
+        """A rank's part of batch(graph_ids) on target-range shards (sharding.TargetRangeShard over the batch's rows, e.g.
+        from shard_bounds), with the keys of batch(): node_features and node_to_graph_map (batch graph ids) of rows
+        [shard.lo, shard.hi), num_graphs_in_batch of the whole batch, and adjacency_list_{t} in batch node ids holding every
+        edge of the graphs that overlap those rows (tfgnn_b200_assemble_batch_rows).  Edges into other ranks' rows are
+        among them; GNN(shard=...) prepares only those into [lo, hi)."""
+        ids_host = self._check_ids(graph_ids)
+        T = self.num_edge_types
+        no, eo = self.node_offsets_host, self.edge_offsets_host
+        batch_off = np.concatenate([[0], np.cumsum(no[ids_host + 1] - no[ids_host])]).astype(np.int64)
+        Vb = int(batch_off[-1])
+        if shard.num_nodes != Vb:
+            raise ValueError(f"shard bounds cover {shard.num_nodes} rows, the batch has {Vb}")
+        lo, hi = shard.lo, shard.hi
+        Eb = [0] * T
+        if hi > lo:
+            g_first = int(np.searchsorted(batch_off, lo, side="right")) - 1   # the graphs holding rows lo and hi - 1
+            g_last = int(np.searchsorted(batch_off, hi - 1, side="right")) - 1
+            win = ids_host[g_first: g_last + 1]
+            Eb = [int((eo[t][win + 1] - eo[t][win]).sum()) for t in range(T)]
+        features, rows = self._assemble(ids_host, Vb, Eb, (lo, hi), with_node_features)
+        if with_node_features:
+            self._last_shard_rows = (ids_host, lo, hi, rows)
+        return features
+
+    def _assemble(self, ids_host: np.ndarray, Vb: int, Eb: List[int], window: Optional[Tuple[int, int]],
+                  with_node_features: bool):
+        """(features, node source rows): tfgnn_b200_assemble_batch, or _assemble_batch_rows over window = (lo, hi)."""
+        dev = self.device
+        Gb = int(ids_host.size)
+        T = self.num_edge_types
+        n = Vb if window is None else window[1] - window[0]
         ids = torch.from_numpy(ids_host).to(dev, non_blocking=True)
-        n2g = torch.empty((Vb,), dtype=torch.int32, device=dev)
-        rows = torch.empty((Vb,), dtype=torch.int32, device=dev) if with_node_features else None
+        n2g = torch.empty((n,), dtype=torch.int32, device=dev)
+        rows = torch.empty((n,), dtype=torch.int32, device=dev) if with_node_features else None
         adj = [torch.empty((Eb[t], 2), dtype=torch.int32, device=dev) for t in range(T)]
         lib = _ffi.lib()
         ws = torch.empty((max(int(lib.tfgnn_b200_assemble_batch_workspace_bytes(T, Gb)), 8),), dtype=torch.uint8, device=dev)
@@ -97,23 +145,30 @@ class DeviceGraphStore:
         edge_ptrs = (c_void_p * max(T, 1))(*[e.data_ptr() if e.numel() else None for e in self.edges])
         out_ptrs = (c_void_p * max(T, 1))(*[a.data_ptr() if a.numel() else None for a in adj])
         Eb_c = (c_int64 * max(T, 1))(*Eb)
-        _ffi.check(lib.tfgnn_b200_assemble_batch(
-            self.node_offsets.data_ptr(), ctypes.cast(eoff_ptrs, _ffi._PP), ctypes.cast(edge_ptrs, _ffi._PP), T,
-            self.num_graphs, ids.data_ptr() if Gb else None, Gb, Vb, Eb_c, n2g.data_ptr() if Vb else None,
-            rows.data_ptr() if (rows is not None and Vb) else None, ctypes.cast(out_ptrs, _ffi._PP), ws.data_ptr(),
-            stream_ptr()))
+        head = (self.node_offsets.data_ptr(), ctypes.cast(eoff_ptrs, _ffi._PP), ctypes.cast(edge_ptrs, _ffi._PP), T,
+                self.num_graphs, ids.data_ptr() if Gb else None, Gb, Vb, Eb_c)
+        tail = (n2g.data_ptr() if n else None, rows.data_ptr() if (rows is not None and n) else None,
+                ctypes.cast(out_ptrs, _ffi._PP), ws.data_ptr(), stream_ptr())
+        if window is None:
+            _ffi.check(lib.tfgnn_b200_assemble_batch(*head, *tail))
+        else:
+            _ffi.check(lib.tfgnn_b200_assemble_batch_rows(*head, window[0], n, *tail))
         features: Dict[str, Any] = {"node_to_graph_map": n2g, "num_graphs_in_batch": Gb}
         if with_node_features:
-            F = int(self.node_features.shape[1]) if self.node_features.dim() == 2 else 0
-            nf = torch.empty((Vb, F), dtype=torch.float32, device=dev)
-            if Vb and F:
-                _ffi.check(lib.tfgnn_b200_gather_rows(self.node_features.data_ptr(), int(self.node_features.shape[0]), F,
-                                                      rows.data_ptr(), 1, Vb, nf.data_ptr(), stream_ptr()))
-            features["node_features"] = nf
-            self._last_rows = (ids_host, rows)
+            features["node_features"] = self._gather(self.node_features, rows)
         for t in range(T):
             features[f"adjacency_list_{t}"] = adj[t]
-        return features
+        return features, rows
+
+    def _gather(self, table: torch.Tensor, rows: torch.Tensor) -> torch.Tensor:
+        """table[rows] (tfgnn_b200_gather_rows)."""
+        n = int(rows.shape[0])
+        F = int(table.shape[1]) if table.dim() == 2 else 0
+        out = torch.empty((n, F), dtype=torch.float32, device=self.device)
+        if n and F:
+            _ffi.check(_ffi.lib().tfgnn_b200_gather_rows(table.data_ptr(), int(table.shape[0]), F, rows.data_ptr(), 1, n,
+                                                         out.data_ptr(), stream_ptr()))
+        return out
 
     def batch_labels(self, graph_ids) -> Dict[str, Any]:
         """batch_labels of graph_dataset.py:226-246 as CUDA tensors: ``node_labels`` [num_nodes_in_batch, C] gathered through
@@ -121,32 +176,67 @@ class DeviceGraphStore:
         the store holds.  Call it after batch(graph_ids), whose node rows it reuses (otherwise it assembles them)."""
         ids_host = self._check_ids(graph_ids)
         labels: Dict[str, Any] = {}
-        lib = _ffi.lib()
         if self.node_labels is not None:
             if self._last_rows is None or not np.array_equal(self._last_rows[0], ids_host):
                 self.batch(ids_host)
-            rows = self._last_rows[1]
-            Vb, C = int(rows.shape[0]), int(self.node_labels.shape[1])
-            out = torch.empty((Vb, C), dtype=torch.float32, device=self.device)
-            if Vb:
-                _ffi.check(lib.tfgnn_b200_gather_rows(self.node_labels.data_ptr(), int(self.node_labels.shape[0]), C,
-                                                      rows.data_ptr(), 1, Vb, out.data_ptr(), stream_ptr()))
-            labels["node_labels"] = out
+            labels["node_labels"] = self._gather(self.node_labels, self._last_rows[1])
         if self.target_value is not None:
-            Gb = int(ids_host.size)
-            out = torch.empty((Gb,), dtype=torch.float32, device=self.device)
-            if Gb:
-                ids = torch.from_numpy(ids_host).to(self.device, non_blocking=True)
-                _ffi.check(lib.tfgnn_b200_gather_rows(self.target_value.data_ptr(), self.num_graphs, 1, ids.data_ptr(), 1, Gb,
-                                                      out.data_ptr(), stream_ptr()))
-            labels["target_value"] = out
+            labels["target_value"] = self._targets(ids_host)
         return labels
+
+    def shard_batch_labels(self, graph_ids, shard) -> Dict[str, Any]:
+        """The labels of shard_batch(graph_ids, shard): ``node_labels`` of rows [shard.lo, shard.hi) and ``target_value`` of all
+        the batch's graphs (the per-graph loss runs on every rank).  Reuses the node rows of the last shard_batch call."""
+        ids_host = self._check_ids(graph_ids)
+        labels: Dict[str, Any] = {}
+        if self.node_labels is not None:
+            last = self._last_shard_rows
+            if last is None or not np.array_equal(last[0], ids_host) or (last[1], last[2]) != (shard.lo, shard.hi):
+                self.shard_batch(ids_host, shard)
+            labels["node_labels"] = self._gather(self.node_labels, self._last_shard_rows[3])
+        if self.target_value is not None:
+            labels["target_value"] = self._targets(ids_host)
+        return labels
+
+    def _targets(self, ids_host: np.ndarray) -> torch.Tensor:
+        Gb = int(ids_host.size)
+        out = torch.empty((Gb,), dtype=torch.float32, device=self.device)
+        if Gb:
+            ids = torch.from_numpy(ids_host).to(self.device, non_blocking=True)
+            _ffi.check(_ffi.lib().tfgnn_b200_gather_rows(self.target_value.data_ptr(), self.num_graphs, 1, ids.data_ptr(), 1,
+                                                         Gb, out.data_ptr(), stream_ptr()))
+        return out
 
     def _check_ids(self, graph_ids) -> np.ndarray:
         ids_host = np.asarray(graph_ids, dtype=np.int32).reshape(-1)
         if ids_host.size and (ids_host.min() < 0 or ids_host.max() >= self.num_graphs):
             raise IndexError("graph id out of range")
         return ids_host
+
+
+def stored_in_degree(node_offsets: np.ndarray, edges: Sequence[Sequence[np.ndarray]]) -> np.ndarray:
+    """int64[V]: the in-degree of every node of the packed node table, summed over edge types.  edges[t][g]: graph g's
+    [e, 2] list of type t in graph-local ids; graph g owns rows [node_offsets[g], node_offsets[g + 1])."""
+    V = int(node_offsets[-1])
+    deg = np.zeros(V, dtype=np.int64)
+    for per_graph in edges:
+        counts = [len(a) for a in per_graph]
+        if sum(counts):
+            tgt = np.concatenate([np.asarray(a).reshape(-1, 2)[:, 1] for a in per_graph]).astype(np.int64)
+            tgt += np.repeat(np.asarray(node_offsets[:-1], dtype=np.int64), counts)
+            deg += np.bincount(tgt, minlength=V)[:V]
+    return deg
+
+
+def shard_bounds_from_tables(node_offsets: np.ndarray, in_degree: np.ndarray, graph_ids: np.ndarray,
+                             world_size: int) -> List[Tuple[int, int]]:
+    """DeviceGraphStore.shard_bounds on the store's host tables: node_offsets int64[G + 1] and in_degree int64[V] of the
+    packed node table.  The batch's in-degree is its graphs' slices of the table in batch order."""
+    ids = np.asarray(graph_ids, dtype=np.int64).reshape(-1)
+    starts, ends = node_offsets[ids], node_offsets[ids + 1]
+    Vb = int((ends - starts).sum())
+    deg = (np.concatenate([in_degree[a:b] for a, b in zip(starts, ends)]) if ids.size else np.zeros(0, np.int64))
+    return sharding.partition_target_range(Vb, int(world_size), deg)
 
 
 def greedy_batches(node_counts: Sequence[int], max_nodes_per_batch: int,

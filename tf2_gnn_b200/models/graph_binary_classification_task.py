@@ -5,7 +5,7 @@ from __future__ import annotations
 from typing import Any, Dict, List, Optional, Tuple
 
 from .graph_regression_task import GraphRegressionTask
-from .task_ops import graph_binary_loss, sigmoid
+from .task_ops import count_once, graph_binary_loss, sigmoid
 
 
 class GraphBinaryClassificationTask(GraphRegressionTask):
@@ -16,13 +16,15 @@ class GraphBinaryClassificationTask(GraphRegressionTask):
         super_params.update(these_hypers)
         return super_params
 
-    def compute_task_output(self, batch_features, final_node_representations, training: bool) -> Any:
-        per_graph_regression_results = super().compute_task_output(batch_features, final_node_representations, training)
+    def compute_task_output(self, batch_features, final_node_representations, training: bool, shard=None) -> Any:
+        per_graph_regression_results = super().compute_task_output(batch_features, final_node_representations, training,
+                                                                   shard=shard)
         return sigmoid(per_graph_regression_results)
 
-    def compute_task_metrics(self, batch_features, task_output, batch_labels) -> Dict[str, Any]:
-        """{"loss", "num_correct", "num_graphs"}; loss and num_correct are 0-d CUDA tensors."""
-        ce, num_correct = graph_binary_loss(task_output, batch_labels["target_value"])
+    def compute_task_metrics(self, batch_features, task_output, batch_labels, shard=None) -> Dict[str, Any]:
+        """{"loss", "num_correct", "num_graphs"}; loss and num_correct are 0-d CUDA tensors.  shard: as
+        GraphRegressionTask.compute_task_metrics."""
+        ce, num_correct = graph_binary_loss(count_once(task_output, shard), batch_labels["target_value"])
         return {"loss": ce, "num_correct": num_correct, "num_graphs": int(batch_features["num_graphs_in_batch"])}
 
     def compute_epoch_metrics(self, task_results: List[Any]) -> Tuple[float, str]:

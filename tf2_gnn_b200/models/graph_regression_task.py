@@ -10,7 +10,7 @@ from ..layers.message_passing.message_passing import Variable
 from ..layers.nodes_to_graph_representation import _MLP
 from ..utils.param_helpers import get_activation_function
 from .graph_task_model import GraphTaskModel
-from .task_ops import graph_regression_loss
+from .task_ops import count_once, graph_regression_loss
 
 
 class GraphRegressionTask(GraphTaskModel):
@@ -69,8 +69,10 @@ class GraphRegressionTask(GraphTaskModel):
         return (self._weighted_avg_of_nodes_to_graph_repr.variables + self._weighted_sum_of_nodes_to_graph_repr.variables
                 + self._regression_mlp.variables)
 
-    def compute_task_output(self, batch_features, final_node_representations, training: bool) -> Any:
-        """graph_regression_task.py:110-150: per-graph regression results [G]."""
+    def compute_task_output(self, batch_features, final_node_representations, training: bool, shard=None) -> Any:
+        """graph_regression_task.py:110-150: per-graph regression results [G].  shard: the readouts merge the ranks' rows
+        in rank order, so the graph representations and the head MLP (with the same dropout masks: every rank's stream is
+        at the same offset) are the same on every rank."""
         if self._params["use_intermediate_gnn_results"]:
             _, intermediate_node_representations = final_node_representations
             # skip the first "intermediate" representation, the output of the initial feature -> GNN input layer
@@ -83,15 +85,16 @@ class GraphRegressionTask(GraphTaskModel):
                                                  num_graphs=batch_features["num_graphs_in_batch"])
         for layer in (self._weighted_avg_of_nodes_to_graph_repr, self._weighted_sum_of_nodes_to_graph_repr):
             layer.dropout_state = self.dropout_state
-        weighted_avg_graph_repr = self._weighted_avg_of_nodes_to_graph_repr(inputs, training=training)
-        weighted_sum_graph_repr = self._weighted_sum_of_nodes_to_graph_repr(inputs, training=training)
+        weighted_avg_graph_repr = self._weighted_avg_of_nodes_to_graph_repr(inputs, training=training, shard=shard)
+        weighted_sum_graph_repr = self._weighted_sum_of_nodes_to_graph_repr(inputs, training=training, shard=shard)
         graph_representations = torch.cat([weighted_avg_graph_repr, weighted_sum_graph_repr], dim=-1)   # [G, GD]
         per_graph_results = self._regression_mlp(graph_representations, training, self.dropout_state)  # [G, 1]
         return per_graph_results.reshape(-1)
 
-    def compute_task_metrics(self, batch_features, task_output, batch_labels) -> Dict[str, Any]:
-        """{"loss": mse, "mae", "num_graphs"}; loss and mae are 0-d CUDA tensors."""
-        mse, mae = graph_regression_loss(task_output, batch_labels["target_value"])
+    def compute_task_metrics(self, batch_features, task_output, batch_labels, shard=None) -> Dict[str, Any]:
+        """{"loss": mse, "mae", "num_graphs"}; loss and mae are 0-d CUDA tensors.  shard: the per-graph output is the same on
+        every rank, and its loss is counted once (task_ops.count_once)."""
+        mse, mae = graph_regression_loss(count_once(task_output, shard), batch_labels["target_value"])
         return {"loss": mse, "mae": mae, "num_graphs": int(batch_features["num_graphs_in_batch"])}
 
     def compute_epoch_metrics(self, task_results: List[Any]) -> Tuple[float, str]:

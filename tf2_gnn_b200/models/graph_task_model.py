@@ -4,15 +4,21 @@ Same hyper-parameters and defaults; `gnn_`-prefixed parameters go to the GNN.  A
 loss (a C-ABI entry with its own backward), torch.autograd.grad over trainable_variables and one optimizer entry
 (tfgnn_b200_optimizer_step): gradients and the update are deterministic.  Batches come from a data.DeviceGraphStore:
 features from `store.batch(graph_ids)`, labels from `store.batch_labels(graph_ids)`.
+
+On target-range shards (sharding.TargetRangeShard, DESIGN.md §6 "Task models on shards") every rank trains on its rows of
+the same batch (`store.shard_batch`): the node loss is merged over the ranks, the replicated per-graph head is counted once,
+and the weight gradients are summed in rank order, so every rank applies the same update.
 """
 from __future__ import annotations
 
+import contextlib
 import time
 from abc import abstractmethod
 from typing import Any, Dict, Iterable, List, Optional, Tuple
 
 import torch
 
+from .. import sharding
 from ..layers import GNN, GNNInput
 from ..layers.message_passing.message_passing import Variable
 from .task_ops import Optimizer, PolynomialWarmupAndDecaySchedule
@@ -84,33 +90,37 @@ class GraphTaskModel:
 
     # ---- forward ----------------------------------------------------------------------------------------------------
     @abstractmethod
-    def compute_task_output(self, batch_features: Dict[str, Any], final_node_representations, training: bool) -> Any:
-        """graph_task_model.py:131-156."""
+    def compute_task_output(self, batch_features: Dict[str, Any], final_node_representations, training: bool,
+                            shard=None) -> Any:
+        """graph_task_model.py:131-156.  shard: the features are the rank's part of the batch (store.shard_batch)."""
 
-    def compute_final_node_representations(self, inputs, training: bool):
+    def compute_final_node_representations(self, inputs, training: bool, shard=None):
         """graph_task_model.py:158-179: (final, all representations incl. the initial one) when
-        use_intermediate_gnn_results, else the final representations."""
+        use_intermediate_gnn_results, else the final representations.  shard (sharding.TargetRangeShard): the GNN runs
+        on the rank's rows (GNN.call), and so do the representations."""
         adjacency_lists = tuple(inputs[f"adjacency_list_{t}"] for t in range(self._num_edge_types))
         gnn_input = GNNInput(node_features=self.compute_initial_node_features(inputs, training),
                              adjacency_lists=adjacency_lists, node_to_graph_map=inputs["node_to_graph_map"],
                              num_graphs=inputs["num_graphs_in_batch"])
-        return self._gnn(gnn_input, training=training, return_all_representations=self._use_intermediate_gnn_results)
+        return self._gnn(gnn_input, training=training, return_all_representations=self._use_intermediate_gnn_results,
+                         shard=shard)
 
-    def call(self, inputs, training: bool):
-        final_node_representations = self.compute_final_node_representations(inputs, training)
-        return self.compute_task_output(inputs, final_node_representations, training)
+    def call(self, inputs, training: bool, shard=None):
+        final_node_representations = self.compute_final_node_representations(inputs, training, shard)
+        return self.compute_task_output(inputs, final_node_representations, training, shard=shard)
 
-    def __call__(self, inputs, training: bool = False):
+    def __call__(self, inputs, training: bool = False, shard=None):
         if not self.built:
             shapes = {"node_features": tuple(inputs["node_features"].shape)}
             shapes.update({f"adjacency_list_{t}": tuple(inputs[f"adjacency_list_{t}"].shape) for t in range(self._num_edge_types)})
             self.build(shapes)
-        return self.call(inputs, training)
+        return self.call(inputs, training, shard)
 
     @abstractmethod
     def compute_task_metrics(self, batch_features: Dict[str, Any], task_output: Any,
-                             batch_labels: Dict[str, Any]) -> Dict[str, Any]:
-        """graph_task_model.py:185-205: must hold "loss"; values may be device tensors."""
+                             batch_labels: Dict[str, Any], shard=None) -> Dict[str, Any]:
+        """graph_task_model.py:185-205: must hold "loss"; values may be device tensors.  shard: the metrics of the whole
+        batch, the same on every rank."""
 
     @abstractmethod
     def compute_epoch_metrics(self, task_results: List[Any]) -> Tuple[float, str]:
@@ -158,35 +168,62 @@ class GraphTaskModel:
         self._optimizer.apply_gradients([(g, v.value) for g, v in pairs])
 
     # ---- training loop ----------------------------------------------------------------------------------------------
-    def train_step(self, batch_features: Dict[str, Any], batch_labels: Dict[str, Any]) -> Dict[str, Any]:
+    def train_step(self, batch_features: Dict[str, Any], batch_labels: Dict[str, Any], shard=None) -> Dict[str, Any]:
         """graph_task_model.py:338-365 with training=True: forward, loss, gradients of every trainable variable, one
-        optimizer step."""
-        task_output = self(batch_features, training=True)
-        task_metrics = self.compute_task_metrics(batch_features, task_output, batch_labels)
+        optimizer step.
+
+        shard (sharding.TargetRangeShard): the features and labels are the rank's part of the batch (store.shard_batch,
+        store.shard_batch_labels).  The forward runs under sharding.regather_saved_tables(), the metrics are the whole
+        batch's, and the gradients are summed over the ranks in rank order before the optimizer step, so every rank that
+        started from the same variables (sharding.broadcast_variables) holds the same variables, slots and step count
+        after it.  Collective: every rank of the shard's group makes the same call."""
+        context = sharding.regather_saved_tables() if shard is not None else contextlib.nullcontext()
+        with context:
+            task_output = self(batch_features, training=True, shard=shard)
+        task_metrics = self.compute_task_metrics(batch_features, task_output, batch_labels, shard=shard)
         variables = self.trainable_variables
-        gradients = torch.autograd.grad(task_metrics["loss"], [v.value for v in variables], allow_unused=True)
+        values = [v.value for v in variables]
+        gradients = torch.autograd.grad(task_metrics["loss"], values, allow_unused=True)
+        if shard is not None:
+            gradients = sharding.sum_gradient_list_over_ranks(gradients, values, shard.group)
         self._apply_gradients(zip(gradients, variables))
         self._train_step_counter += 1
         return task_metrics
 
-    def _run_step(self, batch_features: Dict[str, Any], batch_labels: Dict[str, Any], training: bool) -> Dict[str, Any]:
+    def _run_step(self, batch_features: Dict[str, Any], batch_labels: Dict[str, Any], training: bool,
+                  shard=None) -> Dict[str, Any]:
         if training:
-            return self.train_step(batch_features, batch_labels)
+            return self.train_step(batch_features, batch_labels, shard=shard)
         with torch.no_grad():
-            task_output = self(batch_features, training=False)
-            return self.compute_task_metrics(batch_features, task_output, batch_labels)
+            task_output = self(batch_features, training=False, shard=shard)
+            return self.compute_task_metrics(batch_features, task_output, batch_labels, shard=shard)
 
-    def run_one_epoch(self, store, batches: Iterable, quiet: bool = True,
-                      training: bool = True) -> Tuple[float, float, List[Any]]:
+    def run_one_epoch(self, store, batches: Iterable, quiet: bool = True, training: bool = True,
+                      shard_group=None) -> Tuple[float, float, List[Any]]:
         """graph_task_model.py:367-398 over a data.DeviceGraphStore and an iterable of graph-id arrays (e.g.
         store.iter_batch_graph_ids(max_nodes)).  Returns (graph-average loss, graphs per second, task_results).  The
-        per-batch losses stay on the device until the epoch ends."""
+        per-batch losses stay on the device until the epoch ends.
+
+        shard_group (a torch.distributed process group, e.g. torch.distributed.group.WORLD): train or evaluate every batch
+        on target-range shards over the group's ranks.  Each batch is cut by store.shard_bounds, and each rank takes its
+        part with store.shard_batch / shard_batch_labels.  Every rank must pass the same batches; every rank returns the same
+        losses and metrics, and the slowest rank's graphs per second."""
+        shard_rank = shard_world = None
+        if shard_group is not None:
+            import torch.distributed as dist
+            shard_rank, shard_world = dist.get_rank(shard_group), dist.get_world_size(shard_group)
         epoch_time_start = time.time()
         task_results, losses, counts = [], [], []
         for step, graph_ids in enumerate(batches):
-            batch_features = store.batch(graph_ids)
-            batch_labels = store.batch_labels(graph_ids)
-            task_metrics = self._run_step(batch_features, batch_labels, training)
+            if shard_group is None:
+                shard = None
+                batch_features = store.batch(graph_ids)
+                batch_labels = store.batch_labels(graph_ids)
+            else:
+                shard = sharding.TargetRangeShard(store.shard_bounds(graph_ids, shard_world), shard_rank, shard_group)
+                batch_features = store.shard_batch(graph_ids, shard)
+                batch_labels = store.shard_batch_labels(graph_ids, shard)
+            task_metrics = self._run_step(batch_features, batch_labels, training, shard)
             losses.append(task_metrics["loss"].detach())
             counts.append(int(batch_features["num_graphs_in_batch"]))
             task_results.append(task_metrics)
@@ -194,6 +231,9 @@ class GraphTaskModel:
                 print(f"   Step: {step:4d}", end="\r")
         host_losses = torch.stack(losses).cpu().double().tolist() if losses else []
         total_time = time.time() - epoch_time_start
+        if shard_group is not None:
+            elapsed = torch.tensor([total_time], dtype=torch.float64, device=store.device)
+            total_time = float(sharding.all_gather_stacked(elapsed, shard_group).max())
         total_num_graphs = sum(counts)
         total_loss = sum(l * n for l, n in zip(host_losses, counts))
         return total_loss / float(total_num_graphs), float(total_num_graphs) / total_time, task_results

@@ -48,16 +48,18 @@ class NodeMulticlassTask(GraphTaskModel):
     def _task_variables(self) -> List[Variable]:
         return list(self.node_to_labels_layer)
 
-    def compute_task_output(self, batch_features, final_node_representations, training: bool):
+    def compute_task_output(self, batch_features, final_node_representations, training: bool, shard=None):
+        """[V, num_labels] logits; on a shard, the rank's rows."""
         if self._use_intermediate_gnn_results:
             final_node_representations = final_node_representations[0]
         kernel, bias = self.node_to_labels_layer
         return (node_ops.dense(final_node_representations, kernel.value, bias.value),)
 
-    def compute_task_metrics(self, batch_features, task_output, batch_labels) -> Dict[str, Any]:
-        """{"loss", "f1_score"} as 0-d CUDA tensors (one fused pass over the logits), and the counts behind the F1."""
+    def compute_task_metrics(self, batch_features, task_output, batch_labels, shard=None) -> Dict[str, Any]:
+        """{"loss", "f1_score"} as 0-d CUDA tensors (one fused pass over the logits), and the counts behind the F1.  On a
+        shard: those of the whole batch, from the ranks' partial sums and counts merged in rank order."""
         (per_node_logits,) = task_output
-        loss, f1_score, counts = node_multiclass_loss(per_node_logits, batch_labels["node_labels"])
+        loss, f1_score, counts = node_multiclass_loss(per_node_logits, batch_labels["node_labels"], shard)
         return {"loss": loss, "f1_score": f1_score, "f1_counts": counts}
 
     def compute_epoch_metrics(self, task_results: List[Any]) -> Tuple[float, str]:

@@ -45,6 +45,62 @@ class _NodeMulticlassLoss(torch.autograd.Function):
         return grad, None
 
 
+class _ShardNodeMulticlassLoss(torch.autograd.Function):
+    """_NodeMulticlassLoss over a batch cut by target range: the rank's raw sum and counts (…_loss_partial), all-gathered and
+    merged in rank order over the batch's row count (…_loss_merge), so every rank gets the same (loss, f1_score, counts).
+    The backward needs no collective: a rank's logits enter its own partial only (…_loss_bwd_rows with 1 / total rows)."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, shard):
+        from .. import sharding
+        logits, labels = logits.contiguous(), labels.contiguous()
+        V, C = int(logits.shape[0]), int(logits.shape[1])
+        lib = _ffi.lib()
+        part_sum, part_counts = _scalar(logits, n=(1,)), _scalar(logits, torch.int64, (3,))
+        _ffi.check(lib.tfgnn_b200_node_multiclass_loss_partial(logits.data_ptr(), labels.data_ptr(), V, C,
+                                                               part_sum.data_ptr(), part_counts.data_ptr(), stream_ptr()))
+        sums = sharding.all_gather_stacked(part_sum, shard.group).contiguous()
+        counts_all = sharding.all_gather_stacked(part_counts, shard.group).contiguous()
+        loss, f1, counts = _scalar(logits), _scalar(logits), _scalar(logits, torch.int64, (3,))
+        _ffi.check(lib.tfgnn_b200_node_multiclass_loss_merge(sums.data_ptr(), counts_all.data_ptr(), int(sums.shape[0]),
+                                                             shard.num_nodes, loss.data_ptr(), f1.data_ptr(),
+                                                             counts.data_ptr(), stream_ptr()))
+        ctx.save_for_backward(logits, labels)
+        ctx.total_rows = shard.num_nodes
+        ctx.mark_non_differentiable(f1, counts)
+        return loss, f1, counts
+
+    @staticmethod
+    def backward(ctx, g, _g_f1, _g_counts):
+        logits, labels = ctx.saved_tensors
+        grad = torch.empty_like(logits)
+        _ffi.check(_ffi.lib().tfgnn_b200_node_multiclass_loss_bwd_rows(
+            logits.data_ptr(), labels.data_ptr(), int(logits.shape[0]), int(logits.shape[1]), ctx.total_rows,
+            g.contiguous().data_ptr(), grad.data_ptr(), stream_ptr()))
+        return grad, None, None
+
+
+class _CountOnce(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, rank):
+        ctx.rank = rank
+        return x.view_as(x)
+
+    @staticmethod
+    def backward(ctx, g):
+        return (g if ctx.rank == 0 else torch.zeros_like(g)), None
+
+
+def count_once(x: torch.Tensor, shard) -> torch.Tensor:
+    """The identity, whose backward passes the gradient on rank 0 and exact zeros on every other rank.  For a value that is
+    the same on every rank of a target-range shard (a merged per-graph row and what a replicated head computes from it): its
+    loss is then counted once when the readout's backward sums the ranks' gradients, and the head's weight gradients are
+    rank 0's after sharding.sum_gradient_list_over_ranks.  shard None: the identity."""
+    if shard is None:
+        return x
+    return _CountOnce.apply(x, shard.rank)
+
+
 class _GraphRegressionLoss(torch.autograd.Function):
     """tf.losses.mean_squared_error / mean_absolute_error over the batch's graphs (graph_regression_task.py:152-166).
     Returns (mse, mae)."""
@@ -91,8 +147,12 @@ class _GraphBinaryLoss(torch.autograd.Function):
         return grad, None
 
 
-def node_multiclass_loss(logits: torch.Tensor, labels: torch.Tensor):
-    """(loss, f1_score, counts (tp, fp, fn)) as 0-d / [3] CUDA tensors."""
+def node_multiclass_loss(logits: torch.Tensor, labels: torch.Tensor, shard=None):
+    """(loss, f1_score, counts (tp, fp, fn)) as 0-d / [3] CUDA tensors.  shard (sharding.TargetRangeShard): logits and labels
+    are the rank's rows of the batch; the results are those of the whole batch, the same bits on every rank (collective in
+    the forward only)."""
+    if shard is not None:
+        return _ShardNodeMulticlassLoss.apply(logits, labels.to(torch.float32), shard)
     return _NodeMulticlassLoss.apply(logits, labels.to(torch.float32))
 
 

@@ -326,6 +326,46 @@ def sum_gradients_over_ranks(variables, group=None) -> None:
         off += n
 
 
+def sum_gradient_list_over_ranks(gradients, like, group=None):
+    """sum_gradients_over_ranks for a list of gradients (torch.autograd.grad's result; None = no gradient on this rank) of
+    the float32 tensors `like`.  Returns the sums over ranks, added in rank order: the same bits on every rank.  A gradient
+    that is None on every rank stays None (an optimizer then skips the variable, as it does unsharded); one that is None on
+    some ranks counts as zeros there.  One all-gather; every rank must pass the same variables in the same order."""
+    like = list(like)
+    if not like:
+        return []
+    dev = like[0].device
+    present = torch.tensor([0.0 if g is None else 1.0 for g in gradients], dtype=torch.float32, device=dev)
+    flat = torch.cat([(g if g is not None else torch.zeros_like(t)).reshape(-1).to(torch.float32)
+                      for g, t in zip(gradients, like)] + [present])
+    total = sum_over_ranks(flat, group)
+    flags = total[-len(like):].cpu()
+    out, off = [], 0
+    for i, t in enumerate(like):
+        n = t.numel()
+        out.append(total[off: off + n].view_as(t).clone() if flags[i] > 0 else None)
+        off += n
+    return out
+
+
+def broadcast_variables(variables, group=None) -> None:
+    """Copy rank 0's values of `variables` (tensors or objects with `.value`, the same list on every rank) into every rank's,
+    in place: e.g. the starting weights of a model trained on target-range shards.  Goes through all_gather_stacked, so it
+    uses the module's two collectives only."""
+    tensors = [getattr(v, "value", v) for v in variables]
+    if not tensors:
+        return
+    dev = tensors[0].device
+    flat = torch.cat([t.detach().reshape(-1).to(torch.float32) for t in tensors]).to(dev)
+    first = all_gather_stacked(flat, group)[0]
+    off = 0
+    with torch.no_grad():
+        for t in tensors:
+            n = t.numel()
+            t.copy_(first[off: off + n].view_as(t))
+            off += n
+
+
 # ------------------------------------------------------------------------------------------------
 # 2b. the all-gather fused into the layer kernel: node-state tables in peer-mapped (symmetric) memory
 # ------------------------------------------------------------------------------------------------

@@ -21,6 +21,14 @@ rank's target range (`GNN(..., shard=sharding.TargetRangeShard(bounds, rank))`),
 sharding.sum_gradients_over_ranks and checks on rank 0 the output rows and every gradient against unsharded autograd, and
 that every rank holds the same weight-gradient bits.  The graph is --graphs graphs of equal size, so that cuts fall inside
 graphs.  Multi-GPU step times of this mode are reported by the tool but have not been measured for the documentation.
+
+With --task node|regression every step is a training step of a task model on target-range shards (DESIGN.md §6 "Task
+models on shards"): NodeMulticlassTask with PPI_RGCN.json's layers on PPI-sized graphs, or GraphRegressionTask with its
+defaults on --task-graphs QM9-sized graphs, all in one batch.  Every rank builds the same seeded store, takes rank 0's
+weights (sharding.broadcast_variables), assembles its rows (store.shard_batch over store.shard_bounds) and runs
+train_step(shard=...).  Rank 0 also runs the unsharded steps and checks the losses of every step and the gradients of the
+first step at the test bar (3e-5 norm-wise), and the JSON line says whether every rank holds the same variable bits at the
+end.  Multi-GPU times of this mode are not measured for the documentation.
 """
 import argparse
 import json
@@ -48,11 +56,16 @@ def main():
     ap.add_argument("--train", action="store_true", help="forward + backward per step (gradient check on rank 0)")
     ap.add_argument("--stack", action="store_true", help="train a whole GNN stack with global exchange (check on rank 0)")
     ap.add_argument("--graphs", type=int, default=64, help="--stack: number of equal-size graphs in the node table")
+    ap.add_argument("--task", choices=("node", "regression"), help="train a task model on shards (check on rank 0)")
+    ap.add_argument("--task-graphs", type=int, default=0,
+                    help="--task: graphs in the batch (default: 24 PPI-sized node-task graphs, 2000 QM9-sized graphs)")
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    if args.task:
+        return train_task(args, rank, world)
     V, L, H = args.nodes, args.types, args.hidden
     rng = np.random.default_rng(7)
     adjs = [rng.integers(0, V, size=(args.edges_per_type, 2), dtype=np.int32) for _ in range(L)]
@@ -252,6 +265,99 @@ def train_stack(args, rank, world, bounds, adjs, h0):
                           "rel_err_out": err_out, "rel_err_grad_h": err_h, "max_rel_err_grad_w": err_w,
                           "weight_grads_same_bits_on_every_rank": same_bits, "ok": ok,
                           "ms_per_step_max_over_ranks": float(t.item())}), flush=True)
+    dist.barrier()
+    dist.destroy_process_group()
+    if not ok:
+        raise SystemExit(1)
+
+
+def train_task(args, rank, world):
+    from tf2_gnn_b200.data import DeviceGraphStore
+    from tf2_gnn_b200.models import GraphRegressionTask, NodeMulticlassTask
+    rng = np.random.default_rng(11)
+    node = args.task == "node"
+    G = args.task_graphs or (24 if node else 2000)
+    F, L, C = (50, 3, 121) if node else (15, 4, None)
+    graphs = []
+    for _ in range(G):
+        n = int(rng.integers(1500, 3000) if node else rng.integers(9, 30))
+        s = {"node_features": rng.uniform(-1, 1, (n, F)).astype(np.float32),
+             "adjacency_lists": [rng.integers(0, n, (4 * n, 2)).astype(np.int32) for _ in range(L)]}
+        if node:
+            s["node_labels"] = (rng.uniform(size=(n, C)) < 0.3).astype(np.float32)
+        else:
+            s["target_value"] = float(rng.normal(3.0, 1.0))
+        graphs.append(s)
+    store = DeviceGraphStore(graphs, L)
+    ids = np.arange(G)
+    if node:                                              # PPI_RGCN.json's layers
+        cls = NodeMulticlassTask
+        params = cls.get_default_hyperparameters("rgcn")
+        params.update(gnn_num_layers=4, gnn_hidden_dim=320, gnn_layer_input_dropout_rate=0.1,
+                      gnn_dense_every_num_layers=10000, gnn_residual_every_num_layers=10000,
+                      gnn_global_exchange_every_num_layers=10000)
+    else:
+        cls = GraphRegressionTask
+        params = cls.get_default_hyperparameters()
+    shapes = {"node_features": (None, F)}
+    shapes.update({f"adjacency_list_{t}": (None, 2) for t in range(L)})
+
+    def build(seed):
+        torch.manual_seed(seed)
+        model = cls(params, dataset=store)
+        model.build(shapes)
+        return model
+
+    def recording(model, seen):
+        apply = model._apply_gradients
+
+        def rec(pairs):
+            pairs = list(pairs)
+            seen.append([None if g is None else g.detach().clone() for g, _ in pairs])
+            apply(pairs)
+        model._apply_gradients = rec
+
+    shard = sharding.TargetRangeShard(store.shard_bounds(ids, world), rank)
+    feats, labels = store.shard_batch(ids, shard), store.shard_batch_labels(ids, shard)
+    model = build(rank)                                   # a different seed on every rank: rank 0's weights win
+    sharding.broadcast_variables(model.trainable_variables)
+    grads = []
+    recording(model, grads)
+    losses = [model.train_step(feats, labels, shard=shard)["loss"].item() for _ in range(3)]   # the first two: warm-up
+    torch.cuda.synchronize()
+    dist.barrier()
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    step_losses = [model.train_step(feats, labels, shard=shard)["loss"] for _ in range(args.steps)]
+    ev1.record()
+    torch.cuda.synchronize()
+    losses += [float(l) for l in step_losses]
+    t = torch.tensor([ev0.elapsed_time(ev1) / args.steps], device="cuda")
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    flat = torch.cat([v.value.detach().reshape(-1) for v in model.trainable_variables])
+    stacked = sharding.all_gather_stacked(flat)
+    same_bits = bool(torch.equal(stacked.amax(0), stacked.amin(0)))
+    ok = True
+    if rank == 0:
+        full = build(0)
+        full_grads = []
+        recording(full, full_grads)
+        f_feats, f_labels = store.batch(ids), store.batch_labels(ids)
+        full_losses = [full.train_step(f_feats, f_labels)["loss"].item() for _ in range(3 + args.steps)]
+
+        def rel(a, b):
+            a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+            return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
+
+        pairs = [(a, b) for a, b in zip(grads[0], full_grads[0]) if b is not None]
+        floor = max(float(b.norm()) for _, b in pairs)
+        err_g = max(float((a - b).norm()) / max(float(b.norm()), floor) for a, b in pairs)
+        err_loss = rel(losses, full_losses)
+        ok = err_loss <= 3e-5 and err_g <= 3e-5 and same_bits
+        print(json.dumps({"check": f"{cls.__name__} training on target-range shards == unsharded", "world_size": world,
+                          "graphs": G, "nodes": int(store.node_offsets_host[-1]), "rel_err_losses": err_loss,
+                          "max_rel_err_first_step_grads": err_g, "variables_same_bits_on_every_rank": same_bits,
+                          "ok": ok, "ms_per_step_max_over_ranks": float(t.item())}), flush=True)
     dist.barrier()
     dist.destroy_process_group()
     if not ok:
