@@ -265,7 +265,8 @@ TFGNN_API int tfgnn_b200_rgin_fwd(tfgnn_batch_t* batch, const float* h, int32_t 
                         float* out, void* stream);
 
 /* GNN-FiLM (gnn_film.py:83-108): m = gamma_l(h_v) * EdgeMLP_l(...) + beta_l(h_v),
- * [gamma|beta] = h_v F_l, film_weights: host array of L device pointers [D, 2H] (no hidden layers). */
+ * [gamma|beta] = h_v F_l, film_weights: host array of L device pointers [D, 2H] (no hidden FiLM-MLP layers; for those
+ * see tfgnn_b200_film_in_fwd). */
 TFGNN_API int tfgnn_b200_film_fwd(tfgnn_batch_t* batch, const float* h, int32_t D,
                         const float* const* mlp_weights, int32_t num_hidden_layers,
                         const float* const* film_weights, int32_t H, uint32_t flags,
@@ -292,6 +293,26 @@ TFGNN_API int tfgnn_b200_film_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, 
                         uint32_t flags, int32_t aggregation, int32_t activation, const float* out,
                         const float* grad_out, float* grad_h, float* const* grad_W, float* const* grad_film,
                         void* stream);
+
+/* GNN-FiLM with a per-type FiLM input: tfgnn_b200_film_fwd / _bwd with the last layer of each FiLM MLP fed from
+ * film_in [V_owned, L*S] instead of h_v.  Type l's input z_l is columns [l*S, (l+1)*S), its rows are the batch's owned
+ * targets (rows [lo, hi) of the node table on a target-range shard), and film_weights[l] is [S, 2H]:
+ * [gamma_l | beta_l] = z_l F_l.  GNN-FiLM with hidden FiLM-MLP layers (gnn_film.py:74-78,99-101) computes the hidden chain
+ * z_l = relu(.. relu(h_v F^(0)_l) ..) at node level and passes it here, so no tensor gets a per-edge dimension.
+ * The forward covers every configuration tfgnn_b200_film_fwd covers.  The backward has tfgnn_b200_film_bwd's scope, shard
+ * contract and determinism, plus S > 0 a multiple of 4.  It writes grad_h (may be NULL: the message side and the
+ * target-state term only), grad_film_in [V_owned, L*S] (may be NULL: per type [dgamma_l | dbeta_l] F_l^T), grad_W[l] and
+ * grad_film[l] [S, 2H] = z_l^T [dgamma_l | dbeta_l]. */
+TFGNN_API int tfgnn_b200_film_in_fwd(tfgnn_batch_t* batch, const float* h, int32_t D,
+                        const float* const* mlp_weights, int32_t num_hidden_layers, const float* film_in, int32_t S,
+                        const float* const* film_weights, int32_t H, uint32_t flags, int32_t aggregation,
+                        int32_t activation, int32_t path, float* out, void* stream);
+
+TFGNN_API int tfgnn_b200_film_in_bwd(tfgnn_batch_t* batch, tfgnn_batch_t* batch_t, const float* h, int32_t D,
+                        const float* const* mlp_weights, const float* film_in, int32_t S,
+                        const float* const* film_weights, int32_t H, uint32_t flags, int32_t aggregation,
+                        int32_t activation, const float* out, const float* grad_out, float* grad_h, float* grad_film_in,
+                        float* const* grad_W, float* const* grad_film, void* stream);
 
 /* RGAT (rgat.py:91-163): per-type projection W_l [D,H], attention a_l [K, 2H/K]; softmax over all
  * incoming edges of all types jointly, per head; activation after.  The result is run-to-run reproducible (no float

@@ -54,6 +54,7 @@ EXPORTED_SYMBOLS = (
     "tfgnn_b200_graph_regression_loss_bwd", "tfgnn_b200_graph_binary_loss_fwd", "tfgnn_b200_graph_binary_loss_bwd",
     "tfgnn_b200_optimizer_step", "tfgnn_b200_node_multiclass_loss_partial", "tfgnn_b200_node_multiclass_loss_merge",
     "tfgnn_b200_node_multiclass_loss_bwd_rows", "tfgnn_b200_assemble_batch_rows",
+    "tfgnn_b200_film_in_fwd", "tfgnn_b200_film_in_bwd",
 )
 
 _PP = POINTER(c_void_p)
@@ -98,6 +99,11 @@ def lib() -> ctypes.CDLL:
                                       c_int32, c_int32, c_void_p, c_void_p]
     L.tfgnn_b200_film_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, _PP, _PP, c_int32, c_uint32, c_int32,
                                       c_int32, c_void_p, c_void_p, c_void_p, _PP, _PP, c_void_p]
+    L.tfgnn_b200_film_in_fwd.argtypes = [c_void_p, c_void_p, c_int32, _PP, c_int32, c_void_p, c_int32, _PP, c_int32,
+                                         c_uint32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
+    L.tfgnn_b200_film_in_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, _PP, c_void_p, c_int32, _PP, c_int32,
+                                         c_uint32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, _PP, _PP,
+                                         c_void_p]
     L.tfgnn_b200_edge_mlp_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, _PP, c_int32, c_int32, c_uint32,
                                           c_int32, c_int32, c_void_p, c_void_p, c_void_p, _PP, c_void_p]
     L.tfgnn_b200_rgat_fwd.argtypes = [c_void_p, c_void_p, c_int32, _PP, _PP, c_int32, c_int32, c_int32, c_int32,

@@ -791,54 +791,73 @@ __global__ void add_kernel(float* __restrict__ acc, const float* __restrict__ a,
 
 }  // namespace tfgnn
 
-extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int32_t D,
-                                   const float* const* mlp_weights, const float* const* film_weights, int32_t H,
-                                   uint32_t flags, int32_t aggregation, int32_t activation, const float* out,
-                                   const float* grad_out, float* grad_h, float* const* grad_W, float* const* grad_film,
-                                   void* stream) {
+namespace tfgnn {
+
+// The shared body of tfgnn_b200_film_bwd and tfgnn_b200_film_in_bwd.  The FiLM MLPs' last layers read fin [V, L*S] (owned
+// rows): type l reads columns [l*fstride, l*fstride + S).  fstride 0 (film_bwd): fin is ignored and h's owned rows [V, D]
+// are read instead, S = D, and the
+// FiLM term [dgamma_l | dbeta_l] F_l^T lands in grad_h with the target-state term.  Else it goes to grad_fin [V, L*S] (may be
+// NULL) and grad_h gets the message side and the target-state term only.  `name` prefixes the unsupported-case messages.
+static int film_bwd_core(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int D, const float* const* mlp_weights,
+                         const float* fin, int fstride, int S, const float* const* film_weights, int H,
+                         uint32_t flags, int aggregation, int activation, const float* out, const float* grad_out,
+                         float* grad_h, float* grad_fin, float* const* grad_W, float* const* grad_film, const char* name,
+                         cudaStream_t st) {
   // the configuration is judged from the scalar arguments alone, before any batch is read
-  TFGNN_REQUIRE(D > 0 && H > 0, "D and H must be positive");
-  TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), "unknown activation / aggregation code");
+  const std::string who(name);
+  const std::string dims = fstride ? "D, H and S" : "D and H";
+  TFGNN_REQUIRE(D > 0 && H > 0 && S > 0, who + ": " + dims + " must be positive");
+  TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), who + ": unknown activation / aggregation code");
   if (flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION)
-    return unsupported("film_bwd: activation-before-aggregation is not built yet");
-  if (aggregation == TFGNN_AGG_MAX) return unsupported("film_bwd: max aggregation is not built yet");
-  if (D % 4 != 0 || H % 4 != 0) return unsupported("film_bwd needs D and H to be multiples of 4");
-  TFGNN_REQUIRE(b != nullptr && bt != nullptr, "batch / transposed batch is NULL");
+    return unsupported(who + ": activation-before-aggregation is not built yet");
+  if (aggregation == TFGNN_AGG_MAX) return unsupported(who + ": max aggregation is not built yet");
+  if (D % 4 != 0 || H % 4 != 0 || S % 4 != 0)
+    return unsupported(who + " needs " + dims + " to be multiples of 4");
+  TFGNN_REQUIRE(b != nullptr && bt != nullptr, who + ": batch / transposed batch is NULL");
   // V = owned target rows (of out / grad_out), Vs = rows of h and grad_h, lo = global id of local target 0
   const long long V = b->V, Vs = b->V_src, lo = b->tgt_off;
   const int L = b->L;
   if (int rc = check_backward_pair(b, bt)) return rc;
+  TFGNN_REQUIRE((long long)L * S < (1ll << 31), who + ": L * S overflows");
+  const int ldf = fstride ? L * S : D;   // columns of fin and grad_fin
   TFGNN_REQUIRE(L == 0 || (mlp_weights && film_weights && grad_W && grad_film), "weight / weight-gradient table is NULL");
   const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;   // W_l is then [2D, H]: rows [0,D) source, [D,2D) target
   const int KT = use_target ? 2 * D : D;                          // columns of [A_l | T_l], rows of W_l
   for (int l = 0; l < L; ++l)
     TFGNN_REQUIRE(mlp_weights[l] && film_weights[l] && grad_W[l] && grad_film[l], "a weight pointer is NULL");
-  cudaStream_t st = (cudaStream_t)stream;
   if (V == 0 || L == 0)   // no owned rows (an empty shard) or no edge types: zero contribution
-    return zero_contribution({{grad_W, L, (size_t)KT * H}, {grad_film, L, (size_t)D * 2 * H}}, grad_h, (size_t)Vs * D, st);
-  TFGNN_REQUIRE(h && out && grad_out, "NULL pointer");
-  const float* h_tgt = h + (size_t)lo * D;   // rows of the owned targets (FiLM parameters, target-state input)
+    return zero_contribution({{grad_W, L, (size_t)KT * H}, {grad_film, L, (size_t)S * 2 * H}}, grad_h, (size_t)Vs * D, st);
+  const float* h_tgt = h ? h + (size_t)lo * D : nullptr;   // rows of the owned targets (target-state input)
+  if (!fstride) fin = h_tgt;
+  TFGNN_REQUIRE(h && out && grad_out && fin, who + ": NULL pointer");
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
-  const int LD = L * D;
+  const bool film_to_h = fstride == 0;       // the FiLM input is h itself: its gradient term goes to grad_h
+  if (film_to_h) grad_fin = nullptr;
+  const bool target_side = grad_h && (film_to_h || use_target);   // grad_h gets owned-row terms (dHt)
+  const int LD = L * D, SD = S > D ? S : D;
   // 1. dZ = dOut * act'(out) * rn(v)
   PoolBuffer dz{st};
   int rc = begin_backward(b, bt, out, grad_out, H, activation, aggregation, st, dz, [&](float* z) {
-    return tfgnn_b200_film_fwd(b, h, D, mlp_weights, 0, film_weights, H, flags, aggregation, TFGNN_ACT_NONE,
-                               TFGNN_PATH_AUTO, z, stream);
+    return film_fwd_core(b, h, D, mlp_weights, 0, fin, fstride, S, film_weights, H, flags, aggregation,
+                         TFGNN_ACT_NONE, TFGNN_PATH_AUTO, z, st);
   });
   if (rc) return rc;
   PoolBuffer AT{st}, dQ{st}, dGB{st}, part{st};
   rc = AT.alloc((size_t)V * KT * sizeof(float));                                       // [A_l | T_l], later dT_l
   if (!rc) rc = dQ.alloc((size_t)V * H * sizeof(float));
   if (!rc) rc = dGB.alloc((size_t)V * 2 * H * sizeof(float));                          // [dgamma_l | dbeta_l]
-  if (!rc) rc = part.alloc(tn_partial_floats(V, D, 2 * H) * sizeof(float));   // KT * H <= D * 2H
+  if (!rc) rc = part.alloc(tn_partial_floats(V, SD, 2 * H) * sizeof(float));   // KT * H <= D * 2H
   if (rc) return rc;
   PoolBuffer dA{st}, dHt{st}, WT{st}, FT{st};
   if (grad_h) {
     rc = dA.alloc((size_t)V * LD * sizeof(float));
-    if (!rc) rc = dHt.alloc((size_t)V * D * sizeof(float));   // target-side terms of grad_h, summed over types
+    if (!rc && target_side) rc = dHt.alloc((size_t)V * D * sizeof(float));   // target-side terms of grad_h, summed over types
     if (!rc) rc = WT.alloc((size_t)H * KT * sizeof(float));
-    if (!rc) rc = FT.alloc((size_t)2 * H * D * sizeof(float));
+    if (rc) return rc;
+    if (!film_to_h && use_target) TFGNN_CUDA(cudaMemsetAsync(dHt.f(), 0, (size_t)V * D * sizeof(float), st));
+  }
+  if ((grad_h && film_to_h) || grad_fin) {
+    rc = FT.alloc((size_t)2 * H * S * sizeof(float));
     if (rc) return rc;
   }
 
@@ -849,6 +868,7 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
     const int* rp = b->row_ptr + (size_t)l * V;   // the V segments of type l
     const float* Wl = mlp_weights[l];
     const float* Fl = film_weights[l];
+    const float* zl = fin + (size_t)l * fstride;   // type l's FiLM input
     // 2. [A_l | T_l] (recomputed)
     {
       EdgeReduceParams p;
@@ -863,27 +883,34 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
         if (rc) return rc;
       }
     }
-    // 3. dQ_l = dZ * (h_v Fgamma_l);  dgamma_l = dZ * ([A_l | T_l] W_l);  dbeta_l = c dZ
-    rc = node_gemm(h_tgt, D, Fl, 2 * H, dQ.f(), H, V, H, D, by_dz, TFGNN_PATH_AUTO, st);
+    // 3. dQ_l = dZ * (z_l Fgamma_l);  dgamma_l = dZ * ([A_l | T_l] W_l);  dbeta_l = c dZ
+    rc = node_gemm(zl, ldf, Fl, 2 * H, dQ.f(), H, V, H, S, by_dz, TFGNN_PATH_AUTO, st);
     if (rc) return rc;
     rc = node_gemm(AT.f(), KT, Wl, H, dGB.f(), 2 * H, V, H, KT, by_dz, TFGNN_PATH_AUTO, st);
     if (rc) return rc;
     film_beta_grad_kernel<<<grid_for(V * H), 256, 0, st>>>(dz.f(), rp, V, H, dGB.f());
     TFGNN_LAUNCH_CHECK();
-    // 4. dW_l = [A_l | T_l]^T dQ_l,  dF_l = h_v^T [dgamma_l | dbeta_l]
+    // 4. dW_l = [A_l | T_l]^T dQ_l,  dF_l = z_l^T [dgamma_l | dbeta_l]
     rc = weight_grad(AT.f(), KT, dQ.f(), H, V, KT, H, part.f(), one_table(grad_W[l]), 1, KT, 0, st);
     if (rc) return rc;
-    rc = weight_grad(h_tgt, D, dGB.f(), 2 * H, V, D, 2 * H, part.f(), one_table(grad_film[l]), 1, D, 0, st);
+    rc = weight_grad(zl, ldf, dGB.f(), 2 * H, V, S, 2 * H, part.f(), one_table(grad_film[l]), 1, S, 0, st);
     if (rc) return rc;
+    if (grad_fin) {   // dz_l = [dgamma_l | dbeta_l] F_l^T into type l's columns of grad_fin
+      rc = gemm_transposed(dGB.f(), 2 * H, {one_table(Fl), 1, S, 2 * H}, FT.f(), grad_fin + (size_t)l * fstride, ldf, V,
+                           S, none, st);
+      if (rc) return rc;
+    }
     if (!grad_h) continue;
     // 5. dA_l = dQ_l W^s_l^T into columns [l*D, (l+1)*D) of dA (scaled by s after the loop)
     rc = gemm_transposed(dQ.f(), H, {one_table(Wl), 1, KT, H}, WT.f(), dA.f() + (size_t)l * D, LD, V, D, none, st);
     if (rc) return rc;
-    // 6. target side: dHt (+)= [dgamma_l | dbeta_l] F_l^T (+ coeff(v,l) dQ_l W^t_l^T)
-    GemmEpilogue sum_types;
-    sum_types.accumulate = l > 0;
-    rc = gemm_transposed(dGB.f(), 2 * H, {one_table(Fl), 1, D, 2 * H}, FT.f(), dHt.f(), D, V, D, sum_types, st);
-    if (rc) return rc;
+    // 6. target side: dHt (+)= [dgamma_l | dbeta_l] F_l^T (film_to_h) (+ coeff(v,l) dQ_l W^t_l^T)
+    if (film_to_h) {
+      GemmEpilogue sum_types;
+      sum_types.accumulate = l > 0;
+      rc = gemm_transposed(dGB.f(), 2 * H, {one_table(Fl), 1, D, 2 * H}, FT.f(), dHt.f(), D, V, D, sum_types, st);
+      if (rc) return rc;
+    }
     if (use_target) {   // dT_l overwrites [A_l | T_l] (read for the last time by the dW_l pass above); W^t_l^T is packed
       rc = node_gemm(dQ.f(), H, WT.f() + D, KT, AT.f(), KT, V, D, H, none, TFGNN_PATH_AUTO, st);
       if (rc) return rc;
@@ -899,10 +926,31 @@ extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const fl
   // 7. grad_h[u] = sum over the edges LEAVING u
   rc = reduce_over_sources(bt, dA.f(), LD, D, Vs, grad_h, st);
   if (rc) return rc;
+  if (!target_side) return 0;
   // 8. grad_h[lo + v] += target-side terms
   add_kernel<<<grid_for(V * D), 256, 0, st>>>(grad_h + (size_t)lo * D, dHt.f(), V * D);
   TFGNN_LAUNCH_CHECK();
   return 0;
+}
+
+}  // namespace tfgnn
+
+extern "C" int tfgnn_b200_film_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int32_t D,
+                                   const float* const* mlp_weights, const float* const* film_weights, int32_t H,
+                                   uint32_t flags, int32_t aggregation, int32_t activation, const float* out,
+                                   const float* grad_out, float* grad_h, float* const* grad_W, float* const* grad_film,
+                                   void* stream) {
+  return film_bwd_core(b, bt, h, D, mlp_weights, nullptr, 0, D, film_weights, H, flags, aggregation, activation, out,
+                       grad_out, grad_h, nullptr, grad_W, grad_film, "film_bwd", (cudaStream_t)stream);
+}
+
+extern "C" int tfgnn_b200_film_in_bwd(tfgnn_batch_t* b, tfgnn_batch_t* bt, const float* h, int32_t D,
+                                      const float* const* mlp_weights, const float* film_in, int32_t S,
+                                      const float* const* film_weights, int32_t H, uint32_t flags, int32_t aggregation,
+                                      int32_t activation, const float* out, const float* grad_out, float* grad_h,
+                                      float* grad_film_in, float* const* grad_W, float* const* grad_film, void* stream) {
+  return film_bwd_core(b, bt, h, D, mlp_weights, film_in, S, S, film_weights, H, flags, aggregation, activation,
+                       out, grad_out, grad_h, grad_film_in, grad_W, grad_film, "film_in_bwd", (cudaStream_t)stream);
 }
 
 // =====================================================================================================================

@@ -274,9 +274,10 @@ __global__ void edge_reduce_scalar_kernel(const EdgeReduceParams p) {
 // Target-state term of a 0-hidden-layer edge MLP with use_target_state_as_input
 // (gnn_edge_mlp.py:93-98): sum_e (h_v W^t) / (c+eps) = (c/(c+eps)) * h_v W^t, so the per-(v,l)
 // input row of the node-level contraction is coeff(v,l) * h_v.
+// Type l reads columns [l*in_stride, l*in_stride + D) of h (in_stride 0: every type reads the same row).
 __global__ void target_term_kernel(const float* __restrict__ h, int ldh, const int* __restrict__ row_ptr,
                                    int V, int L, int D, int normalize, float* __restrict__ out, int ldo,
-                                   int col0) {
+                                   int col0, int in_stride) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)V * L * D;
   if (idx >= total) return;
@@ -287,7 +288,7 @@ __global__ void target_term_kernel(const float* __restrict__ h, int ldh, const i
   const long long seg = (long long)l * V + v;
   const float cnt = (float)(row_ptr[seg + 1] - row_ptr[seg]);
   const float coeff = normalize ? cnt * (1.0f / (cnt + kSmallNumber)) : cnt;
-  out[(long long)v * ldo + col0 + (long long)l * D + c] = coeff * h[(long long)v * ldh + c];
+  out[(long long)v * ldo + col0 + (long long)l * D + c] = coeff * h[(long long)v * ldh + (long long)l * in_stride + c];
 }
 
 // float4 version (D, ldh, ldo, col0 multiples of 4, aligned bases): one warp per node, the node's row is read ONCE and
@@ -295,7 +296,8 @@ __global__ void target_term_kernel(const float* __restrict__ h, int ldh, const i
 // GNN-FiLM 1/8 shard, 0.9 TB/s).
 __global__ void __launch_bounds__(256) target_term_vec_kernel(const float* __restrict__ h, int ldh,
                                                               const int* __restrict__ row_ptr, int V, int L, int D,
-                                                              int normalize, float* __restrict__ out, int ldo, int col0) {
+                                                              int normalize, float* __restrict__ out, int ldo, int col0,
+                                                              int in_stride) {
   const int lane = threadIdx.x & 31;
   const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
@@ -304,8 +306,9 @@ __global__ void __launch_bounds__(256) target_term_vec_kernel(const float* __res
     const float* hr = h + v * ldh;
     float* orow = out + v * ldo + col0;
     for (int c4 = lane; c4 < C4; c4 += 32) {
-      const float4 x = ldg_f4(hr + 4 * c4);
+      float4 x = ldg_f4(hr + 4 * c4);
       for (int l = 0; l < L; ++l) {
+        if (in_stride && l) x = ldg_f4(hr + (long long)l * in_stride + 4 * c4);
         const long long seg = (long long)l * V + v;
         const float cnt = (float)(__ldg(row_ptr + seg + 1) - __ldg(row_ptr + seg));
         const float coeff = normalize ? cnt * (1.0f / (cnt + kSmallNumber)) : cnt;
@@ -531,17 +534,19 @@ int launch_edge_grad(const EdgeReduceParams& f, const float* z, const float* dz,
 }
 
 int launch_target_term(const float* h, int ldh, const int* row_ptr, int V, int L, int D, int normalize,
-                       float* out, int ldo, int col0, cudaStream_t st) {
+                       float* out, int ldo, int col0, cudaStream_t st, int in_stride) {
   const long long total = (long long)V * L * D;
   if (total == 0) return 0;
-  if (D % 4 == 0 && ldh % 4 == 0 && ldo % 4 == 0 && col0 % 4 == 0 && aligned16(h) && aligned16(out)) {
+  if (D % 4 == 0 && ldh % 4 == 0 && ldo % 4 == 0 && col0 % 4 == 0 && in_stride % 4 == 0 && aligned16(h) &&
+      aligned16(out)) {
     int blocks = ceil_div((long long)V * 32, 256);
     if (blocks > 132 * 16) blocks = 132 * 16;
-    target_term_vec_kernel<<<blocks, 256, 0, st>>>(h, ldh, row_ptr, V, L, D, normalize, out, ldo, col0);
+    target_term_vec_kernel<<<blocks, 256, 0, st>>>(h, ldh, row_ptr, V, L, D, normalize, out, ldo, col0, in_stride);
     TFGNN_LAUNCH_CHECK();
     return 0;
   }
-  target_term_kernel<<<ceil_div(total, 256), 256, 0, st>>>(h, ldh, row_ptr, V, L, D, normalize, out, ldo, col0);
+  target_term_kernel<<<ceil_div(total, 256), 256, 0, st>>>(h, ldh, row_ptr, V, L, D, normalize, out, ldo, col0,
+                                                            in_stride);
   TFGNN_LAUNCH_CHECK();
   return 0;
 }

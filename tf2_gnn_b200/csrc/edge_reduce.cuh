@@ -40,8 +40,10 @@ int launch_edge_reduce(const EdgeReduceParams& p, bool merged, cudaStream_t st, 
 // with row_ptr_t NULL: dT = d/d f.T over f's own CSR into out [V, L*C].
 int launch_edge_grad(const EdgeReduceParams& f, const float* z, const float* dz, const int* row_ptr_t, const int* tgt,
                      int Vs, float* out, cudaStream_t st);
+// out[v, col0 + l*D + c] = coeff(v,l) h[v, l*in_stride + c], coeff = c_{v,l} or c/(c+eps) (normalize); in_stride 0: one
+// input row for every type (the target-state term), else one input block per type (GNN-FiLM's per-type FiLM input).
 int launch_target_term(const float* h, int ldh, const int* row_ptr, int V, int L, int D, int normalize,
-                       float* out, int ldo, int col0, cudaStream_t st);
+                       float* out, int ldo, int col0, cudaStream_t st, int in_stride = 0);
 int launch_edge_scatter_atomic(const tfgnn_batch* b, const float* X, int ldx, int C, int normalize,
                                float* out, int ldo, int type_stride, cudaStream_t st);
 

@@ -20,6 +20,11 @@ int edge_mlp_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp
 // in_place: out overlaps the caller's state table (the update then keeps the two GEMMs and the gate kernel)
 int gru_update(const float* agg, const float* h, int ldh, const float* gru_kernel, const float* gru_recurrent_kernel,
                const float* gru_bias, long long V, int H, int path, bool in_place, float* out, cudaStream_t st);
+// GNN-FiLM forward (variants.cu) with FiLM input rows fin [V, L*S]: type l reads columns [l*fstride, l*fstride + S) through
+// film_weights[l] [S, 2H]; fstride 0 with fin = the owned rows of h [V, D] and S = D is tfgnn_b200_film_fwd
+int film_fwd_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int num_hidden_layers,
+                  const float* fin, int fstride, int S, const float* const* film_weights, int H, uint32_t flags,
+                  int aggregation, int activation, int path, float* out, cudaStream_t st);
 // literal per-edge path (literal.cu); FB = optional FiLM table [V, L*2H] (gamma | beta per type)
 int edge_mlp_literal(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int n_hidden, int H,
                      uint32_t flags, int aggregation, int activation, const float* FB, int ldf, int path, float* out,

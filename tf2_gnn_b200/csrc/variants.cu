@@ -149,22 +149,23 @@ extern "C" int tfgnn_b200_rgin_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   return 0;
 }
 
-extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, const float* const* mlp_weights,
-                                   int32_t num_hidden_layers, const float* const* film_weights, int32_t H,
-                                   uint32_t flags, int32_t aggregation, int32_t activation, int32_t path,
-                                   float* out, void* stream) {
-  TFGNN_REQUIRE(b != nullptr, "batch is NULL");
-  TFGNN_REQUIRE(D > 0 && H > 0, "D and H must be positive");
-  TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), "unknown activation / aggregation code");
+namespace tfgnn {
+
+// GNN-FiLM forward (gnn_film.py:83-108) with its FiLM MLPs' last layer fed from `fin` (the owned targets' rows): type l
+// reads columns [l*fstride, l*fstride + S) through film_weights[l] [S, 2H]; fin has L*S columns.  fstride 0: every type
+// reads the same S = D columns of the layer's own target state (tfgnn_b200_film_fwd; fin then has D columns).  The scalar
+// arguments and fin are checked by the entries.
+int film_fwd_core(tfgnn_batch* b, const float* h, int D, const float* const* mlp_weights, int num_hidden_layers,
+                  const float* fin, int fstride, int S, const float* const* film_weights, int H, uint32_t flags,
+                  int aggregation, int activation, int path, float* out, cudaStream_t st) {
   const int V = (int)b->V, L = b->L;
   if (V == 0) return 0;
-  if (L == 0)
-    return edge_mlp_core(b, h, D, mlp_weights, 0, H, flags, aggregation, activation, path, out, H,
-                         (cudaStream_t)stream);
+  if (L == 0) return edge_mlp_core(b, h, D, mlp_weights, 0, H, flags, aggregation, activation, path, out, H, st);
   TFGNN_REQUIRE(mlp_weights && film_weights, "weight table is NULL");
   TFGNN_REQUIRE(num_hidden_layers >= 0, "num_hidden_layers must be >= 0");
+  TFGNN_REQUIRE((long long)L * S < (1ll << 31), "L * S overflows");
+  const int ldf = fstride ? L * S : D;   // columns of fin
   if (path == TFGNN_PATH_ATOMIC) return unsupported("TFGNN_PATH_ATOMIC is not available for GNN-FiLM");
-  cudaStream_t st = (cudaStream_t)stream;
   const bool normalize = flags & TFGNN_FLAG_NORMALIZE_BY_NUM_INCOMING;
   const bool act_before = flags & TFGNN_FLAG_ACT_BEFORE_AGGREGATION;
   const bool use_target = flags & TFGNN_FLAG_USE_TARGET_STATE;
@@ -188,7 +189,8 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   const size_t projected_bytes = ((size_t)b->V_src * L * H + (size_t)V * 2 * L * H) * sizeof(float);
   const bool film_att = film_att_env >= 0 ? film_att_env != 0 : (sharded_batch || projected_bytes > ((size_t)20 << 30));   // a quarter of 80 GB
   if (film_att && num_hidden_layers == 0 && aggregation != TFGNN_AGG_MAX && !act_before && D % 4 == 0 && H % 4 == 0 &&
-      (reinterpret_cast<uintptr_t>(h) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) {
+      S % 4 == 0 && ldf % 4 == 0 && (reinterpret_cast<uintptr_t>(h) & 15) == 0 &&
+      (reinterpret_cast<uintptr_t>(fin) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) {
     // ---- aggregate-then-transform ---------------------------------------------------------------------------
     // Every per-edge quantity of gnn_film.py:83-108 but h_u depends on (target, type) only, so
     //   sum_{e in A_l -> v} gamma_l(v) * (s W_l h_u [+ s W^t_l h_v]) + beta_l(v)
@@ -198,10 +200,10 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     // (C += gamma * acc): no [V, L*H] projected table, no [V, 2*L*H] FiLM table, and on a target-range shard only
     // the OWNED rows are ever multiplied (the transform-then-aggregate form projects all num_nodes_total sources on
     // every rank: 123 GB per rank at BASELINE config 5).
-    const int K = L * D;
+    const int K = L * D, KB = L * S;   // columns of A (and of the target-state operand), of the beta operand
     PoolBuffer A{st}, T{st};
     rc = A.alloc((size_t)V * K * sizeof(float));
-    if (!rc) rc = T.alloc((size_t)V * K * sizeof(float));
+    if (!rc) rc = T.alloc((size_t)V * (K > KB ? K : KB) * sizeof(float));
     if (rc) return rc;
     {
       EdgeReduceParams p;
@@ -212,36 +214,46 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
       rc = launch_edge_reduce(p, /*merged=*/false, st);
       if (rc) return rc;
     }
-    // beta part: out = [c_0 h_v | .. | c_{L-1} h_v] [Fbeta_0; ..; Fbeta_{L-1}]   (one K = L*D contraction, not finalised)
-    rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, /*normalize=*/0, T.f(), K, 0, st);
+    // beta part: out = [c_0 z_0 | .. | c_{L-1} z_{L-1}] [Fbeta_0; ..; Fbeta_{L-1}] with z_l = type l's FiLM input (h_v for
+    // fstride 0): one L*S contraction, not finalised
+    rc = launch_target_term(fin, ldf, b->row_ptr, V, L, S, /*normalize=*/0, T.f(), KB, 0, st, fstride);
     if (rc) return rc;
     {
       PoolBuffer Fb{st};
       PtrTable fbeta{};
       for (int l = 0; l < L; ++l) fbeta.p[l] = reinterpret_cast<const float*>(film.p[l]) + H;
-      rc = Fb.alloc((size_t)K * H * sizeof(float));
-      if (!rc) rc = launch_pack_vertical(fbeta, L, 0, D, H, 2 * H, Fb.f(), H, 0, st);
+      rc = Fb.alloc((size_t)KB * H * sizeof(float));
+      if (!rc) rc = launch_pack_vertical(fbeta, L, 0, S, H, 2 * H, Fb.f(), H, 0, st);
       if (rc) return rc;
       GemmEpilogue raw;
       raw.finalize = 0;
-      rc = node_gemm(T.f(), K, Fb.f(), H, out, H, V, H, K, raw, path, st);
+      rc = node_gemm(T.f(), KB, Fb.f(), H, out, H, V, H, KB, raw, path, st);
       if (rc) return rc;
     }
-    if (use_target && normalize) {   // coeff(v,l) h_v with the normalised coefficient (the beta operand used the raw count)
-      rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, 1, T.f(), K, 0, st);
+    // the target-state operand [coeff(v,l) h_v]: the beta operand is it only for fstride 0 without normalisation (the
+    // beta operand uses the raw count)
+    if (use_target && (normalize || fstride)) {
+      rc = launch_target_term(h_tgt, D, b->row_ptr, V, L, D, normalize, T.f(), K, 0, st);
       if (rc) return rc;
     }
     // gamma for all types in ONE wide contraction: Gall [V, L*H] = h_v [Fgamma_0 | .. | Fgamma_{L-1}] (128-column tiles:
     // the k-block rate of the GEMM pipeline is latency-bound, so work per k-block ~ tile width; 6 GEMMs of N = 320 ran in
-    // 80-column tiles at 4.7 ms each, the wide one takes about half of their sum)
+    // 80-column tiles at 4.7 ms each, the wide one takes about half of their sum).  Per-type inputs: one GEMM per type,
+    // z_l Fgamma_l into columns [l*H, (l+1)*H).
     const int LHw = L * H;
     PoolBuffer Gall{st};
-    {
+    rc = Gall.alloc((size_t)V * LHw * sizeof(float));
+    if (rc) return rc;
+    if (fstride == 0) {
       PoolBuffer Fg{st};
-      rc = Gall.alloc((size_t)V * LHw * sizeof(float));
-      if (!rc) rc = Fg.alloc((size_t)D * LHw * sizeof(float));
-      if (!rc) rc = launch_pack_horizontal(film, L, 0, D, H, 2 * H, Fg.f(), LHw, st);   // first H columns of every F_l [D, 2H]
-      if (!rc) rc = node_gemm(h_tgt, D, Fg.f(), LHw, Gall.f(), LHw, V, LHw, D, none, path, st);
+      rc = Fg.alloc((size_t)S * LHw * sizeof(float));
+      if (!rc) rc = launch_pack_horizontal(film, L, 0, S, H, 2 * H, Fg.f(), LHw, st);   // first H columns of every F_l [S, 2H]
+      if (!rc) rc = node_gemm(fin, ldf, Fg.f(), LHw, Gall.f(), LHw, V, LHw, S, none, path, st);
+      if (rc) return rc;
+    } else {
+      for (int l = 0; l < L && !rc; ++l)
+        rc = node_gemm(fin + (size_t)l * fstride, ldf, reinterpret_cast<const float*>(film.p[l]), 2 * H,
+                       Gall.f() + (size_t)l * H, LHw, V, H, S, none, path, st);
       if (rc) return rc;
     }
     for (int l = 0; l < L; ++l) {
@@ -271,14 +283,22 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
     }
     return 0;
   }
-  // FiLM parameters [gamma_l | beta_l] = h F_l depend on (target, type) only (gnn_film.py:99-103)
+  // FiLM parameters [gamma_l | beta_l] = z_l F_l depend on (target, type) only (gnn_film.py:99-103); z_l = h_v for
+  // fstride 0 (one wide GEMM), else type l's block of fin (one GEMM per type)
   PoolBuffer FB{st};
   auto film_parameters = [&]() {
-    PoolBuffer Fcat{st};
     int r = FB.alloc((size_t)V * 2 * LH * sizeof(float));
-    if (!r) r = Fcat.alloc((size_t)D * 2 * LH * sizeof(float));
-    if (!r) r = launch_pack_horizontal(film, L, 0, D, 2 * H, 2 * H, Fcat.f(), 2 * LH, st);
-    return r ? r : node_gemm(h_tgt, D, Fcat.f(), 2 * LH, FB.f(), 2 * LH, V, 2 * LH, D, none, path, st);
+    if (r) return r;
+    if (fstride) {
+      for (int l = 0; l < L && !r; ++l)
+        r = node_gemm(fin + (size_t)l * fstride, ldf, reinterpret_cast<const float*>(film.p[l]), 2 * H,
+                      FB.f() + (size_t)l * 2 * H, 2 * LH, V, 2 * H, S, none, path, st);
+      return r;
+    }
+    PoolBuffer Fcat{st};
+    r = Fcat.alloc((size_t)S * 2 * LH * sizeof(float));
+    if (!r) r = launch_pack_horizontal(film, L, 0, S, 2 * H, 2 * H, Fcat.f(), 2 * LH, st);
+    return r ? r : node_gemm(fin, ldf, Fcat.f(), 2 * LH, FB.f(), 2 * LH, V, 2 * LH, S, none, path, st);
   };
   if (num_hidden_layers > 0) {
     // hidden layers in the edge MLP: FiLM parameters at node level, messages on the literal per-edge path
@@ -316,6 +336,32 @@ extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, 
   p.row_norm = agg_row_norm(aggregation);
   p.final_act = act_before ? TFGNN_ACT_NONE : activation;
   return launch_edge_reduce(p, /*merged=*/true, st);
+}
+
+}  // namespace tfgnn
+
+extern "C" int tfgnn_b200_film_fwd(tfgnn_batch_t* b, const float* h, int32_t D, const float* const* mlp_weights,
+                                   int32_t num_hidden_layers, const float* const* film_weights, int32_t H,
+                                   uint32_t flags, int32_t aggregation, int32_t activation, int32_t path,
+                                   float* out, void* stream) {
+  TFGNN_REQUIRE(b != nullptr, "batch is NULL");
+  TFGNN_REQUIRE(D > 0 && H > 0, "D and H must be positive");
+  TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), "unknown activation / aggregation code");
+  const float* h_tgt = h ? h + (size_t)b->tgt_off * D : nullptr;
+  return film_fwd_core(b, h, D, mlp_weights, num_hidden_layers, h_tgt, 0, D, film_weights, H,
+                       flags, aggregation, activation, path, out, (cudaStream_t)stream);
+}
+
+extern "C" int tfgnn_b200_film_in_fwd(tfgnn_batch_t* b, const float* h, int32_t D, const float* const* mlp_weights,
+                                      int32_t num_hidden_layers, const float* film_in, int32_t S,
+                                      const float* const* film_weights, int32_t H, uint32_t flags, int32_t aggregation,
+                                      int32_t activation, int32_t path, float* out, void* stream) {
+  TFGNN_REQUIRE(b != nullptr, "film_in_fwd: batch is NULL");
+  TFGNN_REQUIRE(D > 0 && H > 0 && S > 0, "film_in_fwd: D, H and S must be positive");
+  TFGNN_REQUIRE(valid_act(activation) && valid_agg(aggregation), "film_in_fwd: unknown activation / aggregation code");
+  TFGNN_REQUIRE(film_in || b->V == 0 || b->L == 0, "film_in_fwd: film_in is NULL");
+  return film_fwd_core(b, h, D, mlp_weights, num_hidden_layers, film_in, S, S, film_weights, H, flags,
+                       aggregation, activation, path, out, (cudaStream_t)stream);
 }
 
 namespace tfgnn {

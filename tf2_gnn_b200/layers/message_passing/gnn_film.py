@@ -7,9 +7,10 @@ import torch
 
 from ... import _ffi
 from ...runtime import PreparedBatch, stream_ptr
+from ...utils.param_helpers import get_activation_function
 from .gnn_edge_mlp import EdgeMLP, GNN_Edge_MLP
 from ..differentiable import edge_mlp_family_forward
-from ..node_ops import _needs_grad
+from ..node_ops import _needs_grad, dense
 from .message_passing import MessagePassingInput, _last_dim, register_message_passing_implementation
 
 
@@ -45,6 +46,42 @@ class _FilmLayerFunction(torch.autograd.Function):
         return (grad_h, None, None, *grad_w)
 
 
+class _FilmInLayerFunction(torch.autograd.Function):
+    """Autograd hook of the FiLM layer with hidden FiLM-MLP layers: forward = tfgnn_b200_film_in_fwd, backward =
+    tfgnn_b200_film_in_bwd.  film_in [V, L*S] holds every type's last hidden FiLM activation z_l (computed at node level by
+    the caller, whose Dense ops differentiate the hidden chain); weights = the L edge-MLP kernels, then the L last FiLM
+    kernels [S, 2H]."""
+
+    @staticmethod
+    def forward(ctx, h, film_in, prepared, cfg, *weights):
+        L = len(weights) // 2
+        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+        _ffi.check(_ffi.lib().tfgnn_b200_film_in_fwd(
+            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights[:L]), 0, film_in.data_ptr(), cfg["S"],
+            _ffi.ptr_array(weights[L:]), cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(),
+            stream_ptr()))
+        ctx.prepared, ctx.cfg = prepared, cfg
+        ctx.save_for_backward(h, film_in, out, *weights)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        h, film_in, out, *weights = ctx.saved_tensors
+        cfg, prepared = ctx.cfg, ctx.prepared
+        L = len(weights) // 2
+        grad_out = grad_out.contiguous()
+        grad_h = torch.empty_like(h) if ctx.needs_input_grad[0] else None
+        grad_in = torch.empty_like(film_in) if ctx.needs_input_grad[1] else None
+        grad_w = [torch.empty_like(w) for w in weights]
+        _ffi.check(_ffi.lib().tfgnn_b200_film_in_bwd(
+            prepared.handle, prepared.transposed().handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights[:L]),
+            film_in.data_ptr(), cfg["S"], _ffi.ptr_array(weights[L:]), cfg["H"], cfg["flags"], cfg["agg"], cfg["act"],
+            out.data_ptr(), grad_out.data_ptr(), grad_h.data_ptr() if grad_h is not None else None,
+            grad_in.data_ptr() if grad_in is not None else None, _ffi.ptr_array(grad_w[:L]), _ffi.ptr_array(grad_w[L:]),
+            stream_ptr()))
+        return (grad_h, grad_in, None, None, *grad_w)
+
+
 @register_message_passing_implementation
 class GNN_FiLM(GNN_Edge_MLP):
     """h'_v = sum_l sum_{(u,v) in A_l} sigma(1/c_{v,l} * gamma_{l,v} * (W_l h_u) + beta_{l,v}),
@@ -70,44 +107,84 @@ class GNN_FiLM(GNN_Edge_MLP):
     def build(self, input_shapes: MessagePassingInput):
         D = _last_dim(input_shapes.node_embeddings)
         for i in range(len(input_shapes.adjacency_lists)):
+            # an int is that many hidden layers of width 2H, as dpu_utils' MLP builds them
+            hidden = self._film_parameter_MLP_hidden_layers
             self._edge_type_film_layer_computations.append(
                 EdgeMLP(self, f"edge_type_{i}-FiLM", D, 2 * self._hidden_dim,
-                        list(self._film_parameter_MLP_hidden_layers)))
+                        hidden if isinstance(hidden, int) else list(hidden)))
         super().build(input_shapes)
 
     def call(self, inputs: MessagePassingInput, training: bool = False,
              prepared: Optional[PreparedBatch] = None):
         h, prepared = self._device_inputs(inputs, prepared)
         self._check_types(prepared)
+        act = self._activation_fn.code if self._activation_fn is not None else _ffi.ACT[None]
+        cfg = dict(H=self._hidden_dim, flags=self._flags(), agg=self._aggregation_fn.code, act=act,
+                   path=_ffi.PATH[self._path])
+        film_hidden = any(m.num_hidden_layers for m in self._edge_type_film_layer_computations)
         if _needs_grad(h, *[v.value for v in self.variables]):
             if self._has_fused_backward(int(h.shape[1])):
-                act = self._activation_fn.code if self._activation_fn is not None else _ffi.ACT[None]
-                cfg = dict(H=self._hidden_dim, flags=self._flags(), agg=self._aggregation_fn.code, act=act,
-                           path=_ffi.PATH[self._path])
                 weights = ([m.layers[0].value for m in self._edge_type_mlps]
                            + [m.layers[0].value for m in self._edge_type_film_layer_computations])
                 return _FilmLayerFunction.apply(h, prepared, cfg, *weights)
-            # hidden layers / max aggregation / activation before aggregation: the reference's literal op order with
-            # per-op backward kernels (layers/differentiable.py)
+            if film_hidden and self._has_fused_film_mlp_backward(int(h.shape[1]), prepared):
+                film_in = self._film_inputs(h, prepared)
+                weights = ([m.layers[0].value for m in self._edge_type_mlps]
+                           + [m.layers[-1].value for m in self._edge_type_film_layer_computations])
+                return _FilmInLayerFunction.apply(h, film_in, prepared, dict(cfg, S=self._film_input_width()), *weights)
+            # edge-MLP hidden layers / max aggregation / activation before aggregation / widths that are not multiples of
+            # 4 / target-range shards: the reference's literal op order with per-op backward kernels
+            # (layers/differentiable.py)
             return edge_mlp_family_forward(
                 self, h, prepared,
                 film_kernels=[[v.value for v in m.layers] for m in self._edge_type_film_layer_computations])
-        if any(m.num_hidden_layers for m in self._edge_type_film_layer_computations):
-            raise NotImplementedError("film_parameter_MLP_hidden_layers != [] is not built yet")
         out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
         ptrs, _keep = self._mlp_weight_ptrs()
-        film = [m.layers[0].value for m in self._edge_type_film_layer_computations]
+        film = [m.layers[-1].value for m in self._edge_type_film_layer_computations]
+        if film_hidden:
+            film_in = self._film_inputs(h, prepared)
+            _ffi.check(_ffi.lib().tfgnn_b200_film_in_fwd(
+                prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, int(self._num_edge_MLP_hidden_layers),
+                film_in.data_ptr(), self._film_input_width(), _ffi.ptr_array(film), self._hidden_dim, self._flags(),
+                cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+            return out
         _ffi.check(_ffi.lib().tfgnn_b200_film_fwd(
             prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, int(self._num_edge_MLP_hidden_layers),
             _ffi.ptr_array(film), self._hidden_dim, self._flags(), self._aggregation_fn.code,
             self._activation_fn.code, _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
         return out
 
+    def _film_input_width(self) -> int:
+        """S: the width of the last hidden FiLM-MLP layer (the same for every type)."""
+        return int(self._edge_type_film_layer_computations[0].layers[-1].value.shape[0])
+
+    def _film_inputs(self, h: torch.Tensor, prepared: PreparedBatch) -> torch.Tensor:
+        """[V_owned, L*S]: type l's hidden FiLM-MLP chain z_l = relu(.. relu(h_v F^(0)_l) ..) on the owned target rows
+        (gnn_film.py:99-101 evaluates it on every edge's gathered target row; it depends on the target only)."""
+        relu = get_activation_function("relu")
+        lo, hi = prepared.target_range
+        rows = h[lo:hi]
+        zs = []
+        for m in self._edge_type_film_layer_computations:
+            z = rows
+            for var in m.layers[:-1]:
+                z = dense(z, var.value, None, relu)
+            zs.append(z)
+        return torch.cat(zs, dim=1)
+
     def _has_fused_backward(self, D: int) -> bool:
         """The configurations tfgnn_b200_film_bwd differentiates (the reference's PPI_GNN_FiLM.json among them)."""
-        return (int(self._num_edge_MLP_hidden_layers) == 0 and not list(self._film_parameter_MLP_hidden_layers)
+        return (int(self._num_edge_MLP_hidden_layers) == 0
+                and not any(m.num_hidden_layers for m in self._edge_type_film_layer_computations)
                 and self._aggregation_fn.name != "max" and not self._message_activation_before_aggregation
                 and D % 4 == 0 and self._hidden_dim % 4 == 0)
+
+    def _has_fused_film_mlp_backward(self, D: int, prepared: PreparedBatch) -> bool:
+        """The configurations with hidden FiLM-MLP layers that tfgnn_b200_film_in_bwd differentiates, on whole batches."""
+        return (int(self._num_edge_MLP_hidden_layers) == 0
+                and self._aggregation_fn.name != "max" and not self._message_activation_before_aggregation
+                and D % 4 == 0 and self._hidden_dim % 4 == 0 and self._film_input_width() % 4 == 0
+                and prepared.target_range == (0, prepared.num_source_nodes))
 
     def set_weights_from_oracle_dict(self, w: Dict[str, Any]) -> None:
         super().set_weights_from_oracle_dict(w)

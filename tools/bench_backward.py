@@ -1,6 +1,7 @@
 """Measurement of the backward pass (SURVEY.md §8f-1) at bench.py's workloads: forward and backward device time of one
 RGCN, GGNN or GNN-FiLM layer through the autograd hook, CUDA events, inputs resident in HBM.
   python tools/bench_backward.py [--workload cfg2] [--steps 10] [--warmup 3] [--shards N] [--film-literal]
+                                 [--film-hidden WIDTHS]
                                  [--kind rgin|gnn_edge_mlp|ggnn] [--literal]
                                  [--aggregation sum|mean|sqrt_n|max] [--act-before] [--activation NAME]
   python tools/bench_backward.py --kind rgat --literal [--steps 5] [--warmup 2]
@@ -11,6 +12,9 @@ For GNN-FiLM the line also carries the device memory in use after the steps (the
 their high-water marks, so this is the peak of the run, inputs included).
 With --film-literal: a reduced FiLM graph on which the literal per-edge path (layers/differentiable.py) fits, 250k nodes /
 6 x 666,667 edges / D = H = 320, with the fused and the literal training step alternated in one process.
+With --film-hidden WIDTHS (e.g. 320 or 320,160): hidden FiLM-MLP layers of those widths (film_parameter_MLP_hidden_layers) in
+the GNN-FiLM layer of --film-literal or of a GNN-FiLM workload (--workload cfg5_shard): the fused path is then the hidden
+chain at node level feeding tfgnn_b200_film_in_fwd / _bwd; the line names the autograd function that trained the layer.
 --workload cfg3 is RGAT (tfgnn_b200_rgat_bwd); with --kind rgat --literal: cfg3's graph and layer shape reduced to 250k
 nodes / 3 x 1M edges, where the literal per-edge path fits, with the fused and the literal step alternated in one process.
 With --kind rgin|gnn_edge_mlp|ggnn: that layer (class defaults, one hidden layer in the edge MLPs; RGIN normalised as in
@@ -46,6 +50,9 @@ def main():
     ap.add_argument("--shards", type=int, default=0, help="time the backward of each of N target-range shards")
     ap.add_argument("--film-literal", action="store_true",
                     help="fused vs literal GNN-FiLM training step on a reduced graph the literal path fits")
+    ap.add_argument("--film-hidden", type=lambda s: [int(x) for x in s.split(",")], default=None, metavar="WIDTHS",
+                    help="comma-separated widths of hidden FiLM-MLP layers for the GNN-FiLM layer (--film-literal or a "
+                         "gnn_film workload)")
     ap.add_argument("--kind", choices=sorted(EDGE_MLP_KINDS) + ["rgat"],
                     help="time this layer kind (class defaults, one hidden layer of width H) on the workload's graph "
                          "instead of the workload's own layer; rgat only with --literal (--workload cfg3 is RGAT)")
@@ -71,6 +78,8 @@ def main():
             ap.error("--kind ggnn has no --literal comparison")
         return bench_edge_mlp_literal(args)
     wl = bench.WORKLOADS[args.workload]
+    if args.film_hidden and (args.kind or wl["kind"]) != "gnn_film":
+        ap.error("--film-hidden goes with --film-literal or a gnn_film workload (cfg5, cfg5_shard)")
     V, H, L = wl["V"], wl["H"], len(wl["E"])
     h_np, adjs_np, w_np = bench.make_inputs(wl, seed=0)
     kind = args.kind or wl["kind"]
@@ -79,6 +88,8 @@ def main():
     params = cls.get_default_hyperparameters()
     params.update(EDGE_MLP_KINDS[kind] if args.kind else wl.get("params", {}))
     params.update(hidden_dim=H, **config_overrides(args))
+    if args.film_hidden:
+        params["film_parameter_MLP_hidden_layers"] = args.film_hidden
     layer = cls(params)
     torch.manual_seed(1)
     layer.build(MessagePassingInput((None, H), tuple((None, 2) for _ in range(L))))
@@ -108,6 +119,8 @@ def main():
         if i >= args.warmup:
             fwd_ms.append(e0.elapsed_time(e1))
             bwd_ms.append(e1.elapsed_time(e2))
+    trained_by = type(out.grad_fn).__name__
+    del out
     M = sum(wl["E"])
     rec = {
         "workload": wl["desc"], "kind": kind, "forward_ms": float(np.median(fwd_ms)), "backward_ms": float(np.median(bwd_ms)),
@@ -123,6 +136,10 @@ def main():
     if config_overrides(args):
         rec["overrides"] = config_overrides(args)
         rec["note"] = NOTES["transform_aggregate"]
+    if args.film_hidden:
+        rec["film_parameter_MLP_hidden_layers"] = args.film_hidden
+        rec["trained_by"] = trained_by
+        rec["note"] = NOTES["gnn_film_mlp"]
     if kind in ("gnn_film", "rgat") + tuple(EDGE_MLP_KINDS) or config_overrides(args):
         rec["device_memory_used_GB"] = device_used_gb()
     print(json.dumps(rec), flush=True)
@@ -174,6 +191,10 @@ NOTES = {
     "gnn_film": "backward = per type: recompute [A_l | T_l] (CSR reduce), dQ_l and dgamma_l (tensor-core GEMMs with the dZ "
                 "multiply in the epilogue), dW_l and dF_l (TN GEMMs, fp32 FFMA), dA_l and the target-side terms "
                 "(tensor-core GEMMs); then one source-keyed CSR reduce for dh; autograd hook overhead included",
+    "gnn_film_mlp": "hidden FiLM-MLP layers: forward = the hidden chain (Dense + ReLU per layer and type, node level), its "
+                    "last activations concatenated to [V, L*S], then the FiLM layer fed them (tfgnn_b200_film_in_fwd); "
+                    "backward = the FiLM layer's (tfgnn_b200_film_in_bwd, as gnn_film with z_l for h_v) and the chain's "
+                    "Dense backward; autograd hook overhead included",
     "rgat": "backward = recompute P = h W and the score halves (the forward's GEMM), target pass (one online-softmax walk "
             "per target, hubs in chunk-ordered partials), source pass over the source-keyed CSR (dP, ds_src), attention "
             "gradients (fixed row chunks), dW (TN), grad_h (tensor-core GEMM, K = L*H); no float atomics; autograd hook "
@@ -209,14 +230,18 @@ def release_memory():
 
 
 def bench_film_literal(args):
-    """Fused (tfgnn_b200_film_bwd) vs literal (layers/differentiable.py) GNN-FiLM training step, alternated step by step."""
+    """Fused (tfgnn_b200_film_bwd, or with --film-hidden the node-level chain and tfgnn_b200_film_in_bwd) vs literal
+    (layers/differentiable.py) GNN-FiLM training step, alternated step by step."""
     from tf2_gnn_b200.layers.differentiable import edge_mlp_family_forward
     wl = dict(V=250_000, E=[666_667] * 6, H=320, kind="gnn_film", graph="er",
               desc="GNN-FiLM reduced graph: 250k nodes / 4M edges / 6 edge types, D = H = 320 (class defaults)")
     V, H, L = wl["V"], wl["H"], len(wl["E"])
     h_np, adjs_np, _ = bench.make_inputs(wl, seed=0)
+    hidden = args.film_hidden or []
+    if hidden:
+        wl["desc"] += f", hidden FiLM-MLP layers {hidden}"
     layer = get_message_passing_class("gnn_film")(dict(get_message_passing_class("gnn_film").get_default_hyperparameters(),
-                                                       hidden_dim=H))
+                                                       hidden_dim=H, film_parameter_MLP_hidden_layers=hidden))
     torch.manual_seed(1)
     layer.build(MessagePassingInput((None, H), tuple((None, 2) for _ in range(L))))
     for v in layer.variables:
@@ -232,6 +257,7 @@ def bench_film_literal(args):
              "literal": lambda: edge_mlp_family_forward(layer, h, prepared, film_kernels=film)}
     ms = {k: ([], []) for k in paths}
     mem = {k: 0.0 for k in paths}
+    trained_by = {}
     for i in range(args.warmup + args.steps):
         for name, fwd in paths.items():
             release_memory()
@@ -246,6 +272,7 @@ def bench_film_literal(args):
             e2.record()
             torch.cuda.synchronize()
             mem[name] = max(mem[name], device_used_gb())
+            trained_by[name] = type(out.grad_fn).__name__
             del out
             if i >= args.warmup:
                 ms[name][0].append(e0.elapsed_time(e1))
@@ -253,7 +280,7 @@ def bench_film_literal(args):
     print(json.dumps({
         "workload": wl["desc"], "kind": "gnn_film", "steps": args.steps, "card": card(),
         "paths": {k: {"forward_ms": float(np.median(f)), "backward_ms": float(np.median(b)),
-                      "device_memory_used_GB": mem[k]} for k, (f, b) in ms.items()},
+                      "device_memory_used_GB": mem[k], "trained_by": trained_by[k]} for k, (f, b) in ms.items()},
         "note": "alternated step by step in one process; memory = device memory in use after the step with the library's "
                 "pool and torch's allocator cache emptied before it (their high-water mark for that path, inputs included)"}),
         flush=True)
