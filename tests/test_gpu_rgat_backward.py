@@ -188,6 +188,19 @@ def test_fused_matches_literal_path(case):
         assert_states_close(b, r, tol=TOL)
 
 
+@pytest.mark.parametrize("route", ["inference", "fused", "literal"])
+def test_every_route_rejects_a_batch_with_other_edge_types(route):
+    """The layer checks its shapes before it picks a path: inference, the fused backward and the literal path (D not a
+    multiple of 4) raise the same ValueError."""
+    _need_gpu()
+    from tf2_gnn_b200.layers import MessagePassingInput
+    p, adjs, h, w, _ = _inputs((4, 8, 18 if route == "literal" else 32, 3, "tanh", False), seed=51)
+    layer, _ = _layer(p, h.shape[1], len(adjs), w)
+    ht = torch.from_numpy(h).cuda().requires_grad_(route != "inference")
+    with pytest.raises(ValueError, match="number of adjacency lists"):
+        layer(MessagePassingInput(ht, tuple(torch.from_numpy(a).cuda() for a in adjs[:-1])))
+
+
 @pytest.mark.parametrize("case", [(4, 32, 64, 3, "relu", True), (3, 80, 16, 2, None, True), (8, 4, 12, 4, "tanh", False)])
 def test_rgat_shard_backward_sums_to_full(case):
     """Worlds of 2 and 3 and a world with an empty middle shard (test_gpu_shard_backward._check_shards).  Each shard runs its

@@ -32,39 +32,25 @@ def _f32(shape, like):
 
 
 # ---- gather / segment reduce (adjoint pair) ---------------------------------------------------------------------
-def _gather_rows(table: torch.Tensor, adj: torch.Tensor, column: int) -> torch.Tensor:
-    """table[adj[:, column]] — tf.nn.embedding_lookup (message_passing.py:197-206)."""
-    E, D = int(adj.shape[0]), int(table.shape[1])
-    out = _f32((E, D), table)
-    if E:
-        _ffi.check(_ffi.lib().tfgnn_b200_gather_rows(table.data_ptr(), int(table.shape[0]), D, adj.data_ptr() + 4 * column, 2,
-                                                     E, out.data_ptr(), stream_ptr()))
-    return out
-
-
-def _segment_sum_by(adj: torch.Tensor, column: int, data: torch.Tensor, num_segments: int) -> torch.Tensor:
-    out = _f32((num_segments, int(data.shape[1])), data)
-    _ffi.check(_ffi.lib().tfgnn_b200_unsorted_segment_reduce(
-        data.data_ptr(), adj.data_ptr() + 4 * column, 2, int(data.shape[0]), int(data.shape[1]), num_segments,
-        _ffi.AGG["sum"], out.data_ptr(), stream_ptr()))
-    return out
-
-
 class _GatherFunction(torch.autograd.Function):
+    """table[ids] — tf.nn.embedding_lookup (message_passing.py:197-206) and tf.gather (graph_global_exchange.py:94-96):
+    backward = segment sum."""
+
     @staticmethod
-    def forward(ctx, table, adj, column):
-        ctx.adj, ctx.column, ctx.V = adj, column, int(table.shape[0])
-        return _gather_rows(table.contiguous(), adj, column)
+    def forward(ctx, table, ids, column):
+        ctx.ids, ctx.column, ctx.n = ids, column, int(table.shape[0])
+        return node_ops.gather_rows(table.contiguous(), ids, column)
 
     @staticmethod
     def backward(ctx, g):
-        return _segment_sum_by(ctx.adj, ctx.column, g.contiguous(), ctx.V), None, None
+        return node_ops.segment_sum(g.contiguous(), ctx.ids, ctx.n, ctx.column), None, None
 
 
 def gather(table: torch.Tensor, adj: torch.Tensor, column: int) -> torch.Tensor:
+    """table[adj[:, column]]."""
     if node_ops._needs_grad(table):
         return _GatherFunction.apply(table, adj, column)
-    return _gather_rows(table.contiguous(), adj, column)
+    return node_ops.gather_rows(table.contiguous(), adj, column)
 
 
 class _SegmentReduceFunction(torch.autograd.Function):
@@ -87,23 +73,17 @@ class _SegmentReduceFunction(torch.autograd.Function):
         g = g.contiguous()
         M, H = int(data.shape[0]), int(data.shape[1])
         lib = _ffi.lib()
-        grad = _f32((M, H), data)
         if M == 0:
-            return grad, None, None, None
+            return _f32((M, H), data), None, None, None
         if ctx.agg == "max":
+            grad = _f32((M, H), data)
             _ffi.check(lib.tfgnn_b200_segment_max_bwd(data.data_ptr(), ctx.ids.data_ptr(), 1, out.data_ptr(), g.data_ptr(), M, H,
                                                       ctx.num_segments, grad.data_ptr(), stream_ptr()))
             return grad, None, None, None
-        _ffi.check(lib.tfgnn_b200_gather_rows(g.data_ptr(), ctx.num_segments, H, ctx.ids.data_ptr(), 1, M, grad.data_ptr(),
-                                              stream_ptr()))
+        grad = node_ops.gather_rows(g, ctx.ids)
         if ctx.agg in ("mean", "sqrt_n"):
             ones = torch.ones((M, 1), dtype=torch.float32, device=data.device)
-            counts = _f32((ctx.num_segments, 1), data)
-            _ffi.check(lib.tfgnn_b200_unsorted_segment_reduce(ones.data_ptr(), ctx.ids.data_ptr(), 1, M, 1, ctx.num_segments,
-                                                              _ffi.AGG["sum"], counts.data_ptr(), stream_ptr()))
-            per_msg = _f32((M, 1), data)
-            _ffi.check(lib.tfgnn_b200_gather_rows(counts.data_ptr(), ctx.num_segments, 1, ctx.ids.data_ptr(), 1, M,
-                                                  per_msg.data_ptr(), stream_ptr()))
+            per_msg = node_ops.gather_rows(node_ops.segment_sum(ones, ctx.ids, ctx.num_segments), ctx.ids)
             scaled = _f32((M, H), data)
             _ffi.check(lib.tfgnn_b200_row_scale(grad.data_ptr(), per_msg.data_ptr(), M, H, 2 if ctx.agg == "mean" else 3,
                                                 scaled.data_ptr(), stream_ptr()))
@@ -222,7 +202,7 @@ def edge_mlp_family_forward(layer, h: torch.Tensor, prepared: PreparedBatch, *, 
         x = torch.cat([src, tgt], dim=1) if layer._use_target_state_as_input else src
         m = _mlp(x, [v.value for v in layer._edge_type_mlps[l].layers])  # gnn_edge_mlp.py:100
         if layer._normalize_by_num_incoming:                            # :102-106
-            n_in = _gather_rows(in_degree[l].reshape(V, 1).contiguous(), adj, 1)
+            n_in = node_ops.gather_rows(in_degree[l].reshape(V, 1).contiguous(), adj, 1)
             m = _RowScaleFunction.apply(m, n_in, 1)
         if film_kernels is not None:                                    # gnn_film.py:99-107
             film = _mlp(tgt, film_kernels[l])
@@ -252,37 +232,6 @@ def edge_mlp_family_forward(layer, h: torch.Tensor, prepared: PreparedBatch, *, 
 # Attention / graph-level pieces: RGAT (rgat.py:91-163), readout (nodes_to_graph_representation.py:170-229) and
 # global exchange (graph_global_exchange.py:83-183) in the reference's op order, every op with its adjoint kernel.
 # ==================================================================================================================
-def _ids_gather(table: torch.Tensor, ids: torch.Tensor) -> torch.Tensor:
-    """table[ids] for a contiguous int32 id vector."""
-    M, D = int(ids.shape[0]), int(table.shape[1])
-    out = _f32((M, D), table)
-    if M:
-        _ffi.check(_ffi.lib().tfgnn_b200_gather_rows(table.data_ptr(), int(table.shape[0]), D, ids.data_ptr(), 1, M,
-                                                     out.data_ptr(), stream_ptr()))
-    return out
-
-
-def _ids_segment_sum(data: torch.Tensor, ids: torch.Tensor, num_segments: int) -> torch.Tensor:
-    out = _f32((num_segments, int(data.shape[1])), data)
-    _ffi.check(_ffi.lib().tfgnn_b200_unsorted_segment_reduce(data.data_ptr(), ids.data_ptr(), 1, int(data.shape[0]),
-                                                             int(data.shape[1]), num_segments, _ffi.AGG["sum"], out.data_ptr(),
-                                                             stream_ptr()))
-    return out
-
-
-class _IdsGatherFunction(torch.autograd.Function):
-    """gather_dense_gradient / tf.gather (graph_global_exchange.py:94-96): backward = segment sum."""
-
-    @staticmethod
-    def forward(ctx, table, ids):
-        ctx.ids, ctx.n = ids, int(table.shape[0])
-        return _ids_gather(table.contiguous(), ids)
-
-    @staticmethod
-    def backward(ctx, g):
-        return _ids_segment_sum(g.contiguous(), ctx.ids, ctx.n), None
-
-
 class _AddFunction(torch.autograd.Function):
     """alpha * a + beta * b."""
 
@@ -343,10 +292,10 @@ class _SegmentSoftmaxFunction(torch.autograd.Function):
             seg_max = _f32((num_segments, K), scores)
             _ffi.check(lib.tfgnn_b200_unsorted_segment_reduce(scores.data_ptr(), ids.data_ptr(), 1, M, K, num_segments,
                                                               _ffi.AGG["max"], seg_max.data_ptr(), stream_ptr()))
-            m_e = _ids_gather(seg_max, ids)
+            m_e = node_ops.gather_rows(seg_max, ids)
             e = torch.empty_like(scores)
             _ffi.check(lib.tfgnn_b200_softmax_apply(scores.data_ptr(), m_e.data_ptr(), None, M * K, e.data_ptr(), stream_ptr()))
-            z_e = _ids_gather(_ids_segment_sum(e, ids, num_segments), ids)
+            z_e = node_ops.gather_rows(node_ops.segment_sum(e, ids, num_segments), ids)
             _ffi.check(lib.tfgnn_b200_softmax_apply(scores.data_ptr(), m_e.data_ptr(), z_e.data_ptr(), M * K, alpha.data_ptr(),
                                                     stream_ptr()))
         ctx.ids, ctx.n = ids, num_segments
@@ -362,7 +311,7 @@ class _SegmentSoftmaxFunction(torch.autograd.Function):
         if M:
             t = torch.empty_like(alpha)
             _mul_add(alpha.data_ptr(), K, g.data_ptr(), K, 0, 0, M, K, t.data_ptr(), K)                 # alpha * d_alpha
-            s_e = _ids_gather(_ids_segment_sum(t, ctx.ids, ctx.n), ctx.ids)
+            s_e = node_ops.gather_rows(node_ops.segment_sum(t, ctx.ids, ctx.n), ctx.ids)
             u = torch.empty_like(alpha)
             _mul_add(alpha.data_ptr(), K, s_e.data_ptr(), K, 0, 0, M, K, u.data_ptr(), K)               # alpha * sum
             out = node_ops._axpby(t, 1.0, u, -1.0)
@@ -421,9 +370,7 @@ class _GruGateFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, gx, gh, h):
         gx, gh, h = gx.contiguous(), gh.contiguous(), h.contiguous()
-        out = torch.empty_like(h)
-        _ffi.check(_ffi.lib().tfgnn_b200_gru_gate_fwd(gx.data_ptr(), None, gh.data_ptr(), h.data_ptr(), int(h.shape[0]),
-                                                      int(h.shape[1]), out.data_ptr(), stream_ptr()))
+        out = node_ops.gru_gate_fwd(gx, None, gh, h)
         ctx.save_for_backward(gx, gh, h)
         return out
 
@@ -441,8 +388,7 @@ class _GruGateFunction(torch.autograd.Function):
 def gru_cell(inputs: torch.Tensor, state: torch.Tensor, kernel, recurrent_kernel, bias) -> torch.Tensor:
     """tf.keras.layers.GRUCell (TF2 defaults), differentiable: the direct path of the state through z * h is added to the
     recurrent path by the autograd tape."""
-    gx = node_ops.dense(inputs, kernel, bias[0])
-    gh = node_ops.dense(state, recurrent_kernel, bias[1])
+    gx, gh = node_ops.gru_gate_inputs(inputs, state, kernel, recurrent_kernel, bias)
     return _GruGateFunction.apply(gx, gh, state)
 
 
@@ -472,7 +418,7 @@ def per_node_graph_representations(exchange, x: torch.Tensor, n2g: torch.Tensor,
     rep = exchange._node_to_graph_representation_layer
     rep.dropout_state = exchange.dropout_state
     g = weighted_sum_graph_representation(rep, x, n2g, num_graphs, training)
-    per_node = _IdsGatherFunction.apply(g, n2g)
+    per_node = _GatherFunction.apply(g, n2g, 0)
     if training and exchange._dropout_rate > 0.0:
         per_node = node_ops.dropout(per_node, exchange._dropout_rate, exchange.dropout_state)
     return per_node

@@ -222,10 +222,7 @@ class GNN:
         all_reps = [cur]
         n2g = None
         if self._global_exchange_layers:
-            n2g = inputs.node_to_graph_map
-            if not isinstance(n2g, torch.Tensor):
-                n2g = torch.as_tensor(n2g)
-            n2g = n2g.to(device=feats.device, dtype=torch.int32).contiguous()
+            n2g = node_ops.node_to_graph_index(inputs.node_to_graph_map, feats.device)
         dropout_rate = float(self._params.get("layer_input_dropout_rate", 0.0))
         for layer_idx, mp_layer in enumerate(self._mp_layers):
             if training:                                                             # gnn.py:285-289

@@ -36,13 +36,7 @@ class _ReadoutFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, scores, reprs, n2g, graph_ptr, num_heads, weighting_fun, lower, upper):
-        weights = None
-        if weighting_fun == "softmax":
-            weights = node_ops.segment_softmax(scores, graph_ptr)
-        elif weighting_fun == "sigmoid":
-            weights = torch.empty_like(scores)
-            _ffi.check(_ffi.lib().tfgnn_b200_activation(scores.data_ptr(), scores.numel(), _ffi.ACT_SIGMOID,
-                                                        weights.data_ptr(), stream_ptr()))
+        weights = node_ops.readout_weights(scores, graph_ptr, weighting_fun)
         reprs = reprs.contiguous()
         clamped = reprs if lower is None and upper is None else node_ops.clamp_(reprs.clone(), lower, upper)
         out = node_ops.weighted_segment_sum(clamped, weights, graph_ptr, num_heads, mean=weighting_fun == "average")
@@ -86,13 +80,10 @@ class _ShardReadoutFunction(torch.autograd.Function):
         reprs = reprs.contiguous()
         clamped = reprs if lower is None and upper is None else node_ops.clamp_(reprs.clone(), lower, upper)
         weights = None
-        if weighting_fun == "softmax":
+        if weighting_fun in ("softmax", "sigmoid"):
             scores = scores.contiguous()
-        elif weighting_fun == "sigmoid":
-            scores = scores.contiguous()
-            weights = torch.empty_like(scores)
-            _ffi.check(_ffi.lib().tfgnn_b200_activation(scores.data_ptr(), scores.numel(), _ffi.ACT_SIGMOID,
-                                                        weights.data_ptr(), stream_ptr()))
+        if weighting_fun == "sigmoid":
+            weights = node_ops.sigmoid(scores)
         G, GD, V = int(num_graphs), int(reprs.shape[1]), int(reprs.shape[0])
         K = 1 if weighting_fun == "none" else int(num_heads)
         partial = torch.empty((G, 2 * K + GD), dtype=torch.float32, device=reprs.device)
@@ -122,7 +113,7 @@ class _ShardReadoutFunction(torch.autograd.Function):
         weights = w_saved
         if weighting_fun == "softmax":                    # exp(score - max_g) / sum_g with the merged normaliser
             weights = torch.empty_like(w_saved)
-            m_rows, s_rows = _gather_graph_rows(gmax, n2g), _gather_graph_rows(gsum, n2g)
+            m_rows, s_rows = node_ops.gather_rows(gmax, n2g), node_ops.gather_rows(gsum, n2g)
             _ffi.check(_ffi.lib().tfgnn_b200_softmax_apply(w_saved.data_ptr(), m_rows.data_ptr(), s_rows.data_ptr(),
                                                            weights.numel(), weights.data_ptr(), stream_ptr()))
         grad_reprs = torch.empty_like(reprs)
@@ -147,20 +138,11 @@ def shard_readout(scores: Optional[torch.Tensor], reprs: torch.Tensor, n2g: torc
 
 
 # ---- per-node copies (only where a per-node dropout mask needs them) ----------------------------------------------
-def _gather_graph_rows(table: torch.Tensor, n2g: torch.Tensor) -> torch.Tensor:
-    V, H = int(n2g.shape[0]), int(table.shape[1])
-    out = torch.empty((V, H), dtype=torch.float32, device=table.device)
-    if V:
-        _ffi.check(_ffi.lib().tfgnn_b200_gather_rows(table.data_ptr(), int(table.shape[0]), H, n2g.data_ptr(), 1, V,
-                                                     out.data_ptr(), stream_ptr()))
-    return out
-
-
 class _GatherGraphRowsFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, table, n2g, graph_ptr):
         ctx.index = (n2g, graph_ptr)
-        return _gather_graph_rows(table.contiguous(), n2g)
+        return node_ops.gather_rows(table.contiguous(), n2g)
 
     @staticmethod
     def backward(ctx, grad_out):
@@ -171,7 +153,7 @@ def gather_graph_rows(table: torch.Tensor, n2g: torch.Tensor, graph_ptr: torch.T
     """table[node_to_graph_map] (graph_global_exchange.py:94-96)."""
     if node_ops._needs_grad(table):
         return _GatherGraphRowsFunction.apply(table, n2g, graph_ptr)
-    return _gather_graph_rows(table.contiguous(), n2g)
+    return node_ops.gather_rows(table.contiguous(), n2g)
 
 
 # ---- exchange combines on (x [V, H], per-graph rows [G, .], node_to_graph_map) -------------------------------------
@@ -213,9 +195,7 @@ class _GruGateIndexedFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, gx, gh, h, n2g, graph_ptr):
         gx, gh, h = gx.contiguous(), gh.contiguous(), h.contiguous()
-        out = torch.empty_like(h)
-        _ffi.check(_ffi.lib().tfgnn_b200_gru_gate_fwd(gx.data_ptr(), n2g.data_ptr(), gh.data_ptr(), h.data_ptr(),
-                                                      int(h.shape[0]), int(h.shape[1]), out.data_ptr(), stream_ptr()))
+        out = node_ops.gru_gate_fwd(gx, n2g, gh, h)
         ctx.index = (n2g, graph_ptr)
         ctx.save_for_backward(gx, gh, h)
         return out
@@ -236,6 +216,5 @@ def gru_cell(graph_reprs: torch.Tensor, n2g: torch.Tensor, graph_ptr: torch.Tens
              bias) -> torch.Tensor:
     """GRUCell(inputs=graph_reprs[node_to_graph_map], states=[state]): both input-side GEMMs (forward, and grad of the
     kernel / of graph_reprs in the backward) have G rows."""
-    gx = node_ops.dense(graph_reprs, kernel, bias[0])
-    gh = node_ops.dense(state, recurrent_kernel, bias[1])
+    gx, gh = node_ops.gru_gate_inputs(graph_reprs, state, kernel, recurrent_kernel, bias)
     return _GruGateIndexedFunction.apply(gx, gh, state, n2g, graph_ptr)

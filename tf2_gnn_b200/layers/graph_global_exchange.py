@@ -71,10 +71,7 @@ class GraphGlobalExchange:
         runs on the rank's rows, and graph_ptr indexes those rows.  Every backward step that sums over a graph's rows
         gives the rank's part, which the readout's backward sums over the ranks."""
         x = to_device_f32(inputs.node_embeddings)
-        n2g = inputs.node_to_graph_map
-        if not isinstance(n2g, torch.Tensor):
-            n2g = torch.as_tensor(n2g)
-        n2g = n2g.to(device=x.device, dtype=torch.int32).contiguous()
+        n2g = node_ops.node_to_graph_index(inputs.node_to_graph_map, x.device)
         num_graphs = int(inputs.num_graphs)
         graph_ptr = node_ops.graph_offsets(n2g, num_graphs)
         self._node_to_graph_representation_layer.dropout_state = self.dropout_state

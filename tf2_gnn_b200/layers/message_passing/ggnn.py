@@ -8,8 +8,19 @@ import torch
 from ... import _ffi
 from ...runtime import PreparedBatch, stream_ptr
 from ..differentiable import edge_mlp_family_forward, gru_cell
+from ..node_ops import _needs_grad
 from .gnn_edge_mlp import GNN_Edge_MLP, _EdgeMLPLayerFunction
 from .message_passing import MessagePassingInput, _last_dim, register_message_passing_implementation
+
+
+def _ggnn_forward(h, prepared: PreparedBatch, cfg, gru_kernel, gru_recurrent_kernel, gru_bias, weights) -> torch.Tensor:
+    """tfgnn_b200_ggnn_fwd: the layer's output rows [num_nodes, H]."""
+    out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+    _ffi.check(_ffi.lib().tfgnn_b200_ggnn_fwd(
+        prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights), cfg["n_hidden"], cfg["H"],
+        cfg["flags"], cfg["agg"], gru_kernel.data_ptr(), gru_recurrent_kernel.data_ptr(), gru_bias.data_ptr(),
+        cfg["path"], out.data_ptr(), stream_ptr()))
+    return out
 
 
 class _GGNNFunction(torch.autograd.Function):
@@ -18,11 +29,7 @@ class _GGNNFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, h, prepared, cfg, gru_kernel, gru_recurrent_kernel, gru_bias, *weights):
-        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
-        _ffi.check(_ffi.lib().tfgnn_b200_ggnn_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights), cfg["n_hidden"], cfg["H"],
-            cfg["flags"], cfg["agg"], gru_kernel.data_ptr(), gru_recurrent_kernel.data_ptr(), gru_bias.data_ptr(),
-            cfg["path"], out.data_ptr(), stream_ptr()))
+        out = _ggnn_forward(h, prepared, cfg, gru_kernel, gru_recurrent_kernel, gru_bias, weights)
         ctx.prepared, ctx.cfg = prepared, cfg
         ctx.save_for_backward(h, gru_kernel, gru_recurrent_kernel, gru_bias, *weights)
         return out
@@ -111,22 +118,13 @@ class GGNN(GNN_Edge_MLP):
         self._check_types(prepared)
         if int(h.shape[1]) != self._hidden_dim:
             raise ValueError("GGNN: the node embedding dimension must equal hidden_dim")
+        cfg, weights = self._cfg(), self._mlp_weights()
         gru = (self._gru_kernel.value, self._gru_recurrent_kernel.value, self._gru_bias.value)
-        _ptrs, weights = self._mlp_weight_ptrs()
-        if torch.is_grad_enabled() and (h.requires_grad or any(t.requires_grad for t in (*gru, *weights))):
+        if _needs_grad(h, *gru, *weights):
             if self._ggnn_bwd_takes_it():
-                cfg = {"H": self._hidden_dim, "n_hidden": int(self._num_edge_MLP_hidden_layers), "flags": self._flags(),
-                       "agg": self._aggregation_fn.code, "path": _ffi.PATH[self._path]}
                 return _GGNNFunction.apply(h, prepared, cfg, *gru, *weights)
-            return self._composed_forward(h, prepared, gru, weights)
-        out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
-        ptrs, _keep = self._mlp_weight_ptrs()
-        _ffi.check(_ffi.lib().tfgnn_b200_ggnn_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, int(self._num_edge_MLP_hidden_layers),
-            self._hidden_dim, self._flags(), self._aggregation_fn.code, self._gru_kernel.value.data_ptr(),
-            self._gru_recurrent_kernel.value.data_ptr(), self._gru_bias.value.data_ptr(),
-            _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
-        return out
+            return self._composed_forward(h, prepared, cfg, gru, weights)
+        return _ggnn_forward(h, prepared, cfg, *gru, weights)
 
     def _ggnn_bwd_takes_it(self) -> bool:
         """The configurations _GGNNFunction trains (tfgnn_b200_ggnn_bwd): linear messages from the source state only,
@@ -135,14 +133,12 @@ class GGNN(GNN_Edge_MLP):
         return (int(self._num_edge_MLP_hidden_layers) == 0 and not self._use_target_state_as_input and H % 4 == 0
                 and (self._aggregation_fn.name != "max" or H <= 512))
 
-    def _composed_forward(self, h: torch.Tensor, prepared: PreparedBatch, gru, weights) -> torch.Tensor:
+    def _composed_forward(self, h: torch.Tensor, prepared: PreparedBatch, cfg, gru, weights) -> torch.Tensor:
         """Every other message MLP under autograd: the messages through GNN_Edge_MLP's own routing without activation
         (GGNN ignores activation-before, as its forward does), then the GRU update.  On the fused message paths this runs
         the kernels of tfgnn_b200_ggnn_fwd in the same order, so training and inference give the same bits."""
         if self._has_fused_backward(int(h.shape[1])):
-            cfg = dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers),
-                       flags=self._flags() & ~_ffi.FLAG_ACT_BEFORE_AGG, agg=self._aggregation_fn.code, act=_ffi.ACT[None],
-                       path=_ffi.PATH[self._path])
+            cfg = dict(cfg, flags=cfg["flags"] & ~_ffi.FLAG_ACT_BEFORE_AGG, act=_ffi.ACT[None])
             agg = _EdgeMLPLayerFunction.apply(h, prepared, cfg, *weights)
         else:
             agg = edge_mlp_family_forward(self, h, prepared, final_activation=False, activation_before=False)

@@ -7,8 +7,18 @@ import torch
 
 from ... import _ffi
 from ...runtime import PreparedBatch, stream_ptr
+from ..node_ops import _needs_grad
 from .message_passing import (MessagePassing, MessagePassingInput, Variable, _last_dim,
                               register_message_passing_implementation)
+
+
+def _edge_mlp_forward(h, prepared: PreparedBatch, cfg, weights) -> torch.Tensor:
+    """tfgnn_b200_edge_mlp_fwd: the layer's output rows [num_nodes, H]."""
+    out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+    _ffi.check(_ffi.lib().tfgnn_b200_edge_mlp_fwd(
+        prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights), cfg["n_hidden"], cfg["H"],
+        cfg["flags"], cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+    return out
 
 
 class _EdgeMLPLayerFunction(torch.autograd.Function):
@@ -18,10 +28,7 @@ class _EdgeMLPLayerFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, h, prepared, cfg, *weights):
-        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
-        _ffi.check(_ffi.lib().tfgnn_b200_edge_mlp_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights), cfg["n_hidden"], cfg["H"],
-            cfg["flags"], cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+        out = _edge_mlp_forward(h, prepared, cfg, weights)
         ctx.prepared, ctx.cfg = prepared, cfg
         ctx.save_for_backward(h, out, *weights)
         return out
@@ -109,9 +116,15 @@ class GNN_Edge_MLP(MessagePassing):
             f |= _ffi.FLAG_USE_TARGET
         return f
 
-    def _mlp_weight_ptrs(self):
-        tensors = [v.value for mlp in self._edge_type_mlps for v in mlp.layers]
-        return _ffi.ptr_array(tensors), tensors
+    def _cfg(self) -> Dict[str, int]:
+        """The layer's arguments of the fused entry points, the same for the training and the inference call."""
+        act = self._activation_fn.code if self._activation_fn is not None else _ffi.ACT[None]
+        return dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers), flags=self._flags(),
+                    agg=self._aggregation_fn.code, act=act, path=_ffi.PATH[self._path])
+
+    def _mlp_weights(self) -> List[torch.Tensor]:
+        """Every edge type's MLP kernels, type by type."""
+        return [v.value for mlp in self._edge_type_mlps for v in mlp.layers]
 
     def _check_types(self, prepared: PreparedBatch):
         if prepared.num_edge_types != len(self._edge_type_mlps):
@@ -122,22 +135,15 @@ class GNN_Edge_MLP(MessagePassing):
              prepared: Optional[PreparedBatch] = None):
         h, prepared = self._device_inputs(inputs, prepared)
         self._check_types(prepared)
-        ptrs, tensors = self._mlp_weight_ptrs()
-        if torch.is_grad_enabled() and (h.requires_grad or any(t.requires_grad for t in tensors)):
+        cfg, weights = self._cfg(), self._mlp_weights()
+        if _needs_grad(h, *weights):
             if not self._has_fused_backward(int(h.shape[1]), self._message_activation_before_aggregation):
                 # two or more hidden layers / one hidden layer with max aggregation or activation before aggregation: the
                 # reference's literal op order with per-op backward kernels (layers/differentiable.py)
                 from ..differentiable import edge_mlp_family_forward
                 return edge_mlp_family_forward(self, h, prepared)
-            cfg = dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers), flags=self._flags(),
-                       agg=self._aggregation_fn.code, act=self._activation_fn.code, path=_ffi.PATH[self._path])
-            return _EdgeMLPLayerFunction.apply(h, prepared, cfg, *tensors)
-        out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
-        _ffi.check(_ffi.lib().tfgnn_b200_edge_mlp_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, int(self._num_edge_MLP_hidden_layers),
-            self._hidden_dim, self._flags(), self._aggregation_fn.code, self._activation_fn.code,
-            _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
-        return out
+            return _EdgeMLPLayerFunction.apply(h, prepared, cfg, *weights)
+        return _edge_mlp_forward(h, prepared, cfg, weights)
 
     def _has_fused_backward(self, D: int, activation_before: bool = False) -> bool:
         """The edge MLPs tfgnn_b200_rgcn_bwd (no hidden layer: every aggregation, the activation before or after it; with
@@ -158,20 +164,19 @@ class GNN_Edge_MLP(MessagePassing):
         (tfgnn_b200_rgcn_ln_fwd): for RGCN-style layers the normalisation happens in the fused kernel's epilogue.  Other
         configurations, and any call that records gradients, compose the two ops."""
         h, prepared = self._device_inputs(inputs, prepared)
-        ptrs, tensors = self._mlp_weight_ptrs()
+        weights = self._mlp_weights()
         fusable = (int(self._num_edge_MLP_hidden_layers) == 0 and not self._use_target_state_as_input
                    and type(self)._compute_is_plain_edge_mlp())
-        if not fusable or (torch.is_grad_enabled() and (h.requires_grad or gamma.requires_grad or beta.requires_grad
-                                                        or any(t.requires_grad for t in tensors))):
+        if not fusable or _needs_grad(h, gamma, beta, *weights):
             from ..node_ops import layer_norm
             return layer_norm(self.call(MessagePassingInput(h, inputs.adjacency_lists), prepared=prepared), gamma, beta,
                               epsilon)
         self._check_types(prepared)
-        out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
+        cfg = self._cfg()
+        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
         _ffi.check(_ffi.lib().tfgnn_b200_rgcn_ln_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, self._hidden_dim, self._flags(), self._aggregation_fn.code,
-            self._activation_fn.code, _ffi.PATH[self._path], gamma.data_ptr(), beta.data_ptr(), float(epsilon),
-            out.data_ptr(), stream_ptr()))
+            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights), cfg["H"], cfg["flags"], cfg["agg"],
+            cfg["act"], cfg["path"], gamma.data_ptr(), beta.data_ptr(), float(epsilon), out.data_ptr(), stream_ptr()))
         return out
 
     @classmethod
@@ -193,10 +198,9 @@ class GNN_Edge_MLP(MessagePassing):
         if int(self._num_edge_MLP_hidden_layers) != 0 or self._use_target_state_as_input:
             raise NotImplementedError("call_allgather needs an RGCN-style layer (no hidden layers, source state only)")
         self._check_types(prepared)
-        _ptrs, tensors = self._mlp_weight_ptrs()
         reps = (c_void_p * len(replica_ptrs))(*[int(p) for p in replica_ptrs])
         _ffi.check(_ffi.lib().tfgnn_b200_rgcn_fwd_allgather(
-            prepared.handle, node_embeddings.data_ptr(), int(node_embeddings.shape[1]), _ffi.ptr_array(tensors),
+            prepared.handle, node_embeddings.data_ptr(), int(node_embeddings.shape[1]), _ffi.ptr_array(self._mlp_weights()),
             self._hidden_dim, self._flags(), self._aggregation_fn.code, self._activation_fn.code, reps, len(replica_ptrs),
             int(own_rank), c_void_p(int(multicast_ptr) or None), stream_ptr()))
 

@@ -14,6 +14,26 @@ from ..node_ops import _needs_grad, dense
 from .message_passing import MessagePassingInput, _last_dim, register_message_passing_implementation
 
 
+def _film_forward(h, prepared: PreparedBatch, cfg, kernels, film) -> torch.Tensor:
+    """tfgnn_b200_film_fwd: the layer's output rows [num_nodes, H]; kernels = the edge MLPs', film = the FiLM kernels."""
+    out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+    _ffi.check(_ffi.lib().tfgnn_b200_film_fwd(
+        prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(kernels), cfg["n_hidden"], _ffi.ptr_array(film),
+        cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+    return out
+
+
+def _film_in_forward(h, film_in, prepared: PreparedBatch, cfg, kernels, film) -> torch.Tensor:
+    """tfgnn_b200_film_in_fwd: as _film_forward with the FiLM input table film_in [V_owned, L*S] and the last FiLM
+    kernels."""
+    out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+    _ffi.check(_ffi.lib().tfgnn_b200_film_in_fwd(
+        prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(kernels), cfg["n_hidden"], film_in.data_ptr(),
+        cfg["S"], _ffi.ptr_array(film), cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(),
+        stream_ptr()))
+    return out
+
+
 class _FilmLayerFunction(torch.autograd.Function):
     """Autograd hook of the FiLM layer without hidden layers: forward = tfgnn_b200_film_fwd, backward =
     tfgnn_b200_film_bwd (aggregate-then-transform, no per-edge tensors).  weights = the L edge-MLP kernels, then the L
@@ -22,10 +42,7 @@ class _FilmLayerFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h, prepared, cfg, *weights):
         L = len(weights) // 2
-        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
-        _ffi.check(_ffi.lib().tfgnn_b200_film_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights[:L]), 0, _ffi.ptr_array(weights[L:]),
-            cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+        out = _film_forward(h, prepared, cfg, weights[:L], weights[L:])
         ctx.prepared, ctx.cfg = prepared, cfg
         ctx.save_for_backward(h, out, *weights)
         return out
@@ -55,11 +72,7 @@ class _FilmInLayerFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h, film_in, prepared, cfg, *weights):
         L = len(weights) // 2
-        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
-        _ffi.check(_ffi.lib().tfgnn_b200_film_in_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights[:L]), 0, film_in.data_ptr(), cfg["S"],
-            _ffi.ptr_array(weights[L:]), cfg["H"], cfg["flags"], cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(),
-            stream_ptr()))
+        out = _film_in_forward(h, film_in, prepared, cfg, weights[:L], weights[L:])
         ctx.prepared, ctx.cfg = prepared, cfg
         ctx.save_for_backward(h, film_in, out, *weights)
         return out
@@ -118,41 +131,27 @@ class GNN_FiLM(GNN_Edge_MLP):
              prepared: Optional[PreparedBatch] = None):
         h, prepared = self._device_inputs(inputs, prepared)
         self._check_types(prepared)
-        act = self._activation_fn.code if self._activation_fn is not None else _ffi.ACT[None]
-        cfg = dict(H=self._hidden_dim, flags=self._flags(), agg=self._aggregation_fn.code, act=act,
-                   path=_ffi.PATH[self._path])
+        cfg, kernels = self._cfg(), self._mlp_weights()
+        film = [m.layers[-1].value for m in self._edge_type_film_layer_computations]
         film_hidden = any(m.num_hidden_layers for m in self._edge_type_film_layer_computations)
         if _needs_grad(h, *[v.value for v in self.variables]):
+            # both fused backwards take edge MLPs without hidden layers: `kernels` holds one kernel per type
             if self._has_fused_backward(int(h.shape[1])):
-                weights = ([m.layers[0].value for m in self._edge_type_mlps]
-                           + [m.layers[0].value for m in self._edge_type_film_layer_computations])
-                return _FilmLayerFunction.apply(h, prepared, cfg, *weights)
+                return _FilmLayerFunction.apply(h, prepared, cfg, *kernels, *film)
             if film_hidden and self._has_fused_film_mlp_backward(int(h.shape[1]), prepared):
                 film_in = self._film_inputs(h, prepared)
-                weights = ([m.layers[0].value for m in self._edge_type_mlps]
-                           + [m.layers[-1].value for m in self._edge_type_film_layer_computations])
-                return _FilmInLayerFunction.apply(h, film_in, prepared, dict(cfg, S=self._film_input_width()), *weights)
+                return _FilmInLayerFunction.apply(h, film_in, prepared, dict(cfg, S=self._film_input_width()), *kernels,
+                                                  *film)
             # edge-MLP hidden layers / max aggregation / activation before aggregation / widths that are not multiples of
             # 4 / target-range shards: the reference's literal op order with per-op backward kernels
             # (layers/differentiable.py)
             return edge_mlp_family_forward(
                 self, h, prepared,
                 film_kernels=[[v.value for v in m.layers] for m in self._edge_type_film_layer_computations])
-        out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
-        ptrs, _keep = self._mlp_weight_ptrs()
-        film = [m.layers[-1].value for m in self._edge_type_film_layer_computations]
         if film_hidden:
             film_in = self._film_inputs(h, prepared)
-            _ffi.check(_ffi.lib().tfgnn_b200_film_in_fwd(
-                prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, int(self._num_edge_MLP_hidden_layers),
-                film_in.data_ptr(), self._film_input_width(), _ffi.ptr_array(film), self._hidden_dim, self._flags(),
-                cfg["agg"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
-            return out
-        _ffi.check(_ffi.lib().tfgnn_b200_film_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, int(self._num_edge_MLP_hidden_layers),
-            _ffi.ptr_array(film), self._hidden_dim, self._flags(), self._aggregation_fn.code,
-            self._activation_fn.code, _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
-        return out
+            return _film_in_forward(h, film_in, prepared, dict(cfg, S=self._film_input_width()), kernels, film)
+        return _film_forward(h, prepared, cfg, kernels, film)
 
     def _film_input_width(self) -> int:
         """S: the width of the last hidden FiLM-MLP layer (the same for every type)."""

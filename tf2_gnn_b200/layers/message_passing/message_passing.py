@@ -18,8 +18,7 @@ from typing import Any, Dict, List, NamedTuple, Optional, Sequence, Tuple
 import torch
 
 from ... import _ffi
-from ...runtime import (PreparedBatch, prepared_batch_for, require_cuda, stream_ptr, to_device_adj,
-                        to_device_f32)
+from ...runtime import PreparedBatch, prepared_batch_for, require_cuda, to_device_adj, to_device_f32
 from ...utils.param_helpers import get_activation_function, get_aggregation_function
 
 
@@ -206,23 +205,14 @@ class MessagePassing:
 
     def _calculate_messages_per_type(self, prepared: PreparedBatch, node_embeddings, training=False):
         """message_passing.py:181-218."""
-        lib = _ffi.lib()
-        V, D = int(node_embeddings.shape[0]), int(node_embeddings.shape[1])
+        from ..node_ops import gather_rows
+        V = int(node_embeddings.shape[0])
         type_to_num_incoming_edges = prepared.in_degree()  # [L, V]
         messages_per_type = []
         for edge_type_idx, adj in enumerate(prepared.adjacency_lists):
-            E = int(adj.shape[0])
-            src_states = torch.empty((E, D), dtype=torch.float32, device=node_embeddings.device)
-            tgt_states = torch.empty((E, D), dtype=torch.float32, device=node_embeddings.device)
-            n_in = torch.empty((E,), dtype=torch.float32, device=node_embeddings.device)
-            if E:
-                base = adj.data_ptr()
-                _ffi.check(lib.tfgnn_b200_gather_rows(node_embeddings.data_ptr(), V, D, base, 2, E,
-                                                      src_states.data_ptr(), stream_ptr()))
-                _ffi.check(lib.tfgnn_b200_gather_rows(node_embeddings.data_ptr(), V, D, base + 4, 2, E,
-                                                      tgt_states.data_ptr(), stream_ptr()))
-                _ffi.check(lib.tfgnn_b200_gather_rows(type_to_num_incoming_edges[edge_type_idx].data_ptr(), V, 1,
-                                                      base + 4, 2, E, n_in.data_ptr(), stream_ptr()))
+            src_states = gather_rows(node_embeddings, adj, 0)
+            tgt_states = gather_rows(node_embeddings, adj, 1)
+            n_in = gather_rows(type_to_num_incoming_edges[edge_type_idx].reshape(V, 1), adj, 1).reshape(-1)
             messages_per_type.append(
                 self._message_function(src_states, tgt_states, n_in, edge_type_idx, training))
         return messages_per_type

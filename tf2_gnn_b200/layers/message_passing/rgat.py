@@ -12,6 +12,15 @@ from .message_passing import (MessagePassing, MessagePassingInput, Variable, _la
                               register_message_passing_implementation)
 
 
+def _rgat_forward(h, prepared: PreparedBatch, cfg, kernels, attention) -> torch.Tensor:
+    """tfgnn_b200_rgat_fwd: the layer's output rows [num_nodes, H]."""
+    out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+    _ffi.check(_ffi.lib().tfgnn_b200_rgat_fwd(
+        prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(kernels), _ffi.ptr_array(attention),
+        cfg["H"], cfg["K"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+    return out
+
+
 class _RgatLayerFunction(torch.autograd.Function):
     """Autograd hook of the RGAT layer: forward = tfgnn_b200_rgat_fwd (so training output equals inference output),
     backward = tfgnn_b200_rgat_bwd (no per-edge tensors, no float atomics).  weights = the L projection kernels, then the L
@@ -20,10 +29,7 @@ class _RgatLayerFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h, prepared, cfg, *weights):
         L = len(weights) // 2
-        out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
-        _ffi.check(_ffi.lib().tfgnn_b200_rgat_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights[:L]), _ffi.ptr_array(weights[L:]),
-            cfg["H"], cfg["K"], cfg["act"], cfg["path"], out.data_ptr(), stream_ptr()))
+        out = _rgat_forward(h, prepared, cfg, weights[:L], weights[L:])
         ctx.prepared, ctx.cfg = prepared, cfg
         ctx.save_for_backward(h, out, *weights)
         return out
@@ -77,26 +83,21 @@ class RGAT(MessagePassing):
     def call(self, inputs: MessagePassingInput, training: bool = False,
              prepared: Optional[PreparedBatch] = None):
         h, prepared = self._device_inputs(inputs, prepared)
+        self._check_shape(prepared)
+        kernels = [v.value for v in self._edge_type_to_message_computation_layer]
+        attention = [v.value for v in self._edge_type_to_attention_parameters]
         if _needs_grad(h, *[v.value for v in self.variables]):
             if self._has_fused_backward(int(h.shape[1])):
-                self._check_shape(prepared)
-                act = self._activation_fn.code if self._activation_fn is not None else _ffi.ACT[None]
-                cfg = dict(H=self._hidden_dim, K=int(self._num_heads), act=act, path=_ffi.PATH[self._path])
-                weights = ([v.value for v in self._edge_type_to_message_computation_layer]
-                           + [v.value for v in self._edge_type_to_attention_parameters])
-                return _RgatLayerFunction.apply(h, prepared, cfg, *weights)
+                return _RgatLayerFunction.apply(h, prepared, self._cfg(), *kernels, *attention)
             # other shapes: the reference's literal op order with per-op backward kernels (layers/differentiable.py)
             from ..differentiable import rgat_forward
             return rgat_forward(self, h, prepared)
-        self._check_shape(prepared)
-        out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
-        kernels = [v.value for v in self._edge_type_to_message_computation_layer]
-        att = [v.value for v in self._edge_type_to_attention_parameters]
-        _ffi.check(_ffi.lib().tfgnn_b200_rgat_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(kernels), _ffi.ptr_array(att),
-            self._hidden_dim, int(self._num_heads), self._activation_fn.code, _ffi.PATH[self._path],
-            out.data_ptr(), stream_ptr()))
-        return out
+        return _rgat_forward(h, prepared, self._cfg(), kernels, attention)
+
+    def _cfg(self) -> Dict[str, int]:
+        """The layer's arguments of tfgnn_b200_rgat_fwd / _bwd, the same for the training and the inference call."""
+        act = self._activation_fn.code if self._activation_fn is not None else _ffi.ACT[None]
+        return dict(H=self._hidden_dim, K=int(self._num_heads), act=act, path=_ffi.PATH[self._path])
 
     def _check_shape(self, prepared: PreparedBatch) -> None:
         if prepared.num_edge_types != len(self._edge_type_to_message_computation_layer):

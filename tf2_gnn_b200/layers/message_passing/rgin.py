@@ -14,6 +14,15 @@ from ..node_ops import _needs_grad, dense
 from .message_passing import MessagePassingInput, Variable, register_message_passing_implementation
 
 
+def _rgin_forward(h, prepared: PreparedBatch, cfg, weights, aggr) -> torch.Tensor:
+    """tfgnn_b200_rgin_fwd: the layer's output rows [num_nodes, H]; `aggr` = the aggregation MLP's kernels."""
+    out = torch.empty((prepared.num_nodes, cfg["H"]), dtype=torch.float32, device=h.device)
+    _ffi.check(_ffi.lib().tfgnn_b200_rgin_fwd(
+        prepared.handle, h.data_ptr(), int(h.shape[1]), _ffi.ptr_array(weights), cfg["n_hidden"], cfg["H"],
+        cfg["flags"], cfg["agg"], cfg["act"], _ffi.ptr_array(aggr), len(aggr), cfg["path"], out.data_ptr(), stream_ptr()))
+    return out
+
+
 @register_message_passing_implementation
 class RGIN(GNN_Edge_MLP):
     """h'_v = sigma(MLP_aggr(sum_l sum_{(u,v) in A_l} MLP_l(h_u)))  (rgin.py:14-59)."""
@@ -48,33 +57,22 @@ class RGIN(GNN_Edge_MLP):
              prepared: Optional[PreparedBatch] = None):
         h, prepared = self._device_inputs(inputs, prepared)
         self._check_types(prepared)
+        cfg, weights = self._cfg(), self._mlp_weights()
+        aggr = [v.value for v in (self._aggregation_mlp or [])]
         if _needs_grad(h, *[v.value for v in self.variables]):
             if self._has_fused_backward(int(h.shape[1])):
                 # the inference forward's op sequence, each op with its fused backward: edge MLP (activation-before is
                 # ignored, rgin.py:88-106), then the aggregation MLP and the activation
-                aggr = [v.value for v in (self._aggregation_mlp or [])]
-                act = self._activation_fn.code if (self._activation_fn is not None and not aggr) else _ffi.ACT[None]
-                cfg = dict(H=self._hidden_dim, n_hidden=int(self._num_edge_MLP_hidden_layers),
-                           flags=self._flags() & ~_ffi.FLAG_ACT_BEFORE_AGG, agg=self._aggregation_fn.code, act=act,
-                           path=_ffi.PATH[self._path])
-                out = _EdgeMLPLayerFunction.apply(h, prepared, cfg, *self._mlp_weight_ptrs()[1])
+                cfg = dict(cfg, flags=cfg["flags"] & ~_ffi.FLAG_ACT_BEFORE_AGG, act=_ffi.ACT[None] if aggr else cfg["act"])
+                out = _EdgeMLPLayerFunction.apply(h, prepared, cfg, *weights)
                 relu = get_activation_function("relu")
                 for i, W in enumerate(aggr):
                     out = dense(out, W, None, self._activation_fn if i == len(aggr) - 1 else relu)
                 return out
             # two or more hidden layers / one hidden layer with max aggregation: the reference's literal op order with
             # per-op backward kernels (layers/differentiable.py)
-            return edge_mlp_family_forward(
-                self, h, prepared, activation_before=False,
-                aggr_kernels=[v.value for v in self._aggregation_mlp] if self._aggregation_mlp is not None else None)
-        out = torch.empty((prepared.num_nodes, self._hidden_dim), dtype=torch.float32, device=h.device)
-        ptrs, _keep = self._mlp_weight_ptrs()
-        aggr = [v.value for v in (self._aggregation_mlp or [])]
-        _ffi.check(_ffi.lib().tfgnn_b200_rgin_fwd(
-            prepared.handle, h.data_ptr(), int(h.shape[1]), ptrs, int(self._num_edge_MLP_hidden_layers),
-            self._hidden_dim, self._flags(), self._aggregation_fn.code, self._activation_fn.code,
-            _ffi.ptr_array(aggr), len(aggr), _ffi.PATH[self._path], out.data_ptr(), stream_ptr()))
-        return out
+            return edge_mlp_family_forward(self, h, prepared, activation_before=False, aggr_kernels=aggr or None)
+        return _rgin_forward(h, prepared, cfg, weights, aggr)
 
     def set_weights_from_oracle_dict(self, w: Dict[str, Any]) -> None:
         super().set_weights_from_oracle_dict(w)

@@ -229,7 +229,39 @@ def dropout(x: torch.Tensor, rate: float, state: Optional[DropoutState] = None, 
     return _dropout_apply(x, float(rate), state.seed, offset, first)
 
 
+# ---- gather / segment sum by int32 ids (forward only) -------------------------------------------------------------
+def _id_column(ids: torch.Tensor, column: int):
+    """(pointer, stride) of the ids: a contiguous int32 vector, or column `column` of a contiguous [E, 2] adjacency list."""
+    return ids.data_ptr() + 4 * column, (2 if ids.dim() == 2 else 1)
+
+
+def gather_rows(table: torch.Tensor, ids: torch.Tensor, column: int = 0) -> torch.Tensor:
+    """table[ids] (ids as in _id_column)."""
+    n, C = int(ids.shape[0]), int(table.shape[1])
+    out = torch.empty((n, C), dtype=torch.float32, device=table.device)
+    if n:
+        _ffi.check(_ffi.lib().tfgnn_b200_gather_rows(table.data_ptr(), int(table.shape[0]), C, *_id_column(ids, column), n,
+                                                     out.data_ptr(), stream_ptr()))
+    return out
+
+
+def segment_sum(data: torch.Tensor, ids: torch.Tensor, num_segments: int, column: int = 0) -> torch.Tensor:
+    """tf.math.unsorted_segment_sum(data, ids, num_segments), the adjoint of gather_rows (ids as in _id_column)."""
+    out = torch.empty((num_segments, int(data.shape[1])), dtype=torch.float32, device=data.device)
+    _ffi.check(_ffi.lib().tfgnn_b200_unsorted_segment_reduce(data.data_ptr(), *_id_column(ids, column), int(data.shape[0]),
+                                                             int(data.shape[1]), num_segments, _ffi.AGG["sum"],
+                                                             out.data_ptr(), stream_ptr()))
+    return out
+
+
 # ---- graph-level primitives (forward only) ----------------------------------------------------------------------
+def node_to_graph_index(node_to_graph_map, device: torch.device) -> torch.Tensor:
+    """node_to_graph_map as a contiguous int32 tensor on `device`."""
+    if not isinstance(node_to_graph_map, torch.Tensor):
+        node_to_graph_map = torch.as_tensor(node_to_graph_map)
+    return node_to_graph_map.to(device=device, dtype=torch.int32).contiguous()
+
+
 def graph_offsets(node_to_graph_map: torch.Tensor, num_graphs: int, validate: bool = False) -> torch.Tensor:
     V = int(node_to_graph_map.shape[0])
     out = torch.empty(int(num_graphs) + 1, dtype=torch.int32, device=node_to_graph_map.device)
@@ -245,6 +277,23 @@ def segment_softmax(scores: torch.Tensor, graph_ptr: torch.Tensor) -> torch.Tens
     _ffi.check(_ffi.lib().tfgnn_b200_segment_softmax(scores.data_ptr(), graph_ptr.data_ptr(), int(graph_ptr.shape[0]) - 1,
                                                      int(scores.shape[1]), out.data_ptr(), stream_ptr()))
     return out
+
+
+def sigmoid(x: torch.Tensor) -> torch.Tensor:
+    """tf.nn.sigmoid on the library's activation kernel."""
+    out = torch.empty_like(x)
+    _ffi.check(_ffi.lib().tfgnn_b200_activation(x.data_ptr(), x.numel(), _ffi.ACT_SIGMOID, out.data_ptr(), stream_ptr()))
+    return out
+
+
+def readout_weights(scores: Optional[torch.Tensor], graph_ptr: torch.Tensor, weighting_fun: str) -> Optional[torch.Tensor]:
+    """The per-(node, head) weights of the graph readout (nodes_to_graph_representation.py:174-186): None for "none" and
+    "average"."""
+    if weighting_fun == "softmax":
+        return segment_softmax(scores, graph_ptr)
+    if weighting_fun == "sigmoid":
+        return sigmoid(scores)
+    return None
 
 
 def weighted_segment_sum(node_reprs: torch.Tensor, weights: Optional[torch.Tensor], graph_ptr: torch.Tensor,
@@ -270,20 +319,29 @@ def gathered_add(a: torch.Tensor, b: torch.Tensor, index: Optional[torch.Tensor]
     return out
 
 
+def gru_gate_inputs(inputs: torch.Tensor, state: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor,
+                    bias: torch.Tensor):
+    """The two Dense halves of a Keras GRUCell(reset_after=True): gx = inputs K + b0, gh = state U + b1."""
+    return dense(inputs, kernel, bias[0]), dense(state, recurrent_kernel, bias[1])
+
+
+def gru_gate_fwd(gx: torch.Tensor, gx_row_index: Optional[torch.Tensor], gh: torch.Tensor,
+                 state: torch.Tensor) -> torch.Tensor:
+    """The GRUCell gate math on gx[gx_row_index[v]] (gx[v] without an index), gh[v] and state[v]."""
+    out = torch.empty_like(state)
+    _ffi.check(_ffi.lib().tfgnn_b200_gru_gate_fwd(gx.data_ptr(), _ptr(gx_row_index), gh.data_ptr(), state.data_ptr(),
+                                                  int(state.shape[0]), int(state.shape[1]), out.data_ptr(), stream_ptr()))
+    return out
+
+
 def gru_cell(inputs: torch.Tensor, inputs_row_index: Optional[torch.Tensor], state: torch.Tensor, kernel: torch.Tensor,
              recurrent_kernel: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
     """tf.keras.layers.GRUCell(units=H) (TF2 defaults: reset_after=True, bias [2,3H], gates z|r|h) applied to
     inputs[inputs_row_index[v]] with state[v].  The input half (inputs K + b0) is computed once per row of `inputs`
     (e.g. once per GRAPH for the global exchange) and picked up per node inside the gate kernel."""
     require_no_grad("gru_cell", inputs, state, kernel, recurrent_kernel, bias)
-    H = int(state.shape[1])
-    gx = dense(inputs, kernel, bias[0])
-    gh = dense(state, recurrent_kernel, bias[1])
-    state = state.contiguous()
-    out = torch.empty_like(state)
-    _ffi.check(_ffi.lib().tfgnn_b200_gru_gate_fwd(gx.data_ptr(), _ptr(inputs_row_index), gh.data_ptr(), state.data_ptr(),
-                                                  int(state.shape[0]), H, out.data_ptr(), stream_ptr()))
-    return out
+    gx, gh = gru_gate_inputs(inputs, state, kernel, recurrent_kernel, bias)
+    return gru_gate_fwd(gx, inputs_row_index, gh, state.contiguous())
 
 
 def clamp_(x: torch.Tensor, lower: Optional[float], upper: Optional[float]) -> torch.Tensor:

@@ -123,10 +123,7 @@ class WeightedSumGraphRepresentation(NodesToGraphRepresentation):
         if shard is not None:
             return self._call_shard(inputs, training, graph_ptr, shard)
         x = to_device_f32(inputs.node_embeddings)
-        n2g = inputs.node_to_graph_map
-        if not isinstance(n2g, torch.Tensor):
-            n2g = torch.as_tensor(n2g)
-        n2g = n2g.to(device=x.device, dtype=torch.int32).contiguous()
+        n2g = node_ops.node_to_graph_index(inputs.node_to_graph_map, x.device)
         num_graphs = int(inputs.num_graphs)
         if graph_ptr is None:
             graph_ptr = node_ops.graph_offsets(n2g, num_graphs)
@@ -139,11 +136,7 @@ class WeightedSumGraphRepresentation(NodesToGraphRepresentation):
         if node_ops._needs_grad(scores, reprs):
             # same forward kernels as below; backward on the graphs' row ranges (graph_autograd.py)
             return graph_autograd.readout(scores, reprs, n2g, graph_ptr, self._num_heads, self._weighting_fun, lower, upper)
-        weights = None
-        if self._weighting_fun == "sigmoid":
-            weights = _sigmoid(scores)
-        elif self._weighting_fun == "softmax":
-            weights = node_ops.segment_softmax(scores, graph_ptr)
+        weights = node_ops.readout_weights(scores, graph_ptr, self._weighting_fun)
         node_ops.clamp_(reprs, lower, upper)
         return node_ops.weighted_segment_sum(reprs, weights, graph_ptr, self._num_heads,      # (3) aggregate by graph
                                              mean=self._weighting_fun == "average")
@@ -152,10 +145,7 @@ class WeightedSumGraphRepresentation(NodesToGraphRepresentation):
         if self._weighting_fun == "average":
             raise NotImplementedError("WeightedSumGraphRepresentation: average weighting is not built for target-range shards")
         x = to_device_f32(inputs.node_embeddings)
-        n2g = inputs.node_to_graph_map
-        if not isinstance(n2g, torch.Tensor):
-            n2g = torch.as_tensor(n2g)
-        n2g = n2g.to(device=x.device, dtype=torch.int32).contiguous()
+        n2g = node_ops.node_to_graph_index(inputs.node_to_graph_map, x.device)
         if int(x.shape[0]) != shard.hi - shard.lo or int(n2g.shape[0]) != shard.hi - shard.lo:
             raise ValueError(f"a shard's node_embeddings and node_to_graph_map hold its {shard.hi - shard.lo} rows, got "
                              f"{int(x.shape[0])} and {int(n2g.shape[0])}")
@@ -218,12 +208,3 @@ class WASGraphRepresentation(NodesToGraphRepresentation):
         avg_graph_repr = self._weighted_avg_graph_repr_layer.call(inputs, training=training)
         sum_graph_repr = self._weighted_sum_graph_repr_layer.call(inputs, training=training)
         return node_ops.dense(torch.cat([avg_graph_repr, sum_graph_repr], dim=-1), self._out_projection.value)
-
-
-def _sigmoid(x: torch.Tensor) -> torch.Tensor:
-    """tf.nn.sigmoid on the library's activation kernel."""
-    from .. import _ffi
-    from ..runtime import stream_ptr
-    out = torch.empty_like(x)
-    _ffi.check(_ffi.lib().tfgnn_b200_activation(x.data_ptr(), x.numel(), _ffi.ACT_SIGMOID, out.data_ptr(), stream_ptr()))
-    return out
